@@ -582,11 +582,16 @@ cudaError_t launch_huf_decode(const BatchGeom& g, void* dst, const void* cbuf, c
 {
     static SmemOptIn optinA, optinB;
     // Table rows per CTA.  Pass A: 306 rows + the 8 KB output staging -> 55.5 KB -> FOUR CTAs (256 blocks) per SM; pass B, for the
-    // blocks whose tables need more (wide, flat alphabets): 808 rows, no staging -> two CTAs per SM.  FSEB200_HUFD_ROWS / _ROWS_B override.
-    static u32 const rowsA = [] { const char* e = std::getenv("FSEB200_HUFD_ROWS"); u32 v = e ? (u32)std::atoi(e) : 306u; return v < hufd::MIN_ROWS ? hufd::MIN_ROWS : v > 1700u ? 1700u : v; }();
-    static u32 const rowsB = [] { const char* e = std::getenv("FSEB200_HUFD_ROWS_B"); u32 v = e ? (u32)std::atoi(e) : 808u; return v > 1700u ? 1700u : v; }();   // 0 = single pass
+    // blocks whose tables need more (wide, flat alphabets): 808 rows, no staging -> two CTAs per SM.  FSEB200_HUFD_ROWS / _ROWS_B override;
+    // each is clamped to what the device's per-block shared-memory opt-in limit holds for its pass (pass A with the staging).
+    static u32 const reqA = [] { const char* e = std::getenv("FSEB200_HUFD_ROWS"); return e ? (u32)std::atoi(e) : 306u; }();
+    static u32 const reqB = [] { const char* e = std::getenv("FSEB200_HUFD_ROWS_B"); return e ? (u32)std::atoi(e) : 808u; }();   // 0 = single pass
     if (g.nBlocks == 0) return cudaSuccess;
     int const dev = current_device();
+    u32 const optin = (u32)device_smem_optin(dev);
+    auto fit = [optin](bool staged) { u32 const fixed = hufd::smem_bytes(0, staged); return optin > fixed ? (optin - fixed) / (hufd::G * 2) : 0u; };
+    u32 const rowsA = max(hufd::MIN_ROWS, min(reqA, fit(true)));     // below MIN_ROWS the opt-in below fails and the call reports it
+    u32 const rowsB = min(reqB, fit(false));
     size_t const smemA = hufd::smem_bytes(rowsA, true);
     bool const twoPass = rowsB > rowsA;
     cudaError_t e = optinA.ensure(hufd::huf_decode_kernel<true>, dev, (int)smemA);

@@ -30,6 +30,19 @@ inline int device_sm_count(int dev)
     return sms[dev];
 }
 
+// Largest dynamic shared memory one block may opt in to (0 if the device cannot say).
+inline int device_smem_optin(int dev)
+{
+    static int bytes[MAX_DEVICES];
+    static std::once_flag once[MAX_DEVICES];
+    std::call_once(once[dev], [dev] {
+        int n = 0;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess || n < 0) n = 0;
+        bytes[dev] = n;
+    });
+    return bytes[dev];
+}
+
 // One instance per kernel (function-local static in its launcher): remembers on which devices the kernel's
 // dynamic shared-memory limit was already raised.
 struct SmemOptIn {

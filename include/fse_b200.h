@@ -42,6 +42,11 @@ extern "C" {
  * All pointers are device pointers; `stream` is a cudaStream_t (NULL = default stream).
  * The compressed buffer must be readable for 32 bytes past the last block's compressed bytes (the decoders load aligned 16- / 32-byte
  * pieces; what lies beyond a block's own bytes is never interpreted) -- bench.c's own buffer of nbChunks * FSE_compressBound() has it.
+ * Alignment and stride: for the byte codecs (HUF, FSE) dSrc, dCBuf and dDst may have any byte alignment and `slot` any value,
+ * odd or below FSE_compressBound(blockSize) (a block that does not fit its slot gets the reference's verdict for that
+ * dstCapacity); buffers may straddle a 4 GiB address boundary.  FSE-U16 holds unsigned shorts: dSrc and dDst must be 2-byte
+ * aligned and blockSize even; its dCBuf and `slot` are tested at even values.  The test-suite checks offsets 0, 1 (U16: 2),
+ * 4, 8, 16, 32, 64 and 96 from a 512-byte aligned start, odd, 128-multiple and below-bound strides, and views across 2^32.
  * Return value: 0, or an error code if the launch itself could not be made.
  * ------------------------------------------------------------------------------------------------ */
 size_t FSEB200_HUF_compress_batch(void* dCBuf, size_t slot, size_t* dCSizes, const void* dSrc, size_t srcTotal,

@@ -7,6 +7,8 @@ import random
 
 import pytest
 
+from paths import split_candidates, table_rows
+
 
 def random_code_lengths(rng, nsym, max_len=12):
     """a complete prefix code with nsym leaves, no code longer than max_len: split random leaves of a one-leaf tree"""
@@ -44,11 +46,7 @@ def test_unified_table_rows_decode_like_the_full_table(seed):
             acc += sum(1 for n in lengths if tl + 1 - n == w) << (w - 1)
             rank_end[w] = acc
         best = 1 << tl
-        for m in range(min(10, tl - 1), 3, -1):             # the kernel's candidates: first level of m bits, 4 <= m < tableLog
-            g = 1 << (tl - m)
-            t = rank_end[tl - m]                            # windows that start a code longer than m bits
-            cut = (t + g - 1) & ~(g - 1)
-            rows = cut + (1 << m) - (cut >> (tl - m))
+        for m, cut, rows in split_candidates(rank_end, tl):   # the kernel's candidates: first level of m bits, 4 <= m < tableLog
             best = min(best, rows)
             d = cut - (cut >> (tl - m))
             table = [full[r] if r < cut else full[(r - d) << (tl - m)] for r in range(rows)]
@@ -56,4 +54,4 @@ def test_unified_table_rows_decode_like_the_full_table(seed):
                 row = min(x - d, x >> (tl - m)) + d         # the kernel's signed minimum
                 assert row == min(x, d + (x >> (tl - m))) and 0 <= row < rows
                 assert table[row] == full[x], (nsym, m, x)
-        assert best <= 1 << tl
+        assert best <= 1 << tl and table_rows(rank_end, tl)[0] == best
