@@ -74,33 +74,39 @@ __device__ __forceinline__ u8 fse_dec_step(u32& state, BitSrc& b, const u32* cel
     return (u8)(cell >> 16);
 }
 
+// The 2-state loops of FSE_decompress_usingDTable_generic (fse_decompress.c:206-235), from output position op with states
+// s1, s2 onwards: returns the decoded size or the reference's verdict.  step(state) decodes one symbol through the caller's
+// table layout and advances that state and b.
+template <typename Step>
+__device__ __forceinline__ u64 d_fse_decode_2state(u8* out, long long op, long long omax, u32 s1, u32 s2, BitSrc& b, Step step)
+{
+    for (; (bs_refill(b) == SRC_MORE) & (op < omax - 3); op += 4) {
+        out[op] = (u8)step(s1);
+        out[op + 1] = (u8)step(s2);
+        out[op + 2] = (u8)step(s1);
+        out[op + 3] = (u8)step(s2);
+    }
+    for (;;) {
+        if (op > omax - 2) return err(E_DST_TOO_SMALL);
+        out[op++] = (u8)step(s1);
+        if (bs_refill(b) == SRC_OVER) { out[op++] = (u8)step(s2); return (u64)op; }
+        if (op > omax - 2) return err(E_DST_TOO_SMALL);
+        out[op++] = (u8)step(s2);
+        if (bs_refill(b) == SRC_OVER) { out[op++] = (u8)step(s1); return (u64)op; }
+    }
+}
+
 // Exact single-lane 2-state decoder (byte symbols).  dt = {tableLog | fastMode<<16, cells...}.
 __device__ inline u64 d_fse_decode_serial(u8* out, u64 cap, const u8* cSrc, u64 cSize, const u32* dt)
 {
     unsigned const tl = dt[0] & 0xFFFF;
     bool const fast = (dt[0] >> 16) != 0;
     const u32* const cells = dt + 1;
-    long long const omax = (long long)cap;
-    long long op = 0;
     BitSrc b;
     {   u64 const e = bs_open(b, cSrc, cSize); if (is_err(e)) return e; }
-    u32 s1 = (u32)bs_read(b, tl); bs_refill(b);
-    u32 s2 = (u32)bs_read(b, tl); bs_refill(b);
-    for (; (bs_refill(b) == SRC_MORE) & (op < omax - 3); op += 4) {
-        out[op] = fse_dec_step(s1, b, cells, fast);
-        out[op + 1] = fse_dec_step(s2, b, cells, fast);
-        out[op + 2] = fse_dec_step(s1, b, cells, fast);
-        out[op + 3] = fse_dec_step(s2, b, cells, fast);
-    }
-    for (;;) {
-        if (op > omax - 2) return err(E_DST_TOO_SMALL);
-        out[op++] = fse_dec_step(s1, b, cells, fast);
-        if (bs_refill(b) == SRC_OVER) { out[op++] = fse_dec_step(s2, b, cells, fast); break; }
-        if (op > omax - 2) return err(E_DST_TOO_SMALL);
-        out[op++] = fse_dec_step(s2, b, cells, fast);
-        if (bs_refill(b) == SRC_OVER) { out[op++] = fse_dec_step(s1, b, cells, fast); break; }
-    }
-    return (u64)op;
+    u32 const s1 = (u32)bs_read(b, tl); bs_refill(b);
+    u32 const s2 = (u32)bs_read(b, tl); bs_refill(b);
+    return d_fse_decode_2state(out, 0, (long long)cap, s1, s2, b, [&](u32& s) { return fse_dec_step(s, b, cells, fast); });
 }
 
 }  // namespace fseb

@@ -381,7 +381,7 @@ FSEB_API size_t FSE_normalizeCount(short* norm, unsigned tl, const unsigned* cou
     if (msv > 4095) return (size_t)err(E_MSV_TOO_LARGE);
     Micro m; m.up(0, count, (msv + 1) * sizeof(unsigned));
     u64 const r = m.run(MOP_NORMALIZE, tl, total, msv);
-    if (!is_err(r)) m.down(norm, 4096, (msv + 1) * sizeof(short));
+    if (!is_err(r)) m.down(norm, MICRO_OUT, (msv + 1) * sizeof(short));
     return (size_t)r;
 }
 FSEB_API size_t FSE_writeNCount(void* buffer, size_t bufferSize, const short* norm, unsigned msv, unsigned tl)     // lib/fse.h:157
@@ -390,7 +390,7 @@ FSEB_API size_t FSE_writeNCount(void* buffer, size_t bufferSize, const short* no
     Micro m; m.up(0, norm, (msv + 1) * sizeof(short));
     size_t const cap = bufferSize > 60000 ? 60000 : bufferSize;
     u64 const r = m.run(MOP_WRITE_NCOUNT, cap, msv, tl);
-    if (!is_err(r)) m.down(buffer, 4096, (size_t)r);
+    if (!is_err(r)) m.down(buffer, MICRO_OUT, (size_t)r);
     return (size_t)r;
 }
 FSEB_API size_t FSE_readNCount(short* norm, unsigned* msvPtr, unsigned* tlPtr, const void* hdr, size_t hbSize)     // lib/fse.h:227
@@ -402,10 +402,10 @@ FSEB_API size_t FSE_readNCount(short* norm, unsigned* msvPtr, unsigned* tlPtr, c
     u64 const r = m.run(MOP_READ_NCOUNT, take, *msvPtr);
     unsigned const declared = *msvPtr;
     unsigned meta[2] = { 0, 0 };
-    m.down(meta, 8192, sizeof(meta));
+    m.down(meta, MICRO_META, sizeof(meta));
     *tlPtr = meta[1];
-    if (is_err(r)) { m.down(norm, 4096, (declared + 1) * sizeof(short)); return (size_t)r; }
-    m.down(norm, 4096, (declared + 1) * sizeof(short));
+    if (is_err(r)) { m.down(norm, MICRO_OUT, (declared + 1) * sizeof(short)); return (size_t)r; }
+    m.down(norm, MICRO_OUT, (declared + 1) * sizeof(short));
     *msvPtr = meta[0];
     return (size_t)r;
 }
@@ -414,7 +414,7 @@ FSEB_API size_t FSE_buildCTable(unsigned* ct, const short* norm, unsigned msv, u
     if (msv > FSE_MAX_SV) return (size_t)err(E_MSV_TOO_LARGE);
     Micro m; m.up(0, norm, (msv + 1) * sizeof(short));
     u64 const r = m.run(MOP_BUILD_CTABLE, msv, tl);
-    if (!is_err(r)) m.down(ct, 4096, (1 + (tl ? ((size_t)1 << (tl - 1)) : 1) + ((size_t)msv + 1) * 2) * sizeof(unsigned));
+    if (!is_err(r)) m.down(ct, MICRO_OUT, (1 + (tl ? ((size_t)1 << (tl - 1)) : 1) + ((size_t)msv + 1) * 2) * sizeof(unsigned));
     return (size_t)r;
 }
 FSEB_API size_t FSE_buildDTable(unsigned* dt, const short* norm, unsigned msv, unsigned tl)                          // lib/fse.h:240
@@ -423,7 +423,7 @@ FSEB_API size_t FSE_buildDTable(unsigned* dt, const short* norm, unsigned msv, u
     if (tl > FSE_MAX_TLOG) return (size_t)err(E_TLOG_TOO_LARGE);
     Micro m; m.up(0, norm, (msv + 1) * sizeof(short));
     u64 const r = m.run(MOP_BUILD_DTABLE, msv, tl, 0);
-    if (!is_err(r)) m.down(dt, 4096, (1 + ((size_t)1 << tl)) * sizeof(unsigned));
+    if (!is_err(r)) m.down(dt, MICRO_OUT, (1 + ((size_t)1 << tl)) * sizeof(unsigned));
     return (size_t)r;
 }
 FSEB_API size_t HUF_buildCTable(unsigned* ctable, const unsigned* count, unsigned msv, unsigned maxNbBits)            // lib/huf.h:188
@@ -433,7 +433,7 @@ FSEB_API size_t HUF_buildCTable(unsigned* ctable, const unsigned* count, unsigne
     std::memcpy(cnt, count, (msv + 1) * sizeof(unsigned));             // CTable and count may overlap (huf.h:188 note)
     Micro m; m.up(0, cnt, (msv + 1) * sizeof(unsigned));
     u64 const r = m.run(MOP_HUF_BUILD_CTABLE, msv, maxNbBits);
-    if (!is_err(r)) m.down(ctable, 4096, (msv + 1) * sizeof(unsigned));
+    if (!is_err(r)) m.down(ctable, MICRO_OUT, (msv + 1) * sizeof(unsigned));
     return (size_t)r;
 }
 FSEB_API size_t HUF_writeCTable(void* dst, size_t maxDstSize, const unsigned* ctable, unsigned msv, unsigned huffLog)  // lib/huf.h:189
@@ -441,7 +441,7 @@ FSEB_API size_t HUF_writeCTable(void* dst, size_t maxDstSize, const unsigned* ct
     if (msv > HUF_MAX_SV) return (size_t)err(E_MSV_TOO_LARGE);
     Micro m; m.up(0, ctable, (msv + 1) * sizeof(unsigned));
     u64 const r = m.run(MOP_HUF_WRITE_CTABLE, maxDstSize, msv, huffLog);
-    if (!is_err(r)) m.down(dst, 4096, (size_t)r);
+    if (!is_err(r)) m.down(dst, MICRO_OUT, (size_t)r);
     return (size_t)r;
 }
 FSEB_API size_t HUF_readStats(unsigned char* huffWeight, size_t hwSize, unsigned* rankStats, unsigned* nbSymbolsPtr,
@@ -454,9 +454,9 @@ FSEB_API size_t HUF_readStats(unsigned char* huffWeight, size_t hwSize, unsigned
     u64 const r = m.run(MOP_HUF_READ_STATS, take, hwSize);
     if (is_err(r)) return (size_t)r;
     unsigned meta[2];
-    m.down(meta, 8192 + 64, sizeof(meta));
-    m.down(rankStats, 8192, 13 * sizeof(unsigned));
-    m.down(huffWeight, 4096, meta[0]);
+    m.down(meta, MICRO_META_HUF, sizeof(meta));
+    m.down(rankStats, MICRO_META, 13 * sizeof(unsigned));
+    m.down(huffWeight, MICRO_OUT, meta[0]);
     *nbSymbolsPtr = meta[0]; *tableLogPtr = meta[1];
     return (size_t)r;
 }
@@ -468,9 +468,9 @@ FSEB_API size_t HUF_readDTableX1(unsigned* DTable, const void* src, size_t srcSi
     u64 const r = m.run(MOP_HUF_READ_DTABLE_X1, take, DTable[0]);
     if (is_err(r)) return (size_t)r;
     unsigned hdr = 0;
-    m.down(&hdr, 16384, sizeof(hdr));
+    m.down(&hdr, MICRO_DTABLE_X1, sizeof(hdr));
     unsigned const tl = (hdr >> 16) & 0xFF;
-    m.down(DTable, 16384, sizeof(unsigned) + ((size_t)1 << tl) * 2);
+    m.down(DTable, MICRO_DTABLE_X1, sizeof(unsigned) + ((size_t)1 << tl) * 2);
     return (size_t)r;
 }
 
@@ -541,6 +541,35 @@ void ctable_image(unsigned (&full)[256], const unsigned* CTable, const void* src
     std::memset(full, 0, sizeof(full));
     std::memcpy(full, CTable, ((size_t)top + 1) * sizeof(unsigned));
 }
+// HUF_compress{4,1}X_usingCTable: the output area, then `stages` private areas of the same size behind it (4X: one per stream).
+size_t huf_encode_using_ctable(int opcode, size_t stages, void* dst, size_t dstSize, const void* src, size_t srcSize, const unsigned* CTable)
+{
+    if (srcSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
+    size_t const cap = dstSize < 2 * srcSize + 64 ? dstSize : 2 * srcSize + 64;
+    size_t const outOff = MICRO_PAYLOAD + al16(srcSize + 16);
+    Micro m(outOff + (1 + stages) * al16(cap) + 64);
+    unsigned full[256]; ctable_image(full, CTable, src, srcSize);
+    m.up(0, full, sizeof(full)); m.up(MICRO_PAYLOAD, src, srcSize);
+    u64 const r = m.run(opcode, srcSize, cap, MICRO_PAYLOAD, outOff);
+    if (!is_err(r) && r) m.down(dst, outOff, (size_t)r);
+    return (size_t)r;
+}
+// HUF_decompress{4,1}X{1,2}_usingDTable: the DTable must be of `type` (0: X1, huf_decompress.c:367,434 ; 1: X2, :866,910); its
+// image is the header word and 2^tableLog cells of cellBytes each.  On success the whole output capacity is copied back.
+size_t huf_decode_using_dtable(int opcode, unsigned type, size_t cellBytes, void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize,
+                               const unsigned* DTable)
+{
+    unsigned const t = (DTable[0] >> 8) & 0xFF, tl = (DTable[0] >> 16) & 0xFF;
+    if (t != type) return (size_t)err(E_GENERIC);
+    if (tl > HUF_MAX_TLOG) return (size_t)err(E_TLOG_TOO_LARGE);
+    if (cSrcSize > MICRO_MAX || maxDstSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
+    size_t const outOff = MICRO_PAYLOAD + al16(cSrcSize + 16);
+    Micro m(outOff + maxDstSize + 64);
+    m.up(0, DTable, sizeof(unsigned) + (cellBytes << tl)); m.up(MICRO_PAYLOAD, cSrc, cSrcSize);
+    u64 const r = m.run(opcode, cSrcSize, maxDstSize, MICRO_PAYLOAD, outOff);
+    if (!is_err(r)) m.down(dst, outOff, maxDstSize);
+    return (size_t)r;
+}
 }
 FSEB_API size_t FSE_compress_usingCTable(void* dst, size_t dstSize, const void* src, size_t srcSize, const unsigned* ct)   // lib/fse.h:222
 {
@@ -550,10 +579,10 @@ FSEB_API size_t FSE_compress_usingCTable(void* dst, size_t dstSize, const void* 
     if (srcSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
     size_t const cap = dstSize < 2 * srcSize + 64 ? dstSize : 2 * srcSize + 64;     // <= 12 bits per symbol: more room can never be used
     size_t const ctBytes = (1 + (tl ? ((size_t)1 << (tl - 1)) : 1) + 2 * ((size_t)msv + 1)) * sizeof(unsigned);   // FSE_CTABLE_SIZE_U32 ; rle tables: fse_compress.c:532
-    size_t const inOff = 16384, outOff = inOff + al16(srcSize + 16);
+    size_t const outOff = MICRO_PAYLOAD + al16(srcSize + 16);
     Micro m(outOff + cap + 64);
-    m.up(0, ct, ctBytes); m.up(inOff, src, srcSize);
-    u64 const r = m.run(MOP_FSE_ENCODE_CT, srcSize, cap, inOff, outOff);
+    m.up(0, ct, ctBytes); m.up(MICRO_PAYLOAD, src, srcSize);
+    u64 const r = m.run(MOP_FSE_ENCODE_CT, srcSize, cap, MICRO_PAYLOAD, outOff);
     if (!is_err(r) && r) m.down(dst, outOff, (size_t)r);
     return (size_t)r;
 }
@@ -562,57 +591,21 @@ FSEB_API size_t FSE_decompress_usingDTable(void* dst, size_t maxDstSize, const v
     unsigned const tl = dt[0] & 0xFFFF;
     if (tl > FSE_MAX_TLOG) return (size_t)err(E_TLOG_TOO_LARGE);
     if (cSrcSize > MICRO_MAX || maxDstSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
-    size_t const inOff = 32768, outOff = inOff + al16(cSrcSize + 16);
+    size_t const outOff = MICRO_PAYLOAD + al16(cSrcSize + 16);
     Micro m(outOff + maxDstSize + 64);
-    m.up(0, dt, (1 + ((size_t)1 << tl)) * sizeof(unsigned)); m.up(inOff, cSrc, cSrcSize);
-    u64 const r = m.run(MOP_FSE_DECODE_DT, cSrcSize, maxDstSize, inOff, outOff);
+    m.up(0, dt, (1 + ((size_t)1 << tl)) * sizeof(unsigned)); m.up(MICRO_PAYLOAD, cSrc, cSrcSize);
+    u64 const r = m.run(MOP_FSE_DECODE_DT, cSrcSize, maxDstSize, MICRO_PAYLOAD, outOff);
     if (!is_err(r) && r) m.down(dst, outOff, (size_t)r);
     return (size_t)r;
 }
 FSEB_API size_t HUF_compress4X_usingCTable(void* dst, size_t dstSize, const void* src, size_t srcSize, const unsigned* CTable)   // lib/huf.h:191
-{
-    if (srcSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
-    size_t const cap = dstSize < 2 * srcSize + 64 ? dstSize : 2 * srcSize + 64;
-    size_t const inOff = 4096, outOff = inOff + al16(srcSize + 16);
-    Micro m(outOff + 5 * al16(cap) + 64);
-    unsigned full[256]; ctable_image(full, CTable, src, srcSize);
-    m.up(0, full, sizeof(full)); m.up(inOff, src, srcSize);
-    u64 const r = m.run(MOP_HUF_ENCODE4X_CT, srcSize, cap, inOff, outOff);
-    if (!is_err(r) && r) m.down(dst, outOff, (size_t)r);
-    return (size_t)r;
-}
+{ return huf_encode_using_ctable(MOP_HUF_ENCODE4X_CT, 4, dst, dstSize, src, srcSize, CTable); }
 FSEB_API size_t HUF_decompress4X1_usingDTable(void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)   // lib/huf.h:277
-{
-    unsigned const type = (DTable[0] >> 8) & 0xFF, tl = (DTable[0] >> 16) & 0xFF;
-    if (type != 0) return (size_t)err(E_GENERIC);                                   // huf_decompress.c:434
-    if (tl > HUF_MAX_TLOG) return (size_t)err(E_TLOG_TOO_LARGE);
-    if (cSrcSize > MICRO_MAX || maxDstSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
-    size_t const inOff = 16384, outOff = inOff + al16(cSrcSize + 16);
-    Micro m(outOff + maxDstSize + 64);
-    m.up(0, DTable, sizeof(unsigned) + ((size_t)1 << tl) * 2); m.up(inOff, cSrc, cSrcSize);
-    u64 const r = m.run(MOP_HUF_DECODE4X1_DT, cSrcSize, maxDstSize, inOff, outOff);
-    if (!is_err(r)) m.down(dst, outOff, maxDstSize);
-    return (size_t)r;
-}
-namespace {
-size_t huf_decode_x2(int opcode, void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)
-{
-    unsigned const type = (DTable[0] >> 8) & 0xFF, tl = (DTable[0] >> 16) & 0xFF;
-    if (type != 1) return (size_t)err(E_GENERIC);                                   // huf_decompress.c:866,910
-    if (tl > HUF_MAX_TLOG) return (size_t)err(E_TLOG_TOO_LARGE);
-    if (cSrcSize > MICRO_MAX || maxDstSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
-    size_t const inOff = 32768, outOff = inOff + al16(cSrcSize + 16);
-    Micro m(outOff + maxDstSize + 64);
-    m.up(0, DTable, sizeof(unsigned) * (1 + ((size_t)1 << tl))); m.up(inOff, cSrc, cSrcSize);
-    u64 const r = m.run(opcode, cSrcSize, maxDstSize, inOff, outOff);
-    if (!is_err(r)) m.down(dst, outOff, maxDstSize);
-    return (size_t)r;
-}
-}
+{ return huf_decode_using_dtable(MOP_HUF_DECODE4X1_DT, 0, 2, dst, maxDstSize, cSrc, cSrcSize, DTable); }
 FSEB_API size_t HUF_decompress4X2_usingDTable(void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)   // lib/huf.h:280
-{ return huf_decode_x2(MOP_HUF_DECODE4X2_DT, dst, maxDstSize, cSrc, cSrcSize, DTable); }
+{ return huf_decode_using_dtable(MOP_HUF_DECODE4X2_DT, 1, 4, dst, maxDstSize, cSrc, cSrcSize, DTable); }
 FSEB_API size_t HUF_decompress1X2_usingDTable(void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)   // lib/huf.h:323
-{ return huf_decode_x2(MOP_HUF_DECODE1X2_DT, dst, maxDstSize, cSrc, cSrcSize, DTable); }
+{ return huf_decode_using_dtable(MOP_HUF_DECODE1X2_DT, 1, 4, dst, maxDstSize, cSrc, cSrcSize, DTable); }
 FSEB_API size_t HUF_decompress4X_usingDTable(void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)    // lib/huf.h:203
 {
     // huf_decompress.c:980-997: dispatch on DTableDesc.tableType
@@ -623,17 +616,7 @@ FSEB_API size_t HUF_decompress4X_usingDTable(void* dst, size_t maxDstSize, const
 // ---- single-stream Huff0 (lib/huf.h:288-320): the same device routines with one stream; HUF_compress1X is the reference's
 //      driver (huf_compress.c:637-724 with HUF_singleStream) composed from the table-level calls above ----
 FSEB_API size_t HUF_compress1X_usingCTable(void* dst, size_t dstSize, const void* src, size_t srcSize, const unsigned* CTable)      // lib/huf.h:290
-{
-    if (srcSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
-    size_t const cap = dstSize < 2 * srcSize + 64 ? dstSize : 2 * srcSize + 64;
-    size_t const inOff = 4096, outOff = inOff + al16(srcSize + 16);
-    Micro m(outOff + cap + 64);
-    unsigned full[256]; ctable_image(full, CTable, src, srcSize);
-    m.up(0, full, sizeof(full)); m.up(inOff, src, srcSize);
-    u64 const r = m.run(MOP_HUF_ENCODE1X_CT, srcSize, cap, inOff, outOff);
-    if (!is_err(r) && r) m.down(dst, outOff, (size_t)r);
-    return (size_t)r;
-}
+{ return huf_encode_using_ctable(MOP_HUF_ENCODE1X_CT, 0, dst, dstSize, src, srcSize, CTable); }
 FSEB_API size_t HUF_compress1X(void* dst, size_t dstSize, const void* src, size_t srcSize, unsigned maxSymbolValue, unsigned huffLog)   // lib/huf.h:288
 {
     unsigned char* const ostart = (unsigned char*)dst;
@@ -757,18 +740,7 @@ FSEB_API size_t HUF_decompress4X_usingDTable_bmi2(void* dst, size_t maxDstSize, 
 { (void)bmi2; return HUF_decompress4X_usingDTable(dst, maxDstSize, cSrc, cSrcSize, DTable); }
 
 FSEB_API size_t HUF_decompress1X1_usingDTable(void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)  // lib/huf.h:320
-{
-    unsigned const type = (DTable[0] >> 8) & 0xFF, tl = (DTable[0] >> 16) & 0xFF;
-    if (type != 0) return (size_t)err(E_GENERIC);                                   // huf_decompress.c:367
-    if (tl > HUF_MAX_TLOG) return (size_t)err(E_TLOG_TOO_LARGE);
-    if (cSrcSize > MICRO_MAX || maxDstSize > MICRO_MAX) return (size_t)err(E_SRC_WRONG);
-    size_t const inOff = 16384, outOff = inOff + al16(cSrcSize + 16);
-    Micro m(outOff + maxDstSize + 64);
-    m.up(0, DTable, sizeof(unsigned) + ((size_t)1 << tl) * 2); m.up(inOff, cSrc, cSrcSize);
-    u64 const r = m.run(MOP_HUF_DECODE1X1_DT, cSrcSize, maxDstSize, inOff, outOff);
-    if (!is_err(r)) m.down(dst, outOff, maxDstSize);
-    return (size_t)r;
-}
+{ return huf_decode_using_dtable(MOP_HUF_DECODE1X1_DT, 0, 2, dst, maxDstSize, cSrc, cSrcSize, DTable); }
 FSEB_API size_t HUF_decompress1X_usingDTable(void* dst, size_t maxDstSize, const void* cSrc, size_t cSrcSize, const unsigned* DTable)   // lib/huf.h:318
 {
     return ((DTable[0] >> 8) & 0xFF) ? HUF_decompress1X2_usingDTable(dst, maxDstSize, cSrc, cSrcSize, DTable)      // huf_decompress.c:962-977
@@ -791,7 +763,7 @@ FSEB_API size_t HUF_readDTableX2(unsigned* DTable, const void* src, size_t srcSi
     u64 const r = m.run(MOP_HUF_READ_DTABLE_X2, take, DTable[0]);
     if (is_err(r)) return (size_t)r;
     unsigned const L = DTable[0] & 0xFF;
-    m.down(DTable, 32768, sizeof(unsigned) * (1 + ((size_t)1 << L)));
+    m.down(DTable, MICRO_DTABLE_X2, sizeof(unsigned) * (1 + ((size_t)1 << L)));
     return (size_t)r;
 }
 

@@ -656,28 +656,13 @@ cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const
     if (g.nBlocks == 0) return cudaSuccess;
     cudaError_t e;
     hufe::Plan* plans = nullptr;
-    // Plan scratch (3.2 KB per block).  Default: one grow-only buffer per stream, reused by successive calls (stream order
-    // makes that safe; a different stream gets its own buffer).  FSEB200_SCRATCH_ASYNC=1 switches to cudaMallocAsync/FreeAsync.
+    // Plan scratch (3.2 KB per block): the per-stream grow-only buffer launch_huf_encode_using_ctable also takes its plans from.
+    // FSEB200_SCRATCH_ASYNC=1 switches to cudaMallocAsync/FreeAsync.
     static int asyncScratch = -1;
     if (asyncScratch < 0) { const char* const v = getenv("FSEB200_SCRATCH_ASYNC"); asyncScratch = (v && atoi(v) == 1) ? 1 : 0; }
     size_t const need = sizeof(hufe::Plan) * (size_t)g.nBlocks;
     if (asyncScratch) e = cudaMallocAsync((void**)&plans, need, stream);
-    else {
-        struct Slot { int dev; cudaStream_t s; void* p; size_t cap; };
-        static std::mutex mu; static std::vector<Slot> slots;
-        std::lock_guard<std::mutex> lock(mu);
-        int dev = 0; cudaGetDevice(&dev);                           // the legacy stream handle is the same on every device
-        Slot* hit = nullptr;
-        for (auto& sl : slots) if (sl.s == stream && sl.dev == dev) { hit = &sl; break; }
-        if (!hit) { slots.push_back(Slot{ dev, stream, nullptr, 0 }); hit = &slots.back(); }
-        e = cudaSuccess;
-        if (hit->cap < need) {
-            if (hit->p) { cudaStreamSynchronize(stream); cudaFree(hit->p); hit->p = nullptr; hit->cap = 0; }
-            e = cudaMalloc(&hit->p, need);
-            if (e == cudaSuccess) hit->cap = need;
-        }
-        plans = (hufe::Plan*)hit->p;
-    }
+    else plans = (hufe::Plan*)stream_scratch(2, stream, need, &e);
     if (e != cudaSuccess) return e;
     // The source is read twice, by the plan kernel (histogram) and by the emit kernel: 1.70x the algorithmic DRAM bytes.  Walking the
     // batch in sub-batches whose source fits the 50 MB L2 (FSEB200_HUF_ENC_SUBBATCH = blocks per sub-batch) turns the second read into

@@ -3,6 +3,8 @@
 //   HUF_decodeSymbolX2 / HUF_decodeLastSymbolX2        lib/huf_decompress.c:659-683
 //   HUF_decodeStreamX2                                 lib/huf_decompress.c:693-720
 //   HUF_decompress{1,4}X2_usingDTable_internal_body    lib/huf_decompress.c:722-862
+// and the payload decode both Huff0 decoders share (stream split, rejections, verdict), with the single-symbol stream loop
+// HUF_decodeStreamX1 (:214-237) beside the double-symbol one.
 // Used by the table-level entry points (micro.cu) and by the verdict fix-up pass of the batch decoder
 // (huf_x2_fixup.cu).  One lane per stream on the byte-granular reader model (bitsrc_dev.cuh): these serve single calls and
 // rejected blocks, not throughput.
@@ -60,9 +62,28 @@ __device__ inline u64 d_huf_build_dtable_x2(u32* dt, u32 hdr, u8* weights, u8* l
     return h;
 }
 
-// One stream with the double-symbol table into out[p .. pe): returns the BIT_initDStream verdict; *done = stream consumed exactly.
-__device__ inline u64 d_huf_decode_stream_x2(u8* out, long long p, long long const pe, const u8* s, u64 len, const u32* cells, u32 dtLog, u32* done)
+// One stream with the single-symbol table into out[p .. pe) (HUF_decodeStreamX1, huf_decompress.c:214-237): returns the
+// BIT_initDStream verdict; *done = stream consumed exactly (:348-349).  dtab = { header word, HUF_DEltX1 { byte, nbBits } cells }.
+__device__ inline u64 d_huf_decode_stream_x1(u8* out, long long p, long long const pe, const u8* s, u64 len, const u32* dtab, u32* done)
 {
+    const u16* const cells = reinterpret_cast<const u16*>(dtab + 1);
+    u32 const dtLog = (dtab[0] >> 16) & 0xFF;
+    BitSrc b;
+    *done = 0;
+    u64 const ie = bs_open(b, s, len);
+    if (is_err(ie)) return ie;
+    auto sym = [&]() { u32 const cell = cells[bs_peek_fast(b, dtLog)]; b.used += cell >> 8; out[p++] = (u8)cell; };
+    while ((bs_refill(b) == SRC_MORE) & (p < pe - 3)) { sym(); sym(); sym(); sym(); }
+    while (p < pe) sym();
+    *done = bs_exhausted(b) ? 1u : 0u;
+    return 0;
+}
+
+// One stream with the double-symbol table into out[p .. pe): returns the BIT_initDStream verdict; *done = stream consumed exactly.
+__device__ inline u64 d_huf_decode_stream_x2(u8* out, long long p, long long const pe, const u8* s, u64 len, const u32* dtab, u32* done)
+{
+    const u32* const cells = dtab + 1;
+    u32 const dtLog = (dtab[0] >> 16) & 0xFF;
     BitSrc b;
     *done = 0;
     u64 const ie = bs_open(b, s, len);
@@ -86,21 +107,24 @@ __device__ inline u64 d_huf_decode_stream_x2(u8* out, long long p, long long con
     return 0;
 }
 
-// CTA-cooperative payload decode with a double-symbol table image: lanes 0..3 take the streams; every thread of the CTA must
-// call it (one barrier inside).  s_init / s_done: 4-entry shared scratch.  Returns the reference's value (all threads).
-__device__ inline u64 cta_huf_decode_x2(bool four, const u32* dtab, const u8* c, u64 cs, u8* out, u64 n, u64* s_init, u32* s_done)
+typedef u64 (*HufStreamDecoder)(u8* out, long long p, long long pe, const u8* s, u64 len, const u32* dtab, u32* done);
+
+// CTA-cooperative payload decode with a table image: four streams (HUF_decompress4X{1,2}_usingDTable, huf_decompress.c:262-354,
+// 749-862) or one (HUF_decompress1X{1,2}_usingDTable, :240-260,722-747), thread k decoding stream k with DEC
+// (d_huf_decode_stream_x1 or _x2).  Every thread of the CTA must call it (barriers inside).  s_init / s_done: 4-entry shared
+// scratch.  Returns the reference's value (all threads).
+template <HufStreamDecoder DEC>
+__device__ inline u64 cta_huf_decode(bool four, const u32* dtab, const u8* c, u64 cs, u8* out, u64 n, u64* s_init, u32* s_done)
 {
     int const tid = threadIdx.x;
-    const u32* const cells = dtab + 1;
-    u32 const dtLog = (dtab[0] >> 16) & 0xFF;
-    bool bad = four && cs < 10;                                                      // :751
+    bool bad = four && cs < 10;                                                      // :268,751
     u64 l1 = 0, l2 = 0, l3 = 0, l4 = 0;
     if (four && !bad) {
         l1 = c[0] | ((u64)c[1] << 8); l2 = c[2] | ((u64)c[3] << 8); l3 = c[4] | ((u64)c[5] << 8);
         if (l1 + l2 + l3 + 6 > cs) bad = true; else l4 = cs - (l1 + l2 + l3 + 6);   // :787 (the reference would read out of bounds)
     }
     u64 const seg = four ? (n + 3) / 4 : n;
-    if (four && !bad && 3 * seg > n) bad = true;                                     // dstSize < 6: same guard as the single-symbol path
+    if (four && !bad && 3 * seg > n) bad = true;                                     // dstSize < 6: the reference writes out of bounds (documented deviation)
     int const nStreams = four ? 4 : 1;
     if (tid < nStreams) {
         u64 ie = 0; u32 done = 0;
@@ -108,7 +132,7 @@ __device__ inline u64 cta_huf_decode_x2(bool four, const u32* dtab, const u8* c,
             u64 const lens[4] = { four ? l1 : cs, l2, l3, l4 };
             u64 off = four ? 6 : 0; for (int k = 0; k < tid; k++) off += lens[k];
             long long const p = (long long)(seg * tid); long long const pe = (four && tid < 3) ? (long long)(seg * (tid + 1)) : (long long)n;
-            ie = d_huf_decode_stream_x2(out, p, pe, c + off, lens[tid], cells, dtLog, &done);
+            ie = DEC(out, p, pe, c + off, lens[tid], dtab, &done);
         }
         s_init[tid] = ie; s_done[tid] = done;
     }

@@ -52,7 +52,7 @@ huf_x2_fixup_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cb
             u64 r;
             if (is_err(h)) r = h;                                                   // :934
             else if (h >= cs) r = err(E_SRC_WRONG);                                 // :935
-            else r = cta_huf_decode_x2(true, s_dt, c + h, cs - h, dst + (u64)bb * g.blockSize, n, s_init, s_done);
+            else r = cta_huf_decode<d_huf_decode_stream_x2>(true, s_dt, c + h, cs - h, dst + (u64)bb * g.blockSize, n, s_init, s_done);
             if (tid == 0) results[bb] = r;
             __syncthreads();
         }

@@ -6,6 +6,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <mutex>
+#include <vector>
 
 namespace fseb {
 
@@ -65,16 +66,12 @@ inline void* stream_scratch(int purpose, cudaStream_t stream, size_t bytes, cuda
 {
     struct Slot { int purpose, dev; cudaStream_t s; void* p; size_t cap; };
     static std::mutex mu;
-    static Slot slots[256];
-    static int nSlots = 0;
+    static std::vector<Slot> slots;
     std::lock_guard<std::mutex> lock(mu);
     int const dev = current_device();
     Slot* hit = nullptr;
-    for (int i = 0; i < nSlots; i++) if (slots[i].purpose == purpose && slots[i].s == stream && slots[i].dev == dev) { hit = &slots[i]; break; }
-    if (!hit) {
-        if (nSlots == 256) { *err = cudaErrorMemoryAllocation; return nullptr; }
-        slots[nSlots] = Slot{ purpose, dev, stream, nullptr, 0 }; hit = &slots[nSlots++];
-    }
+    for (auto& sl : slots) if (sl.purpose == purpose && sl.s == stream && sl.dev == dev) { hit = &sl; break; }
+    if (!hit) { slots.push_back(Slot{ purpose, dev, stream, nullptr, 0 }); hit = &slots.back(); }
     *err = cudaSuccess;
     if (hit->cap < bytes) {
         if (hit->p) { cudaStreamSynchronize(stream); cudaFree(hit->p); hit->p = nullptr; hit->cap = 0; }

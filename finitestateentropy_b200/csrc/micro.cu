@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(256) hist16_kernel(const u16* src, u64 n, u32 
 }
 
 // ---- everything O(alphabet)/O(table): one kernel, op-code dispatched ----
-// buf layout is op specific (see capi.cu); a[] carries scalars.
+// buf layout: the offsets in micro.h, per op below; a[] carries scalars.
 __global__ void __launch_bounds__(256) micro_kernel(int op, MicroArgs A, u8* buf, u64* ret)
 {
     __shared__ u32 s_count[256];
@@ -72,56 +72,56 @@ __global__ void __launch_bounds__(256) micro_kernel(int op, MicroArgs A, u8* buf
     __shared__ u32 s_w[384];
     int const tid = threadIdx.x;
     switch (op) {
-    case MOP_NORMALIZE: {          // in: count u32[msv+1] @0 ; out: norm i16[msv+1] @4096
-        if (tid == 0) *ret = d_normalize((short*)(buf + 4096), (unsigned)A.a[0], (const unsigned*)buf, A.a[1], (unsigned)A.a[2]);
+    case MOP_NORMALIZE: {          // in: count u32[msv+1] @0 ; out: norm i16[msv+1] @MICRO_OUT
+        if (tid == 0) *ret = d_normalize((short*)(buf + MICRO_OUT), (unsigned)A.a[0], (const unsigned*)buf, A.a[1], (unsigned)A.a[2]);
         break; }
-    case MOP_WRITE_NCOUNT: {       // in: norm @0 ; out: bytes @4096
-        if (tid == 0) *ret = d_write_ncount(buf + 4096, A.a[0], (const short*)buf, (unsigned)A.a[1], (unsigned)A.a[2]);
+    case MOP_WRITE_NCOUNT: {       // in: norm @0 ; out: bytes @MICRO_OUT
+        if (tid == 0) *ret = d_write_ncount(buf + MICRO_OUT, A.a[0], (const short*)buf, (unsigned)A.a[1], (unsigned)A.a[2]);
         break; }
-    case MOP_READ_NCOUNT: {        // in: header bytes @0 (size a0), msv in a1 ; out: norm @4096, msv/tl as u32 @8192
+    case MOP_READ_NCOUNT: {        // in: header bytes @0 (size a0), msv in a1 ; out: norm @MICRO_OUT, msv/tl as u32 @MICRO_META
         if (tid == 0) {
             unsigned msv = (unsigned)A.a[1], tl = 0;
-            *ret = d_read_ncount((short*)(buf + 4096), &msv, &tl, buf, A.a[0]);
-            ((u32*)(buf + 8192))[0] = msv; ((u32*)(buf + 8192))[1] = tl;
+            *ret = d_read_ncount((short*)(buf + MICRO_OUT), &msv, &tl, buf, A.a[0]);
+            ((u32*)(buf + MICRO_META))[0] = msv; ((u32*)(buf + MICRO_META))[1] = tl;
         }
         break; }
-    case MOP_BUILD_CTABLE: {       // in: norm @0 ; out: ct @4096 ; scratch @65536
+    case MOP_BUILD_CTABLE: {       // in: norm @0 ; out: ct @MICRO_OUT ; scratch @MICRO_WORK
         if (tid == 0) {
             unsigned const msv = (unsigned)A.a[0], tl = (unsigned)A.a[1];
             if (tl > 13 || msv > 4095) { *ret = err(E_TLOG_TOO_LARGE); break; }
-            d_build_ctable_serial((u32*)(buf + 4096), (const short*)buf, msv, tl, (u16*)(buf + 65536), (u32*)(buf + 65536 + 32768));
+            d_build_ctable_serial((u32*)(buf + MICRO_OUT), (const short*)buf, msv, tl, (u16*)(buf + MICRO_WORK), (u32*)(buf + MICRO_WORK + 32768));
             *ret = 0;
         }
         break; }
-    case MOP_BUILD_DTABLE: {       // in: norm @0 ; out: dt @4096 ; a2 = wide
+    case MOP_BUILD_DTABLE: {       // in: norm @0 ; out: dt @MICRO_OUT ; a2 = wide
         if (tid == 0) {
             unsigned const msv = (unsigned)A.a[0], tl = (unsigned)A.a[1];
-            if (A.a[2]) *ret = d_build_dtable_serial<true>((u32*)(buf + 4096), (const short*)buf, msv, tl, U16_MAX_SV, U16_MAX_TLOG, (u16*)(buf + 65536), (u16*)(buf + 65536 + 32768));
-            else *ret = d_build_dtable_serial<false>((u32*)(buf + 4096), (const short*)buf, msv, tl, FSE_MAX_SV, FSE_MAX_TLOG, (u16*)(buf + 65536), (u16*)(buf + 65536 + 32768));
+            if (A.a[2]) *ret = d_build_dtable_serial<true>((u32*)(buf + MICRO_OUT), (const short*)buf, msv, tl, U16_MAX_SV, U16_MAX_TLOG, (u16*)(buf + MICRO_WORK), (u16*)(buf + MICRO_WORK + 32768));
+            else *ret = d_build_dtable_serial<false>((u32*)(buf + MICRO_OUT), (const short*)buf, msv, tl, FSE_MAX_SV, FSE_MAX_TLOG, (u16*)(buf + MICRO_WORK), (u16*)(buf + MICRO_WORK + 32768));
         }
         break; }
-    case MOP_HUF_BUILD_CTABLE: {   // in: count u32[256] @0 ; out: ctable u32[256] @4096
+    case MOP_HUF_BUILD_CTABLE: {   // in: count u32[256] @0 ; out: ctable u32[256] @MICRO_OUT
         s_count[tid] = ((u32)tid <= A.a[0]) ? ((const u32*)buf)[tid] : 0;
         __syncthreads();
         u64 const r = cta_huf_build_ctable(s_ct, s_count, (u32)A.a[0], (u32)A.a[1], s_nodes, s_a, s_b);
-        if (!is_err(r)) ((u32*)(buf + 4096))[tid] = s_ct[tid];
+        if (!is_err(r)) ((u32*)(buf + MICRO_OUT))[tid] = s_ct[tid];
         if (tid == 0) *ret = r;
         break; }
-    case MOP_HUF_WRITE_CTABLE: {   // in: ctable u32[256] @0 ; out: bytes @4096 ; a0 = cap, a1 = msv, a2 = huffLog
-        if (tid == 0) *ret = d_huf_write_ctable(buf + 4096, A.a[0] < 136 ? A.a[0] : 136, (const u32*)buf, (unsigned)A.a[1], (unsigned)A.a[2], s_w);
+    case MOP_HUF_WRITE_CTABLE: {   // in: ctable u32[256] @0 ; out: bytes @MICRO_OUT ; a0 = cap, a1 = msv, a2 = huffLog
+        if (tid == 0) *ret = d_huf_write_ctable(buf + MICRO_OUT, A.a[0] < 136 ? A.a[0] : 136, (const u32*)buf, (unsigned)A.a[1], (unsigned)A.a[2], s_w);
         break; }
-    case MOP_HUF_READ_STATS: {     // in: bytes @0 (a0) ; out: weights @4096 (hwSize a1), rankStats u32[13] @8192, nbSym,tl @8192+64
+    case MOP_HUF_READ_STATS: {     // in: bytes @0 (a0) ; out: weights @MICRO_OUT (hwSize a1), rankStats u32[13] @MICRO_META, nbSym,tl @MICRO_META_HUF
         if (tid == 0) {
             u32 nb = 0, tl = 0;
-            *ret = d_huf_read_stats(buf + 4096, A.a[1], (u32*)(buf + 8192), &nb, &tl, buf, A.a[0]);
-            ((u32*)(buf + 8192 + 64))[0] = nb; ((u32*)(buf + 8192 + 64))[1] = tl;
+            *ret = d_huf_read_stats(buf + MICRO_OUT, A.a[1], (u32*)(buf + MICRO_META), &nb, &tl, buf, A.a[0]);
+            ((u32*)(buf + MICRO_META_HUF))[0] = nb; ((u32*)(buf + MICRO_META_HUF))[1] = tl;
         }
         break; }
-    case MOP_HUF_READ_DTABLE_X1: { // in: bytes @0 (a0), a1 = DTable header word ; out: dtable u32[1+2048] @16384
+    case MOP_HUF_READ_DTABLE_X1: { // in: bytes @0 (a0), a1 = DTable header word ; out: dtable u32[1+2048] @MICRO_DTABLE_X1
         if (tid == 0) {
-            u8* const weights = buf + 4096;
+            u8* const weights = buf + MICRO_OUT;
             u32 rank[17]; u32 nb = 0, tl = 0;
-            u32* const dt = (u32*)(buf + 16384);
+            u32* const dt = (u32*)(buf + MICRO_DTABLE_X1);
             u16* const cells = (u16*)(dt + 1);
             u64 const h = d_huf_read_stats(weights, 256, rank, &nb, &tl, buf, A.a[0]);
             u32 const hdr = (u32)A.a[1];
@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(256) micro_kernel(int op, MicroArgs A, u8* buf
         }
         break; }
     // ---- payload coding with a caller-supplied table image (the *_usingCTable / *_usingDTable entry points): table @0,
-    //      input @a2 (a0 bytes), output @a3 (capacity a1).  One lane per stream; these serve single calls, not throughput.
+    //      input @a2 = MICRO_PAYLOAD (a0 bytes), output @a3 (capacity a1).  One lane per stream; these serve single calls, not throughput.
     case MOP_FSE_ENCODE_CT: {      // FSE_compress_usingCTable (fse_compress.c:554-623)
         if (tid == 0) *ret = d_fse_encode_serial(buf + A.a[3], A.a[1], buf + A.a[2], A.a[0], (const u32*)buf);
         break; }
@@ -180,51 +180,6 @@ __global__ void __launch_bounds__(256) micro_kernel(int op, MicroArgs A, u8* buf
             *ret = r;
         }
         break; }
-    case MOP_HUF_DECODE4X1_DT: {   // HUF_decompress4X1_usingDTable (huf_decompress.c:262-354): lane k decodes stream k into segment k
-        __shared__ u64 s_init[4]; __shared__ u32 s_done[4];
-        const u32* const dtab = (const u32*)buf;
-        const u16* const cells = (const u16*)(dtab + 1);                             // HUF_DEltX1 { byte, nbBits }
-        u32 const dtLog = (dtab[0] >> 16) & 0xFF;
-        const u8* const c = buf + A.a[2]; u8* const out = buf + A.a[3];
-        u64 const cs = A.a[0], n = A.a[1];
-        bool bad = cs < 10;                                                          // :268
-        u64 l1 = 0, l2 = 0, l3 = 0, l4 = 0;
-        if (!bad) {
-            l1 = c[0] | ((u64)c[1] << 8); l2 = c[2] | ((u64)c[3] << 8); l3 = c[4] | ((u64)c[5] << 8);
-            if (l1 + l2 + l3 + 6 > cs) bad = true; else l4 = cs - (l1 + l2 + l3 + 6);   // the reference would read out of bounds here
-        }
-        u64 const seg = (n + 3) / 4;
-        if (!bad && 3 * seg > n) bad = true;                                         // dstSize < 6: the reference writes out of bounds (documented deviation)
-        if (tid < 4) {
-            u64 ie = 0; u32 done = 0;
-            if (!bad) {
-                u64 const lens[4] = { l1, l2, l3, l4 };
-                u64 off = 6; for (int k = 0; k < tid; k++) off += lens[k];
-                long long p = (long long)(seg * tid); long long const pe = tid < 3 ? (long long)(seg * (tid + 1)) : (long long)n;
-                BitSrc b;
-                ie = bs_open(b, c + off, lens[tid]);
-                if (!is_err(ie)) {
-                    ie = 0;
-                    auto sym = [&]() { u32 const cell = cells[bs_peek_fast(b, dtLog)]; b.used += cell >> 8; out[p++] = (u8)cell; };
-                    while ((bs_refill(b) == SRC_MORE) & (p < pe - 3)) { sym(); sym(); sym(); sym(); }   // HUF_decodeStreamX1 :214-237
-                    while (p < pe) sym();
-                    done = bs_exhausted(b) ? 1u : 0u;                                // :348-349
-                }
-            }
-            s_init[tid] = ie; s_done[tid] = done;
-        }
-        __syncthreads();
-        if (tid == 0) {
-            u64 r = n;
-            if (bad) r = err(E_CORRUPT);
-            else {
-                bool initFailed = false;
-                for (int k = 0; k < 4; k++) if (is_err(s_init[k])) { r = s_init[k]; initFailed = true; break; }   // CHECK_F in stream order (:297-300)
-                if (!initFailed && !(s_done[0] & s_done[1] & s_done[2] & s_done[3])) r = err(E_CORRUPT);
-            }
-            *ret = r;
-        }
-        break; }
     case MOP_HUF_ENCODE1X_CT: {    // HUF_compress1X_usingCTable (huf_compress.c:457-502): one stream, last symbol first
         if (tid == 0) {
             const u32* const ct = (const u32*)buf; const u8* const in = buf + A.a[2];
@@ -236,29 +191,19 @@ __global__ void __launch_bounds__(256) micro_kernel(int op, MicroArgs A, u8* buf
             *ret = sink_close(sk);
         }
         break; }
-    case MOP_HUF_DECODE1X1_DT: {   // HUF_decompress1X1_usingDTable (huf_decompress.c:240-260)
-        if (tid == 0) {
-            const u32* const dtab = (const u32*)buf;
-            const u16* const cells = (const u16*)(dtab + 1);
-            u32 const dtLog = (dtab[0] >> 16) & 0xFF;
-            u8* const out = buf + A.a[3];
-            long long p = 0; long long const pe = (long long)A.a[1];
-            BitSrc b;
-            u64 const e = bs_open(b, buf + A.a[2], A.a[0]);
-            if (is_err(e)) { *ret = e; break; }
-            auto sym = [&]() { u32 const cell = cells[bs_peek_fast(b, dtLog)]; b.used += cell >> 8; out[p++] = (u8)cell; };
-            while ((bs_refill(b) == SRC_MORE) & (p < pe - 3)) { sym(); sym(); sym(); sym(); }
-            while (p < pe) sym();
-            *ret = bs_exhausted(b) ? (u64)pe : err(E_CORRUPT);
-        }
+    case MOP_HUF_READ_DTABLE_X2: { // HUF_readDTableX2 (huf_decompress.c:551-649): in: bytes @0 (a0), a1 = DTable header word ; out: dtable u32[1+4096] @MICRO_DTABLE_X2
+        if (tid == 0) *ret = d_huf_build_dtable_x2((u32*)(buf + MICRO_DTABLE_X2), (u32)A.a[1], buf + MICRO_OUT, buf + MICRO_META, buf + MICRO_META + 256, buf, A.a[0]);
         break; }
-    case MOP_HUF_READ_DTABLE_X2: { // HUF_readDTableX2 (huf_decompress.c:551-649): in: bytes @0 (a0), a1 = DTable header word ; out: dtable u32[1+4096] @32768
-        if (tid == 0) *ret = d_huf_build_dtable_x2((u32*)(buf + 32768), (u32)A.a[1], buf + 4096, buf + 8192, buf + 8192 + 256, buf, A.a[0]);
-        break; }
-    case MOP_HUF_DECODE4X2_DT:     // HUF_decompress4X2_usingDTable (huf_decompress.c:749-862): lane k decodes stream k with the double-symbol table
-    case MOP_HUF_DECODE1X2_DT: {   // HUF_decompress1X2_usingDTable (:722-747): one stream
-        __shared__ u64 s_init2[4]; __shared__ u32 s_done2[4];
-        u64 const r = cta_huf_decode_x2(op == MOP_HUF_DECODE4X2_DT, (const u32*)buf, buf + A.a[2], A.a[0], buf + A.a[3], A.a[1], s_init2, s_done2);
+    case MOP_HUF_DECODE4X1_DT:     // HUF_decompress4X1_usingDTable (huf_decompress.c:262-354)
+    case MOP_HUF_DECODE1X1_DT:     // HUF_decompress1X1_usingDTable (:240-260)
+    case MOP_HUF_DECODE4X2_DT:     // HUF_decompress4X2_usingDTable (:749-862)
+    case MOP_HUF_DECODE1X2_DT: {   // HUF_decompress1X2_usingDTable (:722-747)
+        __shared__ u64 s_init[4]; __shared__ u32 s_done[4];
+        bool const four = op == MOP_HUF_DECODE4X1_DT || op == MOP_HUF_DECODE4X2_DT;
+        const u32* const dtab = (const u32*)buf; const u8* const c = buf + A.a[2]; u8* const out = buf + A.a[3];
+        u64 const r = (op == MOP_HUF_DECODE4X1_DT || op == MOP_HUF_DECODE1X1_DT)
+                    ? cta_huf_decode<d_huf_decode_stream_x1>(four, dtab, c, A.a[0], out, A.a[1], s_init, s_done)
+                    : cta_huf_decode<d_huf_decode_stream_x2>(four, dtab, c, A.a[0], out, A.a[1], s_init, s_done);
         if (tid == 0) *ret = r;
         break; }
     default: if (tid == 0) *ret = err(E_GENERIC);

@@ -337,6 +337,34 @@ def test_full_compare_at_256mib(codec, mib):
     assert int(sizes.sum()) > n // 20
 
 
+def test_fse_stream_longer_than_2_32_bits():
+    """one 1 GiB FSE block on the chain-warp kernel (16-byte aligned source, size a multiple of 64) whose stream is longer than
+    2^32 bits: 64 equally likely symbols cost 6 bits each, and the most frequent one stays above the n >> 7 early exit.  The
+    return value and the compressed bytes against the compiled reference, and the reference decoding them back."""
+    lib, isref = checker()
+    if not isref:
+        pytest.skip("needs the compiled reference")
+    n = 1 << 30
+    gen = torch.Generator(device="cuda")
+    gen.manual_seed(1)
+    d = torch.randint(0, 64, (n,), dtype=torch.uint8, device="cuda", generator=gen)
+    assert d.data_ptr() % 16 == 0
+    data = d.cpu().numpy()
+    slot = fb.compress_bound(n)
+    want_c = np.empty(slot, np.uint8)
+    want = lib.FSE_compress2(ptr(want_c), slot, ptr(data), n, 255, 12)
+    assert not is_error(want) and 8 * (want - 512 - 1) > 1 << 32, want     # the NCount header takes at most 512 bytes
+    cbuf, cs = fb.fse_compress_batch(d, n, slot, 255, 12)
+    assert int(cs.cpu().numpy().view(np.uint64)[0]) == want
+    got_c = cbuf[:want].cpu().numpy()
+    del cbuf, d
+    assert np.array_equal(got_c, want_c[:want])
+    out = np.empty(n, np.uint8)
+    assert lib.FSE_decompress(ptr(out), n, ptr(got_c), want) == n
+    assert np.array_equal(out, data)
+    torch.cuda.empty_cache()
+
+
 def test_raw_and_rle_tables_through_payload_calls():
     """FSE_buildCTable_raw/_rle + FSE_buildDTable_raw/_rle images driven through FSE_compress_usingCTable /
     FSE_decompress_usingDTable on the GPU vs the compiled reference (fullbench.c:595-629 call pattern)"""
