@@ -62,6 +62,8 @@ def _declare(L):
     sig("FSEB200_batch_blocks", c_sz, c_sz, c_sz)
     sig("FSEB200_HUF_decompress_batch", c_sz, c_vp, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp)
     sig("HUF_decompress", c_sz, c_vp, c_sz, c_vp, c_sz)
+    sig("FSEB200_HUF_compress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
+    sig("FSEB200_HUF_decompress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     for name in ("FSEB200_HUF_compress_batch", "FSEB200_FSE_compress_batch", "FSEB200_FSE_decompress_batch",
                  "FSEB200_FSEU16_compress_batch", "FSEB200_FSEU16_decompress_batch"):
         if hasattr(L, name):
@@ -72,4 +74,5 @@ def _declare(L):
 
 
 from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch, fse_decompress_batch,  # noqa: E402,F401
-                    fseu16_compress_batch, fseu16_decompress_batch, nblocks)
+                    fseu16_compress_batch, fseu16_decompress_batch, nblocks,
+                    huf_compress_blocks, huf_decompress_blocks, block_pointers)

@@ -2,7 +2,10 @@
 
 Geometry is the one programs/bench.c:530-548 builds: a flat uncompressed buffer split into
 `block_size` blocks (last one shorter), compressed block b in the fixed slot `cbuf[b*slot : (b+1)*slot]`,
-`csizes[b]` = the reference's return value for that block (0 = stored raw, 1 = RLE, error codes in-band)."""
+`csizes[b]` = the reference's return value for that block (0 = stored raw, 1 = RLE, error codes in-band).
+
+The `*_blocks` calls take per-block descriptors instead (FSEB200_HUF_*_blocks): int64 CUDA tensors of device addresses and
+sizes, one entry per block, so blocks of any size may sit anywhere -- e.g. packed back to back."""
 import torch
 
 
@@ -87,3 +90,47 @@ def fseu16_compress_batch(src, block_size=32768, slot=32768, max_symbol_value=0,
 
 def fseu16_decompress_batch(cbuf, csizes, total, block_size=32768, slot=32768, out=None, results=None, orig=None):
     return _decompress("FSEB200_FSEU16_decompress_batch", cbuf, csizes, total, block_size, slot, out, results, orig)
+
+
+def block_pointers(views):
+    """(ptrs, sizes): int64 tensors of the device addresses and lengths of a list of 1-D uint8 CUDA views, on their device"""
+    dev = views[0].device if views else torch.device("cuda")
+    for v in views:
+        assert v.is_cuda and v.dtype == torch.uint8 and v.dim() == 1 and v.is_contiguous() and v.device == dev, (v.device, v.dtype)
+    ptrs = torch.tensor([v.data_ptr() for v in views], dtype=torch.int64).to(dev)
+    sizes = torch.tensor([v.numel() for v in views], dtype=torch.int64).to(dev)
+    return ptrs, sizes
+
+
+def _blocks_args(*arrays):
+    n = arrays[0].numel()
+    for a in arrays:
+        _check(a, torch.int64)
+        assert a.numel() == n and a.device == arrays[0].device, (a.numel(), n, a.device)
+    return n
+
+
+def huf_compress_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes=None, max_symbol_value=255, table_log=12):
+    """HUF_compress2 on every block b: src_ptrs[b] / src_sizes[b] into dst_ptrs[b] of capacity dst_caps[b], on the current
+    stream.  Returns csizes (int64; the reference's value per block, error codes as their two's-complement)."""
+    from . import lib
+    if csizes is None:
+        csizes = torch.empty(src_ptrs.numel(), dtype=torch.int64, device=src_ptrs.device)
+    n = _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes)
+    r = lib().FSEB200_HUF_compress_blocks(n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
+                                          src_sizes.data_ptr(), max_symbol_value, table_log, _stream_ptr())
+    _ret(r, "FSEB200_HUF_compress_blocks")
+    return csizes
+
+
+def huf_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=None):
+    """HUF_decompress on every block b: csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of dst_sizes[b] bytes, on the current
+    stream.  Returns results (int64; regenerated size or error code per block)."""
+    from . import lib
+    if results is None:
+        results = torch.empty(csrc_ptrs.numel(), dtype=torch.int64, device=csrc_ptrs.device)
+    n = _blocks_args(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results)
+    r = lib().FSEB200_HUF_decompress_blocks(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), csrc_ptrs.data_ptr(),
+                                            csrc_sizes.data_ptr(), _stream_ptr())
+    _ret(r, "FSEB200_HUF_decompress_blocks")
+    return results

@@ -3,6 +3,7 @@
 // Two tiers:
 //   1. FSEB200_*_batch : device-pointer, stream-ordered, whole-batch entry points -- what the
 //      per-chunk loops of the reference harness (programs/bench.c:353-364 and :389-424) collapse into.
+//      FSEB200_HUF_*_blocks: the same for Huff0 blocks given by per-block device descriptors (common.cuh BlockDescs).
 //   2. the reference's own one-block-per-call symbols (lib/fse.h, lib/huf.h, lib/hist.h,
 //      lib/fseU16.h) with HOST pointers: they stage the block through a private device workspace and
 //      run the same kernels with a batch of one.  Correct drop-ins for unmodified callers; not the
@@ -22,6 +23,8 @@ namespace fseb {
 cudaError_t launch_huf_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t, u32 flags);
 cudaError_t launch_huf_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_huf_encode_using_ctable(const BatchGeom&, void*, u64*, const void*, const u32*, cudaStream_t);
+cudaError_t launch_huf_encode_blocks(const BlockDescs&, unsigned, unsigned, cudaStream_t);
+cudaError_t launch_huf_decode_blocks(const BlockDescs&, cudaStream_t);
 cudaError_t launch_fse_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t);
 cudaError_t launch_fse_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fseu16_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t);
@@ -188,6 +191,31 @@ FSEB_API size_t FSEB200_HUF_compress4X_usingCTable_batch(void* dCBuf, size_t slo
 {
     if (blockSize == 0 || blockSize > HUF_BLOCK_MAX || slot > 0xFFFFFFFFull || !dCTable) return (size_t)err(E_SRC_WRONG);
     return ok_or_generic(launch_huf_encode_using_ctable(geom(srcTotal, blockSize, slot), dCBuf, (u64*)dCSizes, dSrc, dCTable, (cudaStream_t)stream));
+}
+
+// Per-block descriptors (see common.cuh BlockDescs): every array and every buffer it points to is device memory, and the host never
+// reads them -- the per-block verdicts (sizes above a block, capacities, parameters) all come from the kernels.
+namespace {
+size_t huf_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dOut, const void* const* dSrcs, const size_t* dSrcSizes,
+                  bool compress, unsigned msv, unsigned tlog, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || !dDsts || !dDstSizes || !dOut || !dSrcs || !dSrcSizes) return (size_t)err(E_SRC_WRONG);
+    BlockDescs g;
+    g.dst = (u8* const*)dDsts; g.dstCap = (const u64*)dDstSizes; g.result = (u64*)dOut;
+    g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes; g.nBlocks = (u32)nBlocks;
+    return ok_or_generic(compress ? launch_huf_encode_blocks(g, msv, tlog, (cudaStream_t)stream) : launch_huf_decode_blocks(g, (cudaStream_t)stream));
+}
+}
+FSEB_API size_t FSEB200_HUF_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                            const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, true, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                              const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
+{
+    return huf_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, false, 0, 0, stream);
 }
 
 FSEB_API size_t FSEB200_batch_blocks(size_t total, size_t blockSize) { return blockSize ? (total + blockSize - 1) / blockSize : 0; }

@@ -44,6 +44,7 @@ __device__ __forceinline__ u32 rd32(const u8* p) { return rd16(p) | (rd16(p + 2)
 //   fixed slot cbuf + b*slot (slot = FSE_compressBound(blockSize) in the reference harness).
 // -------------------------------------------------------------------------------------------
 struct BatchGeom {
+    static constexpr bool DESCS = false;
     u64 total;       // uncompressed bytes in the whole batch
     u32 blockSize;   // uncompressed bytes per block (last block may be shorter)
     u32 slot;        // byte stride between compressed blocks == per-block dst capacity
@@ -55,5 +56,65 @@ __host__ __device__ __forceinline__ u32 block_len(const BatchGeom& g, u32 b)
     u64 const left = g.total - off;
     return left < g.blockSize ? (u32)left : g.blockSize;
 }
+
+// -------------------------------------------------------------------------------------------
+// Descriptor geometry: block b is wherever the caller's device arrays say, every block with its own sizes.
+//   compress:   src[b] / srcSize[b] = uncompressed input, dst[b] / dstCap[b] = output capacity, result[b] = cSize
+//   decompress: src[b] / srcSize[b] = compressed input,   dst[b] / dstCap[b] = dstSize,         result[b] = regenerated size
+// Contract (include/fse_b200.h): no destination overlaps another destination, a source or the arrays; `result` overlaps no
+// other array (the emit kernel, the decoder's verdicts and the X2 pass read the sizes after earlier kernels wrote results);
+// sources may overlap each other; a compressed input is readable up to the end of the 32-byte sector that holds its last byte.
+// -------------------------------------------------------------------------------------------
+struct BlockDescs {
+    static constexpr bool DESCS = true;
+    u8* const* dst;
+    const u64* dstCap;
+    u64* result;
+    const u8* const* src;
+    const u64* srcSize;
+    u32 nBlocks;
+};
+__host__ __forceinline__ BlockDescs slice(const BlockDescs& g, u32 b0, u32 n)   // blocks [b0, b0 + n) as a batch of their own
+{
+    BlockDescs s = g;
+    s.dst += b0; s.dstCap += b0; s.result += b0; s.src += b0; s.srcSize += b0; s.nBlocks = n;
+    return s;
+}
+
+// The Huff0 kernels locate a block only through these accessors, one set per geometry.  The uniform geometry's pointer
+// arguments are the batch's buffers; the descriptor geometry ignores them (its launchers pass nullptr).
+// A size above what any Huff0 block can have is reported as HUF_BLOCK_MAX + 1: every verdict the kernels derive from it
+// ("larger than a block", "larger than the compressed size") is the same as for the literal value.
+__device__ __forceinline__ u32 clamp_len(u64 n) { return n > HUF_BLOCK_MAX ? HUF_BLOCK_MAX + 1 : (u32)n; }
+
+// encoder: uncompressed source, its length, the output, its capacity, the compressed size
+__device__ __forceinline__ const u8* enc_src(const BatchGeom& g, const u8* src, u32 b) { return src + (u64)b * g.blockSize; }
+__device__ __forceinline__ u32 enc_len(const BatchGeom& g, u32 b) { return block_len(g, b); }
+__device__ __forceinline__ u8* enc_dst(BatchGeom g, u8* cbuf, u32 b) { return cbuf + (u64)b * g.slot; }   // by value: the emit kernel then compiles as it did before the accessors
+__device__ __forceinline__ u64 enc_cap(const BatchGeom& g, u32) { return g.slot; }
+__device__ __forceinline__ u64& enc_out(const BatchGeom&, u64* csizes, u32 b) { return csizes[b]; }
+__device__ __forceinline__ const u8* enc_src(const BlockDescs& g, const u8*, u32 b) { return g.src[b]; }
+__device__ __forceinline__ u32 enc_len(const BlockDescs& g, u32 b) { return clamp_len(g.srcSize[b]); }
+__device__ __forceinline__ u8* enc_dst(const BlockDescs& g, u8*, u32 b) { return g.dst[b]; }
+__device__ __forceinline__ u64 enc_cap(const BlockDescs& g, u32 b) { u64 const c = g.dstCap[b]; return c > 0xFFFFFF00ull ? 0xFFFFFF00ull : c; }   // as one_block_compress
+__device__ __forceinline__ u64& enc_out(const BlockDescs& g, u64*, u32 b) { return g.result[b]; }
+
+// decoder: compressed source, its size, the output, the regenerated size, the result; `orig` (stored blocks) is uniform-only
+__device__ __forceinline__ const u8* dec_src(const BatchGeom& g, const u8* cbuf, u32 b) { return cbuf + (u64)b * g.slot; }
+__device__ __forceinline__ u64 dec_csize(const BatchGeom&, const u64* csizes, u32 b) { return csizes[b]; }
+__device__ __forceinline__ u8* dec_dst(const BatchGeom& g, u8* dst, u32 b) { return dst + (u64)b * g.blockSize; }
+__device__ __forceinline__ u32 dec_len(const BatchGeom& g, u32 b) { return block_len(g, b); }
+__device__ __forceinline__ u64& dec_out(const BatchGeom&, u64* results, u32 b) { return results[b]; }
+__device__ __forceinline__ const u8* dec_orig(const BatchGeom& g, const u8* orig, u32 b) { return orig + (u64)b * g.blockSize; }
+__device__ __forceinline__ const u8* dec_src(const BlockDescs& g, const u8*, u32 b) { return g.src[b]; }
+__device__ __forceinline__ u64 dec_csize(const BlockDescs& g, const u64*, u32 b) { return g.srcSize[b]; }
+__device__ __forceinline__ u8* dec_dst(const BlockDescs& g, u8*, u32 b) { return g.dst[b]; }
+__device__ __forceinline__ u32 dec_len(const BlockDescs& g, u32 b) { return clamp_len(g.dstCap[b]); }
+__device__ __forceinline__ u64& dec_out(const BlockDescs& g, u64*, u32 b) { return g.result[b]; }
+__device__ __forceinline__ const u8* dec_orig(const BlockDescs&, const u8*, u32) { return nullptr; }
+// The lowest address the decoder's stream feeder may read for block b: the batch buffer's first 32-byte sector, or, for
+// descriptors, the block's own first sector (a block may be the first bytes of an allocation).
+__device__ __forceinline__ u64 dec_floor(const BatchGeom&, const u8* cbuf, const u8*) { return reinterpret_cast<u64>(cbuf) & ~31ull; }
+__device__ __forceinline__ u64 dec_floor(const BlockDescs&, const u8*, const u8* block) { return reinterpret_cast<u64>(block) & ~31ull; }
 
 }  // namespace fseb

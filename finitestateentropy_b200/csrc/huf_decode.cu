@@ -41,6 +41,10 @@
 namespace fseb {
 namespace hufd {
 
+#ifndef FSEB200_HUFD_HEAD
+#define FSEB200_HUFD_HEAD 1       // 0: descriptor batches decode misaligned segments per symbol (a build for measuring the head decode)
+#endif
+
 constexpr int G = 64;             // block columns per CTA
 constexpr int THREADS = 4 * G;    // one lane per stream
 constexpr int NWARPS = THREADS / 32;
@@ -80,6 +84,9 @@ __host__ __device__ constexpr u32 smem_bytes(u32 rows, bool staged) { return row
 __device__ __forceinline__ u32 lds_u16(u32 addr) { u16 v; asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr)); return v; }
 __device__ __forceinline__ u32 lds_u32(u32 addr) { u32 v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr)); return v; }
 __device__ __forceinline__ void sts_u32(u32 addr, u32 v) { asm volatile("st.shared.u32 [%0], %1;" :: "r"(addr), "r"(v) : "memory"); }
+
+// symbols a stream decodes one at a time before its output position reaches a 32-byte boundary (descriptor batches)
+__device__ __forceinline__ u32 head_symbols(const u8* outp) { return (u32)(0ull - reinterpret_cast<u64>(outp)) & 31u; }
 
 // canonical-code look-up in tableLog-bit index space -> (nbBits | symbol << 8)
 __device__ __forceinline__ u32 canon_cell(const u16* rankEnd, const u16* listStart, const u8* sorted, u32 idx, u32 tl)
@@ -209,9 +216,9 @@ __device__ void setup_block(u16* tbl, Facts& fx, BuildScratch& bs, u32 rows, int
     __syncwarp();
 }
 
-template <bool PASS_A>
+template <bool PASS_A, class Geo>
 __global__ void __launch_bounds__(THREADS, 4)
-huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf, const u64* __restrict__ csizes,
+huf_decode_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, const u64* __restrict__ csizes,
                   u64* __restrict__ results, const u8* __restrict__ orig, u32 flags, u32 gEff, u32 rows,
                   const u32* __restrict__ list, const u32* __restrict__ listCount, u32* __restrict__ deferList, u32* __restrict__ deferCount)
 {
@@ -238,20 +245,29 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
     for (int j = warp; j < G; j += NWARPS) {
         u32 const b = fx.bid[j];
         if (b == NOBLOCK) continue;                                     // warp-uniform
-        u64 const n = block_len(g, b);
-        u64 const cs = csizes[b];
+        u64 const n = dec_len(g, b);
+        u64 const cs = dec_csize(g, csizes, b);
         int kind;
-        if (flags & 1u) kind = 0;                                       // HUF_decompress4X1 / 4X2 semantics: always a Huffman block
-        else if (is_err(cs)) { kind = 3; if (lane == 0) results[b] = cs; }   // propagated compressor error
-        else if (cs == 0) { kind = orig ? 1 : 3; if (lane == 0) results[b] = orig ? n : 0; }   // stored raw by the harness (bench.c:393-397)
-        else if (n == 0) { kind = 3; if (lane == 0) results[b] = err(E_DST_TOO_SMALL); }        // huf_decompress.c:1063
-        else if (cs > n) { kind = 3; if (lane == 0) results[b] = err(E_CORRUPT); }              // :1064
-        else if (cs == n) kind = 1;                                                                // :1065
-        else if (cs == 1) kind = 2;                                                                // :1066
-        else kind = 0;
+        if constexpr (!Geo::DESCS) {
+            if (flags & 1u) kind = 0;                                  // HUF_decompress4X1 / 4X2 semantics: always a Huffman block
+            else if (is_err(cs)) { kind = 3; if (lane == 0) results[b] = cs; }   // propagated compressor error
+            else if (cs == 0) { kind = orig ? 1 : 3; if (lane == 0) results[b] = orig ? n : 0; }   // stored raw by the harness (bench.c:393-397)
+            else if (n == 0) { kind = 3; if (lane == 0) results[b] = err(E_DST_TOO_SMALL); }        // huf_decompress.c:1063
+            else if (cs > n) { kind = 3; if (lane == 0) results[b] = err(E_CORRUPT); }              // :1064
+            else if (cs == n) kind = 1;                                                                // :1065
+            else if (cs == 1) kind = 2;                                                                // :1066
+            else kind = 0;
+        } else {                                                        // HUF_decompress on the literal sizes, the library's limit first
+            if (n == 0) { kind = 3; if (lane == 0) dec_out(g, results, b) = err(E_DST_TOO_SMALL); }             // huf_decompress.c:1063
+            else if (n > HUF_BLOCK_MAX) { kind = 3; if (lane == 0) dec_out(g, results, b) = err(E_SRC_WRONG); } // capi.cu HUF_decompress
+            else if (cs > n) { kind = 3; if (lane == 0) dec_out(g, results, b) = err(E_CORRUPT); }              // :1064
+            else if (cs == n) kind = 1;                                                                            // :1065
+            else if (cs == 1) kind = 2;                                                                            // :1066
+            else kind = 0;
+        }
         if (lane == 0) fx.kind[j] = (u8)kind;
         if (kind == 0) {
-            setup_block(tbl, fx, bs, rows, j, cbuf + (u64)b * g.slot, cs, warp);
+            setup_block(tbl, fx, bs, rows, j, dec_src(g, cbuf, b), cs, warp);
             if (deferList && fx.hard[j] && fx.status[j] == NOERR) {     // pass A: hand the block to the pass with the larger table budget
                 if (lane == 0) { deferList[atomicAdd(deferCount, 1u)] = b; fx.kind[j] = 3; }
             }
@@ -264,18 +280,20 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
     int const strm = warp & 3;
     u32 const b = fx.bid[col];
     bool const live = (b != NOBLOCK) && fx.kind[col] == 0 && fx.status[col] == NOERR;
-    u32 const n = live ? block_len(g, b) : 0;
+    u32 const n = live ? dec_len(g, b) : 0;
     u32 const seg = (n + 3) / 4;
     u32 segLen = 0;                                  // symbols this lane must produce
-    u8* outp = dst + (u64)b * g.blockSize + (u64)strm * seg;
+    u8* outp = (Geo::DESCS && !live) ? nullptr : dec_dst(g, dst, b) + (u64)strm * seg;   // an empty column has no descriptor to read
+    const u8* blockStart = nullptr;                  // the block's compressed bytes (the feeder's lower limit, dec_floor)
     u64 chunkTop = 0;                                // address just above chunk 0
     u32 expectBits = 0;                              // stream bits between chunkTop and the first byte of the stream
     u32 c0 = 0;                                      // bits to skip at the top of chunk 0: garbage above the stream + zero padding + end mark
     u32 const tl = fx.tlog[col];
 
     if (live) {
-        const u8* const cs0 = cbuf + (u64)b * g.slot;
-        u64 const cs = csizes[b];
+        const u8* const cs0 = dec_src(g, cbuf, b);
+        u64 const cs = dec_csize(g, csizes, b);
+        blockStart = cs0;
         const u8* const pay = cs0 + fx.hsize[col];
         u64 const psize = cs - fx.hsize[col];
         u32 code = 0;
@@ -318,12 +336,14 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
     // and a rejected block's bytes are not part of the contract.  That keeps the hot loop to ONE unconditional 16-byte load:
     // with a second, conditional load path inlined next to it, ptxas shared a scoreboard slot between the two and every
     // 16 symbols the window shift waited a DRAM round trip for a load it does not depend on.
-    // Chunks that would lie below the compressed buffer itself re-read its first 16 bytes (address clamp, never dereferenced
-    // out of bounds).
+    // Chunks that would lie below the compressed buffer itself (for descriptors: below the block's own first 32-byte sector)
+    // re-read its first sector (address clamp, never dereferenced out of bounds).
     u32 const ringLane = (u32)__cvta_generic_to_shared(ringRaw) + tid * 4;      // + slot * (THREADS*4)
     // Chunks are fetched a PAIR at a time: one whole 32-byte sector, as two back-to-back 16-byte loads (sm_90 has no
     // 32-byte LDG).  The pair waits in eight registers; its two chunks enter the ring one after the other.
-    u32 const pLimit = go ? (u32)((chunkTop - (reinterpret_cast<u64>(cbuf) & ~31ull)) >> 5) - 1u : 0u;   // last pair at or above the buffer start
+    u32 pLimit;                                      // last pair at or above the buffer start (descriptors: the block's first sector)
+    if constexpr (Geo::DESCS) pLimit = go ? (u32)((chunkTop - dec_floor(g, cbuf, blockStart)) >> 5) - 1u : 0u;
+    else pLimit = go ? (u32)((chunkTop - (reinterpret_cast<u64>(cbuf) & ~31ull)) >> 5) - 1u : 0u;
     u32 m0 = 0, m1 = 0, m2 = 0, m3 = 0, m4 = 0, m5 = 0, m6 = 0, m7 = 0;        // pending pair, memory order (m7 = highest address = first consumed)
     // L2 residency (pass A): all 131,072 streams of a 1 GiB batch are in flight at once and a lane takes ~50 us to use up a
     // 128-byte input line, so the live lines of the batch (one input + one partial output line per lane, 32 MiB) come close to
@@ -448,8 +468,24 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
     // sectors (0.45 ms per GiB in the same benchmark).  Lanes leave the fast path at different trip counts: the loop runs the
     // warp's longest count and a finished lane only takes part in the transposed stores.  Pass B has no room for the staging
     // (its larger table budget keeps the near-flat alphabets off the per-symbol path): its lanes write their sectors directly.
-    bool const fastOk = go && !hardBlk && ((reinterpret_cast<u64>(outp) & 31) == 0);
-    u32 const nIter = fastOk ? segLen >> 5 : 0u;
+    // Descriptor batches: a segment of seg = ceil(n / 4) bytes starts on a 32-byte boundary for about one stream in four, so a
+    // lane whose segment start is misaligned first decodes the (-outp) & 31 symbols up to the next boundary one at a time
+    // ("head", topped up like the tail loop) and then enters the fast loop there.  Hard blocks and segments with less than one
+    // sector after the head stay on the per-symbol path.  The uniform geometry keeps its aligned-segments-only rule.
+    constexpr bool withHead = Geo::DESCS && FSEB200_HUFD_HEAD;
+    bool const fastOk = withHead ? go && !hardBlk && segLen >= head_symbols(outp) + 32u
+                                 : go && !hardBlk && ((reinterpret_cast<u64>(outp) & 31) == 0);
+    u32 const headN = (withHead && fastOk) ? head_symbols(outp) : 0u;
+    if constexpr (withHead) {
+        for (u32 i = 0; i < headN; i++) {            // <= 8 symbols (<= 3 words) between checks, as in the tail loop: the fast
+            if ((i & 7) == 0) top_up(4);             // loop's first group-start check still finds 1 <= unread <= 8
+            u32 e;
+            HUFD_LOOKUP(e, hi);
+            HUFD_ADVANCE(e);
+            outp[pos++] = (u8)(e >> 8);
+        }
+    }
+    u32 const nIter = fastOk ? (segLen - headN) >> 5 : 0u;
     u32 const nIterW = __reduce_max_sync(FULL, nIter);
     u32 const stageW = (u32)__cvta_generic_to_shared(tbl) + rows * (G * 2) + (u32)warp * STAGE_WARP_BYTES;
     for (u32 it = 0; it < nIterW; it++) {
@@ -489,7 +525,7 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
         // evict_last.  As for the loads, the policy is chosen by per-lane predicates over two stores with constant policies.
         // Pass B (direct stores) runs at half the occupancy and keeps the default policy.
         u32 const o32 = (u32)dstHere - pos;                                      // low bits of outp
-        bool const lineDone = ((((o32 + pos) | 127u) + 1u) - o32) <= nIter * 32u;    // the fast path finishes this sector's line
+        bool const lineDone = ((((o32 + pos) | 127u) + 1u) - o32) <= headN + nIter * 32u;   // the fast path finishes this sector's line
         u32 const flags = (act ? 1u : 0u) | (lineDone ? 2u : 0u);
         #pragma unroll
         for (int k = 0; k < 2; k++) {                                            // lanes 2j, 2j+1 write the two halves of lane 16k + j's sector
@@ -545,12 +581,12 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
         u32 const bb = fx.bid[tid];
         if (bb != NOBLOCK && fx.kind[tid] == 0) {
             u32 const st = fx.status[tid];
-            u64 rv = (st == NOERR) ? (u64)block_len(g, bb) : err(st & 0xFF);
+            u64 rv = (st == NOERR) ? (u64)dec_len(g, bb) : err(st & 0xFF);
             // Rejected only by the exact-consumption rule of the single-symbol decoder: where the reference would have run
             // its double-symbol decoder (always for HUF_decompress4X2, by HUF_selectDecoder for HUF_decompress) the verdict
             // is the second pass's (huf_x2_fixup.cu).
-            if ((st >> 8) == 5u && ((flags & 2u) || (!(flags & 1u) && d_huf_select_decoder(block_len(g, bb), csizes[bb])))) rv = HUF_X2_PENDING;
-            results[bb] = rv;
+            if ((st >> 8) == 5u && ((flags & 2u) || (!(flags & 1u) && d_huf_select_decoder(dec_len(g, bb), dec_csize(g, csizes, bb))))) rv = HUF_X2_PENDING;
+            dec_out(g, results, bb) = rv;
         }
     }
     // ---- raw / RLE blocks (huf_decompress.c:1065-1066; the harness' own 0-size convention, bench.c:393-402) ----
@@ -558,27 +594,31 @@ huf_decode_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf
         int const kd = fx.kind[j];
         if (kd != 1 && kd != 2) continue;
         u32 const bb = fx.bid[j];
-        u32 const nn = block_len(g, bb);
-        u64 const cs = csizes[bb];
-        u8* const o = dst + (u64)bb * g.blockSize;
-        if (kd == 2) { u8 const v = cbuf[(u64)bb * g.slot]; for (u32 i = tid; i < nn; i += THREADS) o[i] = v; }
+        u32 const nn = dec_len(g, bb);
+        u64 const cs = dec_csize(g, csizes, bb);
+        u8* const o = dec_dst(g, dst, bb);
+        if (kd == 2) { u8 const v = dec_src(g, cbuf, bb)[0]; for (u32 i = tid; i < nn; i += THREADS) o[i] = v; }
         else {
-            const u8* const s = (cs == 0) ? orig + (u64)bb * g.blockSize : cbuf + (u64)bb * g.slot;
+            const u8* const s = (cs == 0) ? dec_orig(g, orig, bb) : dec_src(g, cbuf, bb);    // cs == 0 is never raw for descriptors
             for (u32 i = tid; i < nn; i += THREADS) o[i] = s[i];
         }
-        if (tid == 0) results[bb] = nn;
+        if (tid == 0) dec_out(g, results, bb) = nn;
     }
 }
 
 }  // namespace hufd
 
 cudaError_t launch_huf_x2_fixup(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream);
+cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, cudaStream_t stream);
+
+namespace {
 
 // flags: bit 0 = every block is a Huffman block (HUF_decompress4X1 / 4X2 semantics: no raw / RLE forms);
 //        bit 1 = verdicts of the double-symbol decoder for every block (HUF_decompress4X2);
 //        0     = HUF_decompress: raw / RLE forms, decoder (and hence verdict on malformed input) by HUF_selectDecoder.
-cudaError_t launch_huf_decode(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results,
-                              const void* orig, cudaStream_t stream, u32 flags)
+template <class Geo>
+cudaError_t huf_decode(const Geo& g, void* dst, const void* cbuf, const u64* csizes, u64* results,
+                       const void* orig, cudaStream_t stream, u32 flags)
 {
     static SmemOptIn optinA, optinB;
     // Table rows per CTA.  Pass A: 306 rows + the 8 KB output staging -> 55.5 KB -> FOUR CTAs (256 blocks) per SM; pass B, for the
@@ -594,8 +634,8 @@ cudaError_t launch_huf_decode(const BatchGeom& g, void* dst, const void* cbuf, c
     u32 const rowsB = min(reqB, fit(false));
     size_t const smemA = hufd::smem_bytes(rowsA, true);
     bool const twoPass = rowsB > rowsA;
-    cudaError_t e = optinA.ensure(hufd::huf_decode_kernel<true>, dev, (int)smemA);
-    if (e == cudaSuccess && twoPass) e = optinB.ensure(hufd::huf_decode_kernel<false>, dev, (int)hufd::smem_bytes(rowsB, false));
+    cudaError_t e = optinA.ensure(hufd::huf_decode_kernel<true, Geo>, dev, (int)smemA);
+    if (e == cudaSuccess && twoPass) e = optinB.ensure(hufd::huf_decode_kernel<false, Geo>, dev, (int)hufd::smem_bytes(rowsB, false));
     if (e != cudaSuccess) return e;
     u32* scratch = nullptr;
     if (twoPass) {
@@ -609,7 +649,7 @@ cudaError_t launch_huf_decode(const BatchGeom& g, void* dst, const void* cbuf, c
     // the machine is spread evenly -- every SM the same number of blocks per round, CTAs only partly full; a small batch (a pipeline
     // chunk, a scatter/gather piece, one block) packs its CTAs full instead, so that each SM hosts as few warps as possible.
     int perSm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, hufd::huf_decode_kernel<true>, hufd::THREADS, smemA) != cudaSuccess || perSm < 1) perSm = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, hufd::huf_decode_kernel<true, Geo>, hufd::THREADS, smemA) != cudaSuccess || perSm < 1) perSm = 1;
     u32 const slots = (u32)perSm * (u32)device_sm_count(dev);
     u32 gEff = (u32)hufd::G;
     if ((u64)g.nBlocks * 5 > (u64)slots * hufd::G * 4) {                 // more than 80 % of what the machine holds at once (threshold chosen before the H100 port, not re-tuned)
@@ -619,19 +659,33 @@ cudaError_t launch_huf_decode(const BatchGeom& g, void* dst, const void* cbuf, c
         if (gEff < 1) gEff = 1;
     }
     unsigned const grid = (g.nBlocks + gEff - 1) / gEff;
-    hufd::huf_decode_kernel<true><<<grid, hufd::THREADS, smemA, stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results, (const u8*)orig, flags, gEff, rowsA,
+    hufd::huf_decode_kernel<true, Geo><<<grid, hufd::THREADS, smemA, stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results, (const u8*)orig, flags, gEff, rowsA,
                                                                     nullptr, nullptr, twoPass ? scratch + 1 : nullptr, scratch);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     if (twoPass) {   // pass B over the deferred list; its length lives on the device, so the grid covers the worst case and idle CTAs leave at once
         unsigned const gridB = (g.nBlocks + hufd::G - 1) / hufd::G;
-        hufd::huf_decode_kernel<false><<<gridB, hufd::THREADS, hufd::smem_bytes(rowsB, false), stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results, (const u8*)orig, flags,
+        hufd::huf_decode_kernel<false, Geo><<<gridB, hufd::THREADS, hufd::smem_bytes(rowsB, false), stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results, (const u8*)orig, flags,
                                                                                             (u32)hufd::G, rowsB, scratch + 1, scratch, nullptr, nullptr);
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
     if (flags == 1u) return cudaSuccess;                                // X1-only semantics: no verdict pass
-    return launch_huf_x2_fixup(g, dst, cbuf, csizes, results, stream);
+    if constexpr (Geo::DESCS) return launch_huf_x2_fixup_blocks(g, stream);
+    else return launch_huf_x2_fixup(g, dst, cbuf, csizes, results, stream);
+}
+}  // namespace
+
+cudaError_t launch_huf_decode(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results,
+                              const void* orig, cudaStream_t stream, u32 flags)
+{
+    return huf_decode(g, dst, cbuf, csizes, results, orig, stream, flags);
+}
+
+// per-block descriptors (BlockDescs), HUF_decompress semantics on every block: the same passes, budgets and grid shape
+cudaError_t launch_huf_decode_blocks(const BlockDescs& g, cudaStream_t stream)
+{
+    return huf_decode(g, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 0u);
 }
 
 }  // namespace fseb

@@ -150,16 +150,16 @@ __device__ __forceinline__ void warp_hist4_pipelined(u32 (*count4)[256], const u
     }
 }
 
+template <class Geo>
 __global__ void __launch_bounds__(32 * PLAN_WARPS, 3)
-huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8* __restrict__ src,
+huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8* __restrict__ src,
                 unsigned msvReq, unsigned tlogReq, Plan* __restrict__ plans)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PlanCta& S = *reinterpret_cast<PlanCta*>(smem_raw);
     unsigned const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     u32 const b0 = blockIdx.x * GROUP;
-    u64 const cap = g.slot;
-#define FSEB_FINAL(v) { if (lane == 0) { P.state = 1; csizes[b] = (v); S.live[c] = 0; } continue; }   // next block of the loop
+#define FSEB_FINAL(v) { if (lane == 0) { P.state = 1; enc_out(g, csizes, b) = (v); S.live[c] = 0; } continue; }   // next block of the loop
 
     // ---- phase 1: one warp per block ----
     u32 (*const count4)[256] = reinterpret_cast<u32 (*)[256]>(&S.nd[257][0] + warp * 4 * 256);
@@ -168,8 +168,9 @@ huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, co
         __syncwarp();                                                   // the previous block is done with count4
         u32 const b = b0 + c;
         if (b >= g.nBlocks) { if (lane == 0) S.live[c] = 0; continue; }
-        u32 const n = block_len(g, b);
-        const u8* const s = src + (u64)b * g.blockSize;
+        u32 const n = enc_len(g, b);
+        u64 const cap = enc_cap(g, b);
+        const u8* const s = enc_src(g, src, b);
         Plan& P = plans[b];
         // argument checks of HUF_compress_internal (huf_compress.c:656-664), in its order
         if (!n) FSEB_FINAL(0);
@@ -203,7 +204,7 @@ huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, co
         #pragma unroll
         for (int dlt = 16; dlt; dlt >>= 1) { top = max(top, __shfl_xor_sync(FULL, top, dlt)); best = max(best, __shfl_xor_sync(FULL, best, dlt)); }
         if (msvDecl < 255 && top > msvDecl) FSEB_FINAL(err(E_MSV_TOO_SMALL));                     // hist.c:128
-        if (best == n) { if (lane == 0) cbuf[(u64)b * g.slot] = s[0]; FSEB_FINAL(1); }             // huf_compress.c:673
+        if (best == n) { if (lane == 0) enc_dst(g, cbuf, b)[0] = s[0]; FSEB_FINAL(1); }             // huf_compress.c:673
         if (best <= (n >> 7) + 4) FSEB_FINAL(0);                                                  // :674
         u32 const msv = top;
         // segment counts for phase 3, compacted to u16
@@ -278,6 +279,7 @@ huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, co
         }
         __syncwarp();                                                   // every lane is done with the tree rows: header areas next
         if (live && !is_err(res)) {
+            u64 const cap = enc_cap(g, b0 + c);
             u32* const area = &S.nd[0][0] + c * HDR_STRIDE;
             struct Col { const u32* p; __device__ u32 operator[](u32 i) const { return p[i * GROUP]; } };
             res = d_huf_write_ctable(reinterpret_cast<u8*>(area), cap < 136 ? cap : 136, Col{ ct }, msv, S.tlog[c], area + 34);
@@ -292,7 +294,8 @@ huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, co
     for (u32 c = warp; c < GROUP; c += PLAN_WARPS) {
         if (!S.live[c]) continue;
         u32 const b = b0 + c;
-        u32 const n = block_len(g, b);
+        u32 const n = enc_len(g, b);
+        u64 const cap = enc_cap(g, b);
         Plan& P = plans[b];
         u64 const hs = S.res[c];
         if (is_err(hs)) FSEB_FINAL(hs);
@@ -330,7 +333,7 @@ huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, co
         const u8* const hdr = reinterpret_cast<const u8*>(&S.nd[0][0] + c * HDR_STRIDE);
         for (u32 i = lane; i < (u32)hs; i += 32) P.header[i] = hdr[i];
         if (lane < 4) { P.streamOff[lane] = offs[lane]; P.streamBytes[lane] = lens[lane]; }
-        if (lane == 0) { P.hSize = (u32)hs; P.state = 0; P.total = (u32)total; csizes[b] = total; }
+        if (lane == 0) { P.hSize = (u32)hs; P.state = 0; P.total = (u32)total; enc_out(g, csizes, b) = total; }
     }
 #undef FSEB_FINAL
 }
@@ -348,16 +351,19 @@ huf_plan_kernel(BatchGeom g, u8* __restrict__ cbuf, u64* __restrict__ csizes, co
 constexpr int THREADS = 128;
 
 // A 16-byte piece of a stream window that touches the stream's first or last bytes: only local bytes [a0, endByte) belong to
-// this stream (the neighbours are another warp's), so it goes out byte by byte.  Out of line: once or twice per stream.
-__device__ __noinline__ void store_piece_exact(u32* gw, u32 j, uint4 v, u32 a0, u32 endByte)
+// this stream (the neighbours are another warp's), so it goes out byte by byte.  Out of line: once or twice per stream.  One copy
+// per geometry: shared, the uniform batch's copy would lose the global stores the compiler proves for its kernel parameters.
+template <class Geo>
+static __device__ __noinline__ void store_piece_exact(u32* gw, u32 j, uint4 v, u32 a0, u32 endByte)
 {
     u32 const wd[4] = { v.x, v.y, v.z, v.w };
     u8* const pb = reinterpret_cast<u8*>(gw + j);
     for (u32 t = 0; t < 16; t++) { u32 const at = 4 * j + t; if (at >= a0 && at < endByte) pb[t] = (u8)(wd[t >> 2] >> (8 * (t & 3))); }
 }
 
+template <class Geo>
 __global__ void __launch_bounds__(THREADS)
-huf_emit_kernel(BatchGeom g, u8* __restrict__ cbuf, const u8* __restrict__ src, const Plan* __restrict__ plans, const u32* __restrict__ sharedCT)
+huf_emit_kernel(Geo g, u8* __restrict__ cbuf, const u8* __restrict__ src, const Plan* __restrict__ plans, const u32* __restrict__ sharedCT)
 {
     constexpr u32 W = 512;                                          // words of stream window per warp (a double group adds <= 176, < 128 wait for the next flush)
     __shared__ u32 ctab[256];                                       // cells nbBits | code << 8.  4-byte cells: the kernel is bound by shared-memory
@@ -369,9 +375,9 @@ huf_emit_kernel(BatchGeom g, u8* __restrict__ cbuf, const u8* __restrict__ src, 
     u32 const b = blockIdx.x;
     const Plan& P = plans[b];
     if (P.state != 0) return;                                       // verdict already delivered by the plan kernel
-    u32 const n = block_len(g, b);
-    const u8* const s = src + (u64)b * g.blockSize;
-    u8* const d = cbuf + (u64)b * g.slot;
+    u32 const n = enc_len(g, b);
+    const u8* const s = enc_src(g, src, b);
+    u8* const d = enc_dst(g, cbuf, b);
     u32 const hSize = P.hSize, total = P.total;
 
     {   const u32* const ct = sharedCT ? sharedCT : P.ctable;       // one caller-supplied table for the whole batch, or the block's own
@@ -445,7 +451,7 @@ huf_emit_kernel(BatchGeom g, u8* __restrict__ cbuf, const u8* __restrict__ src, 
                     *reinterpret_cast<uint4*>(win + i) = make_uint4(0, 0, 0, 0);
                     if (i == 0) { v.x |= win[W]; v.y |= win[W + 1]; v.z |= win[W + 2]; win[W] = 0; win[W + 1] = 0; win[W + 2] = 0; }
                     if (!all && (j != 0 || a0 == 0)) *reinterpret_cast<uint4*>(gw + j) = v;   // interior piece: below bitpos, inside the stream
-                    else store_piece_exact(gw, j, v, a0, endByte);  // first / last pieces
+                    else store_piece_exact<Geo>(gw, j, v, a0, endByte);  // first / last pieces
                 }
                 flushed += 128;
             }
@@ -646,12 +652,27 @@ cudaError_t launch_huf_encode_using_ctable(const BatchGeom& g, void* cbuf, u64* 
     if (e != cudaSuccess) return e;
     unsigned const grid = (g.nBlocks + hufe::PLAN_WARPS - 1) / hufe::PLAN_WARPS;
     hufe::huf_sizes_kernel<<<grid, 32 * hufe::PLAN_WARPS, 0, stream>>>(g, csizes, (const u8*)src, dCTable, plans);
-    hufe::huf_emit_kernel<<<g.nBlocks, hufe::THREADS, 0, stream>>>(g, (u8*)cbuf, (const u8*)src, plans, dCTable);
+    hufe::huf_emit_kernel<BatchGeom><<<g.nBlocks, hufe::THREADS, 0, stream>>>(g, (u8*)cbuf, (const u8*)src, plans, dCTable);
     return cudaGetLastError();
 }
 
-cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const void* src,
-                              unsigned msv, unsigned tlog, cudaStream_t stream)
+namespace {
+// blocks [b0, b0 + n) of a batch as a batch of their own: the same geometry over shifted buffers, or a slice of the arrays
+struct SubBatch { BatchGeom g; u8* cbuf; const u8* src; };
+SubBatch sub_batch(const BatchGeom& g, u8* cbuf, const u8* src, u32 b0, u32 n)
+{
+    BatchGeom gs = g;
+    gs.nBlocks = n;
+    u64 const off = (u64)b0 * g.blockSize;
+    u64 const span = (u64)n * g.blockSize;
+    gs.total = (g.total - off < span) ? g.total - off : span;
+    return { gs, cbuf + (u64)b0 * g.slot, src + off };
+}
+struct SubDescs { BlockDescs g; u8* cbuf; const u8* src; };
+SubDescs sub_batch(const BlockDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
+
+template <class Geo>
+cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
     if (g.nBlocks == 0) return cudaSuccess;
     cudaError_t e;
@@ -671,23 +692,32 @@ cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const
     static u32 const subBatch = [] { const char* const v = getenv("FSEB200_HUF_ENC_SUBBATCH"); long n = v ? atol(v) : 0; return (u32)(n < 0 ? 0 : n); }();
     size_t const smem = sizeof(hufe::PlanCta);
     static SmemOptIn optin;
-    e = optin.ensure(hufe::huf_plan_kernel, current_device(), (int)smem);
+    e = optin.ensure(hufe::huf_plan_kernel<Geo>, current_device(), (int)smem);
     if (e != cudaSuccess) return e;
     u32 const step = (subBatch && subBatch < g.nBlocks) ? subBatch : g.nBlocks;
     for (u32 b0 = 0; b0 < g.nBlocks; b0 += step) {
-        BatchGeom gs = g;
-        gs.nBlocks = (g.nBlocks - b0 < step) ? g.nBlocks - b0 : step;
-        u64 const off = (u64)b0 * g.blockSize;
-        u64 const span = (u64)gs.nBlocks * g.blockSize;
-        gs.total = (g.total - off < span) ? g.total - off : span;
-        u8* const cb = (u8*)cbuf + (u64)b0 * g.slot; const u8* const sp = (const u8*)src + off;
-        unsigned const grid = (gs.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
-        hufe::huf_plan_kernel<<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(gs, cb, csizes + b0, sp, msv, tlog, plans + b0);
-        hufe::huf_emit_kernel<<<gs.nBlocks, hufe::THREADS, 0, stream>>>(gs, cb, sp, plans + b0, nullptr);
+        auto const sb = sub_batch(g, (u8*)cbuf, (const u8*)src, b0, (g.nBlocks - b0 < step) ? g.nBlocks - b0 : step);
+        u64* const cs = csizes ? csizes + b0 : nullptr;
+        unsigned const grid = (sb.g.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
+        hufe::huf_plan_kernel<Geo><<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(sb.g, sb.cbuf, cs, sb.src, msv, tlog, plans + b0);
+        hufe::huf_emit_kernel<Geo><<<sb.g.nBlocks, hufe::THREADS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);
     }
     e = cudaGetLastError();
     cudaError_t const e2 = asyncScratch ? cudaFreeAsync(plans, stream) : cudaSuccess;
     return e != cudaSuccess ? e : e2;
+}
+}  // namespace
+
+cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const void* src,
+                              unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return huf_encode(g, cbuf, csizes, src, msv, tlog, stream);
+}
+
+// per-block descriptors (BlockDescs): the same kernels, sub-batches and scratch; the host never reads the arrays
+cudaError_t launch_huf_encode_blocks(const BlockDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return huf_encode(g, nullptr, nullptr, nullptr, msv, tlog, stream);
 }
 
 }  // namespace fseb

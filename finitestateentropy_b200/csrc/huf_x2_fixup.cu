@@ -20,8 +20,9 @@ namespace hufx {
 
 constexpr int THREADS = 128;
 
+template <class Geo>
 __global__ void __launch_bounds__(THREADS)
-huf_x2_fixup_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cbuf, const u64* __restrict__ csizes, u64* __restrict__ results)
+huf_x2_fixup_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, const u64* __restrict__ csizes, u64* __restrict__ results)
 {
     __shared__ u32 s_dt[1 + 4096];
     __shared__ u8 s_scratch[768];
@@ -38,22 +39,22 @@ huf_x2_fixup_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cb
         if (tid == 0) s_nhits = 0;
         __syncthreads();
         u32 const b = base + tid;
-        if (b < c1 && results[b] == HUF_X2_PENDING) s_hits[atomicAdd(&s_nhits, 1u)] = b;
+        if (b < c1 && dec_out(g, results, b) == HUF_X2_PENDING) s_hits[atomicAdd(&s_nhits, 1u)] = b;
         __syncthreads();
         u32 const nh = s_nhits;
         for (u32 i = 0; i < nh; i++) {
             u32 const bb = s_hits[i];
-            const u8* const c = cbuf + (u64)bb * g.slot;
-            u64 const cs = csizes[bb];
-            u64 const n = block_len(g, bb);
+            const u8* const c = dec_src(g, cbuf, bb);
+            u64 const cs = dec_csize(g, csizes, bb);
+            u64 const n = dec_len(g, bb);
             if (tid == 0) s_h = d_huf_build_dtable_x2(s_dt, HUF_MAX_TLOG * 0x01000001u, s_scratch, s_scratch + 256, s_scratch + 512, c, cs);   // HUF_CREATE_STATIC_DTABLEX2(.., HUF_TABLELOG_MAX), :944
             __syncthreads();
             u64 const h = s_h;
             u64 r;
             if (is_err(h)) r = h;                                                   // :934
             else if (h >= cs) r = err(E_SRC_WRONG);                                 // :935
-            else r = cta_huf_decode<d_huf_decode_stream_x2>(true, s_dt, c + h, cs - h, dst + (u64)bb * g.blockSize, n, s_init, s_done);
-            if (tid == 0) results[bb] = r;
+            else r = cta_huf_decode<d_huf_decode_stream_x2>(true, s_dt, c + h, cs - h, dec_dst(g, dst, bb), n, s_init, s_done);
+            if (tid == 0) dec_out(g, results, bb) = r;
             __syncthreads();
         }
     }
@@ -61,14 +62,27 @@ huf_x2_fixup_kernel(BatchGeom g, u8* __restrict__ dst, const u8* __restrict__ cb
 
 }  // namespace hufx
 
-cudaError_t launch_huf_x2_fixup(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream)
+namespace {
+template <class Geo>
+cudaError_t huf_x2_fixup(const Geo& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream)
 {
     if (g.nBlocks == 0) return cudaSuccess;
     unsigned grid = 2u * (unsigned)device_sm_count(current_device());
     unsigned const need = (g.nBlocks + hufx::THREADS - 1) / hufx::THREADS;
     if (grid > need) grid = need;
-    hufx::huf_x2_fixup_kernel<<<grid, hufx::THREADS, 0, stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results);
+    hufx::huf_x2_fixup_kernel<Geo><<<grid, hufx::THREADS, 0, stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results);
     return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t launch_huf_x2_fixup(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream)
+{
+    return huf_x2_fixup(g, dst, cbuf, csizes, results, stream);
+}
+
+cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, cudaStream_t stream)
+{
+    return huf_x2_fixup(g, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 }  // namespace fseb

@@ -12,7 +12,8 @@
  *   - tables are caller-owned `unsigned[]` with the reference's documented layouts and sizes
  *     (lib/fse.h:295-300, lib/huf.h:136-149).
  *
- * Tier 1 (FSEB200_*_batch) works on DEVICE memory and a CUDA stream, a whole batch per call.
+ * Tier 1 (FSEB200_*_batch) works on DEVICE memory and a CUDA stream, a whole batch per call; for Huff0,
+ * FSEB200_HUF_*_blocks does the same for blocks of any size at any address, given by per-block device descriptors.
  * Tier 2 (the reference's own names) works on HOST memory, one block per synchronous call, and is
  * implemented by running the same kernels with a batch of one -- a correct drop-in for unmodified
  * callers (programs/bench.c, the fuzzers), not the fast path.
@@ -62,6 +63,31 @@ size_t FSEB200_FSEU16_compress_batch(void* dCBuf, size_t slot, size_t* dCSizes, 
 size_t FSEB200_FSEU16_decompress_batch(void* dDst, size_t dstTotal, size_t blockSize, const void* dCBuf, size_t slot,
                                        const size_t* dCSizes, size_t* dResults, const void* dOrig, void* stream);
 size_t FSEB200_batch_blocks(size_t total, size_t blockSize);
+
+/* Tier 1, per-block descriptors (Huff0): block b has its own addresses and sizes, given by device arrays -- e.g. the
+ * variable-size literal sections of a zstd-style caller, packed back to back.  All six arrays and every buffer they point to
+ * are in DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).
+ *   compress:   dCSizes[b] = exactly what HUF_compress2(dDsts[b], dDstCapacities[b], dSrcs[b], dSrcSizes[b], maxSymbolValue,
+ *               tableLog) returns: 0, 1 (the byte in dDsts[b][0]), a size or an error code; bytes [0, dCSizes[b]) are the
+ *               reference's.  Per-block verdicts come from the kernels: srcSize > 128 KB gives srcSize_wrong, a bad
+ *               maxSymbolValue / tableLog the reference's error, and a capacity above 2^32 acts as 0xFFFFFF00.
+ *   decompress: dResults[b] = exactly what this library's HUF_decompress(dDsts[b], dDstSizes[b], dCSrcs[b], dCSrcSizes[b])
+ *               returns, sizes taken literally: dstSize 0 gives dstSize_tooSmall, dstSize > 128 KB srcSize_wrong, cSize >
+ *               dstSize corruption_detected, cSize == dstSize is a raw copy, cSize == 1 RLE, anything else is Huffman-decoded
+ *               with the decoder (and verdict on malformed input) HUF_selectDecoder picks.  Unlike the uniform call, cSize 0
+ *               does not mean "stored" and an error code in dCSrcSizes is not passed through.
+ * Contract: no destination may overlap another destination, any source or the arrays (sources may overlap each other), and
+ * the output array (dCSizes / dResults) may not overlap the other arrays: the kernels read the sizes again after writing it.  Each
+ * compressed input must be readable up to the end of the 32-byte-aligned sector that holds its last byte (blocks packed back
+ * to back meet this when the buffer has 32 bytes of slack).  Bytes of [dst, dst + capacity) beyond the returned size are
+ * unspecified; nothing outside the destinations is written.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing); srcSize_wrong if nBlocks > 0xFFFFFFFF or an array is NULL
+ * while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_HUF_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                   const void* const* dSrcs, const size_t* dSrcSizes,
+                                   unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                     const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
 
 /* Table reuse across blocks (lib/huf.h:191 per block; the shape programs/bench.c:610-633 and HUF_compress4X_repeat,
  * lib/huf_compress.c:664-712, reduce to when the previous table is kept): every block of the batch is coded with ONE

@@ -1,0 +1,198 @@
+"""Huff0 through the per-block descriptor calls (FSEB200_HUF_*_blocks) against the uniform batch calls, on one GPU.
+
+  (a) bench layout   1 GiB of probagen P14 in 32 KB blocks: the uniform calls, then the descriptor calls at
+                     ptr = base + b * blockSize (same bytes, same kernels, a few descriptor loads per block more);
+  (b) ragged layout  the same stream cut into seeded sizes uniform in [1 KiB, 128 KiB], sources back to back: encode into
+                     bound-sized destinations, then decode from the compressed blocks packed back to back (packed outside the
+                     timed region) into outputs back to back.  Also the share of streams per decode path and emit path.
+
+Builds are libraries given as LABEL=PATH (default: this tree's).  Each run of each build is a child process; builds alternate
+run by run.  Prints one JSON line with the GPU's name, power limit and SM clock, per build and metric the median and range in
+ms per GiB, and digests of the compressed and decoded bytes, so that builds can be checked to compute the same thing.
+
+    python scripts/huf_blocks_bench.py --make-nohead build/variants/libfse_b200_nohead.so
+    python scripts/huf_blocks_bench.py --runs 5 --build new=finitestateentropy_b200/libfse_b200.so \
+        --build nohead=build/variants/libfse_b200_nohead.so
+
+`--make-nohead PATH` compiles this tree's library with the project's nvcc flags plus -DFSEB200_HUFD_HEAD=0 (descriptor batches
+decode misaligned segments per symbol) into PATH, the build the head decode is measured against.
+"""
+import argparse
+import ctypes as C
+import hashlib
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+GIB = 1 << 30
+BLOCK = 32768
+
+
+def declare(L):
+    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
+    L.FSEB200_probagen.restype = sz; L.FSEB200_probagen.argtypes = [vp, sz, sz, C.c_double, vp]
+    L.FSEB200_HUF_compress_batch.restype = sz; L.FSEB200_HUF_compress_batch.argtypes = [vp, sz, vp, vp, sz, sz, u, u, vp]
+    L.FSEB200_HUF_decompress_batch.restype = sz; L.FSEB200_HUF_decompress_batch.argtypes = [vp, sz, sz, vp, sz, vp, vp, vp, vp]
+    have = hasattr(L, "FSEB200_HUF_compress_blocks")
+    if have:
+        L.FSEB200_HUF_compress_blocks.restype = sz; L.FSEB200_HUF_compress_blocks.argtypes = [sz, vp, vp, vp, vp, vp, u, u, vp]
+        L.FSEB200_HUF_decompress_blocks.restype = sz; L.FSEB200_HUF_decompress_blocks.argtypes = [sz, vp, vp, vp, vp, vp, vp]
+    return have
+
+
+def ragged_sizes(total, seed=7):
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    sizes = rng.integers(1024, 128 * 1024 + 1, total // 1024)
+    ends = np.cumsum(sizes)
+    k = int(np.searchsorted(ends, total))
+    sizes = sizes[: k + 1].copy()
+    sizes[-1] -= int(ends[k] - total)
+    return [int(x) for x in sizes if x > 0]
+
+
+def path_shares(sizes):
+    """share of decode streams per path (head+fast / fast / symbol) and of emit streams per group width, for blocks back to back
+    from a 512-byte aligned start (every block is a pass-A Huffman block for P14)"""
+    from collections import Counter
+    from blocks_paths import stream_paths, stream_kind, emit_groups
+    dec, emit, off = Counter(), Counter(), 0
+    for n in sizes:
+        dec.update(stream_kind(*s) for s in stream_paths("A", n, off))
+        emit.update(emit_groups(off, n))
+        off += n
+    nd, ne = sum(dec.values()), sum(emit.values())
+    return {k: round(v / nd, 4) for k, v in dec.items()}, {k: round(v / ne, 4) for k, v in emit.items()}
+
+
+def child(lib_path, reps):
+    import numpy as np
+    import torch
+    L = C.CDLL(lib_path)
+    have = declare(L)
+    dev = torch.device("cuda")
+    stream = torch.cuda.current_stream().cuda_stream
+    slot = 512 + BLOCK + (BLOCK >> 7) + 12
+    src = torch.empty(GIB + 64, dtype=torch.uint8, device=dev)
+    assert L.FSEB200_probagen(src.data_ptr(), GIB, 0, 0.14, stream) == 0
+    nb = GIB // BLOCK
+
+    def timed(fn):
+        fn()                                                            # warm-up (module load, scratch growth)
+        ts = []
+        for _ in range(reps):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(); fn(); b.record(); b.synchronize()
+            ts.append(a.elapsed_time(b))
+        return sorted(ts)[len(ts) // 2]
+
+    def t64(a):
+        return torch.tensor(np.asarray(a, dtype=np.int64), device=dev)
+
+    out = {}
+    cbuf = torch.empty(nb * slot + 64, dtype=torch.uint8, device=dev)
+    cs = torch.empty(nb, dtype=torch.int64, device=dev)
+    dst = torch.empty(GIB, dtype=torch.uint8, device=dev)
+    res = torch.empty(nb, dtype=torch.int64, device=dev)
+    out["a_enc_uniform"] = timed(lambda: L.FSEB200_HUF_compress_batch(cbuf.data_ptr(), slot, cs.data_ptr(), src.data_ptr(), GIB, BLOCK, 255, 12, stream))
+    out["a_dec_uniform"] = timed(lambda: L.FSEB200_HUF_decompress_batch(dst.data_ptr(), GIB, BLOCK, cbuf.data_ptr(), slot, cs.data_ptr(), res.data_ptr(), None, stream))
+    assert torch.equal(dst, src[:GIB])
+    used = torch.arange(slot, device=dev)[None, :] < cs[:, None]          # bytes [0, cSize) of each slot: the rest is unspecified
+    digest = {"a_cbuf": hashlib.sha256(cbuf[: nb * slot].view(nb, slot)[used].cpu().numpy().tobytes()).hexdigest()[:16]}
+    del used
+    if have:
+        b = np.arange(nb, dtype=np.int64)
+        sp, sn = t64(src.data_ptr() + b * BLOCK), t64(np.full(nb, BLOCK))
+        dp, dc = t64(cbuf.data_ptr() + b * slot), t64(np.full(nb, slot))
+        cs2 = torch.empty_like(cs)
+        out["a_enc_blocks"] = timed(lambda: L.FSEB200_HUF_compress_blocks(nb, dp.data_ptr(), dc.data_ptr(), cs2.data_ptr(), sp.data_ptr(), sn.data_ptr(), 255, 12, stream))
+        assert torch.equal(cs, cs2)
+        op = t64(dst.data_ptr() + b * BLOCK)
+        dst.zero_()
+        out["a_dec_blocks"] = timed(lambda: L.FSEB200_HUF_decompress_blocks(nb, op.data_ptr(), sn.data_ptr(), res.data_ptr(), dp.data_ptr(), cs2.data_ptr(), stream))
+        assert torch.equal(dst, src[:GIB]) and bool((res == BLOCK).all())
+        # (b) ragged
+        sizes = ragged_sizes(GIB)
+        n = len(sizes)
+        offs = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
+        bounds = np.array([129 + s + (s >> 8) + 8 for s in sizes], np.int64)
+        boffs = np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64)
+        del cbuf
+        carena = torch.empty(int(bounds.sum()) + 64, dtype=torch.uint8, device=dev)
+        rsp, rsn = t64(src.data_ptr() + offs), t64(sizes)
+        rdp, rdc = t64(carena.data_ptr() + boffs), t64(bounds)
+        rcs = torch.empty(n, dtype=torch.int64, device=dev)
+        out["b_enc"] = timed(lambda: L.FSEB200_HUF_compress_blocks(n, rdp.data_ptr(), rdc.data_ptr(), rcs.data_ptr(), rsp.data_ptr(), rsn.data_ptr(), 255, 12, stream))
+        csz = rcs.cpu().numpy()
+        assert (csz > 1).all() and (csz < np.array(sizes)).all()
+        poffs = np.concatenate([[0], np.cumsum(csz)[:-1]]).astype(np.int64)
+        packed = torch.empty(int(csz.sum()) + 64, dtype=torch.uint8, device=dev)
+        for i in range(n):                                              # packing: outside the timed region
+            packed[poffs[i]: poffs[i] + csz[i]].copy_(carena[boffs[i]: boffs[i] + csz[i]])
+        del carena
+        digest["b_packed"] = hashlib.sha256(packed[: int(csz.sum())].cpu().numpy().tobytes()).hexdigest()[:16]
+        pp = t64(packed.data_ptr() + poffs)
+        od = t64(dst.data_ptr() + offs)
+        rres = torch.empty(n, dtype=torch.int64, device=dev)
+        dst.zero_()
+        out["b_dec"] = timed(lambda: L.FSEB200_HUF_decompress_blocks(n, od.data_ptr(), rsn.data_ptr(), rres.data_ptr(), pp.data_ptr(), rcs.data_ptr(), stream))
+        assert torch.equal(dst, src[:GIB]) and torch.equal(rres, rsn)
+        out["b_blocks"] = n
+    print(json.dumps({"ms": out, "digest": digest}))
+
+
+def gpu_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    return q[0] if q else "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--build", action="append", default=[], help="LABEL=path/to/libfse_b200.so (repeatable)")
+    ap.add_argument("--runs", type=int, default=5)
+    ap.add_argument("--reps", type=int, default=3, help="timed calls per metric and run (median taken)")
+    ap.add_argument("--child", default=None)
+    ap.add_argument("--make-nohead", metavar="PATH", default=None, help="build the library without the head decode into PATH and exit")
+    a = ap.parse_args()
+    if a.make_nohead:
+        sys.path.insert(0, ROOT)
+        from finitestateentropy_b200 import _build
+        import glob
+        os.makedirs(os.path.dirname(os.path.abspath(a.make_nohead)), exist_ok=True)
+        nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+        srcs = sorted(glob.glob(os.path.join(_build.CSRC, "*.cu")))
+        subprocess.check_call([nvcc] + _build.NVCC_FLAGS + ["-DFSEB200_HUFD_HEAD=0", "-I", os.path.join(ROOT, "include"),
+                               "-o", a.make_nohead] + srcs)
+        return
+    if a.child:
+        child(a.child, a.reps)
+        return
+    builds = [b.split("=", 1) for b in a.build] or [["this", os.path.join(ROOT, "finitestateentropy_b200", "libfse_b200.so")]]
+    runs = {lab: [] for lab, _ in builds}
+    info_before = gpu_info()
+    for _ in range(a.runs):
+        for lab, path in builds:
+            r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", os.path.abspath(path), "--reps", str(a.reps)],
+                               capture_output=True, text=True)
+            assert r.returncode == 0, (lab, r.stderr[-3000:])
+            runs[lab].append(json.loads(r.stdout.strip().splitlines()[-1]))
+    summary = {}
+    for lab, rs in runs.items():
+        ms = {}
+        for k in rs[0]["ms"]:
+            if k == "b_blocks":
+                continue
+            v = sorted(x["ms"][k] for x in rs)                           # per GiB: every layout moves 1 GiB uncompressed
+            ms[k] = {"median": round(v[len(v) // 2], 3), "min": round(v[0], 3), "max": round(v[-1], 3)}
+        summary[lab] = {"ms_per_gib": ms, "digests": sorted({json.dumps(x["digest"], sort_keys=True) for x in rs})}
+    dec, emit = path_shares(ragged_sizes(GIB))
+    print(json.dumps({"gpu": info_before, "gpu_after": gpu_info(), "runs": a.runs, "builds": summary,
+                      "ragged_blocks": len(ragged_sizes(GIB)), "ragged_decode_stream_paths": dec, "ragged_emit_stream_groups": emit}))
+
+
+if __name__ == "__main__":
+    main()
