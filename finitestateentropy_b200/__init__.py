@@ -64,6 +64,9 @@ def _declare(L):
     sig("HUF_decompress", c_sz, c_vp, c_sz, c_vp, c_sz)
     sig("FSEB200_HUF_compress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     sig("FSEB200_HUF_decompress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    for codec in ("FSE", "FSEU16"):
+        sig("FSEB200_%s_compress_blocks" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
+        sig("FSEB200_%s_decompress_blocks" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     for name in ("FSEB200_HUF_compress_batch", "FSEB200_FSE_compress_batch", "FSEB200_FSE_decompress_batch",
                  "FSEB200_FSEU16_compress_batch", "FSEB200_FSEU16_decompress_batch"):
         if hasattr(L, name):
@@ -75,4 +78,5 @@ def _declare(L):
 
 from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch, fse_decompress_batch,  # noqa: E402,F401
                     fseu16_compress_batch, fseu16_decompress_batch, nblocks,
-                    huf_compress_blocks, huf_decompress_blocks, block_pointers)
+                    huf_compress_blocks, huf_decompress_blocks, block_pointers,
+                    fse_compress_blocks, fse_decompress_blocks, fseu16_compress_blocks, fseu16_decompress_blocks)

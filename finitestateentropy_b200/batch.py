@@ -4,8 +4,9 @@ Geometry is the one programs/bench.c:530-548 builds: a flat uncompressed buffer 
 `block_size` blocks (last one shorter), compressed block b in the fixed slot `cbuf[b*slot : (b+1)*slot]`,
 `csizes[b]` = the reference's return value for that block (0 = stored raw, 1 = RLE, error codes in-band).
 
-The `*_blocks` calls take per-block descriptors instead (FSEB200_HUF_*_blocks): int64 CUDA tensors of device addresses and
-sizes, one entry per block, so blocks of any size may sit anywhere -- e.g. packed back to back."""
+The `*_blocks` calls take per-block descriptors instead (FSEB200_{HUF,FSE,FSEU16}_*_blocks): int64 CUDA tensors of device
+addresses and sizes, one entry per block, so blocks of any size may sit anywhere -- e.g. packed back to back.  As in the
+reference's functions, the U16 calls count uncompressed sizes in 16-bit symbols (`block_pointers` gives bytes: halve them)."""
 import torch
 
 
@@ -134,3 +135,41 @@ def huf_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=No
                                             csrc_sizes.data_ptr(), _stream_ptr())
     _ret(r, "FSEB200_HUF_decompress_blocks")
     return results
+
+
+def _codec_blocks(fn_name, n_ptrs, arrays, out, extra=()):
+    from . import lib
+    if out is None:
+        out = torch.empty(n_ptrs.numel(), dtype=torch.int64, device=n_ptrs.device)
+    src_ptrs, src_sizes, dst_ptrs, dst_caps = arrays
+    n = _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, out)
+    r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), out.data_ptr(), src_ptrs.data_ptr(),
+                                src_sizes.data_ptr(), *extra, _stream_ptr())
+    _ret(r, fn_name)
+    return out
+
+
+def fse_compress_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes=None, max_symbol_value=255, table_log=12):
+    """FSE_compress2 on every block b: src_ptrs[b] / src_sizes[b] bytes into dst_ptrs[b] of capacity dst_caps[b], on the current
+    stream.  Returns csizes (int64; the reference's value per block, error codes as their two's-complement)."""
+    return _codec_blocks("FSEB200_FSE_compress_blocks", src_ptrs, (src_ptrs, src_sizes, dst_ptrs, dst_caps), csizes,
+                         (max_symbol_value, table_log))
+
+
+def fse_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_caps, results=None):
+    """FSE_decompress on every block b: csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of capacity dst_caps[b] bytes, on the
+    current stream.  Returns results (int64; regenerated size or error code per block)."""
+    return _codec_blocks("FSEB200_FSE_decompress_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_caps), results)
+
+
+def fseu16_compress_blocks(src_ptrs, src_symbols, dst_ptrs, dst_caps, csizes=None, max_symbol_value=0, table_log=12):
+    """FSE_compressU16 on every block b: src_symbols[b] 16-bit symbols at src_ptrs[b] (2-byte aligned) into dst_ptrs[b] of
+    dst_caps[b] bytes, on the current stream.  Returns csizes (int64, bytes or error codes)."""
+    return _codec_blocks("FSEB200_FSEU16_compress_blocks", src_ptrs, (src_ptrs, src_symbols, dst_ptrs, dst_caps), csizes,
+                         (max_symbol_value, table_log))
+
+
+def fseu16_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_symbols, results=None):
+    """FSE_decompressU16 on every block b: csrc_ptrs[b] / csrc_sizes[b] bytes into dst_ptrs[b] (2-byte aligned) of room for
+    dst_symbols[b] symbols, on the current stream.  Returns results (int64; regenerated symbols or error code per block)."""
+    return _codec_blocks("FSEB200_FSEU16_decompress_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_symbols), results)

@@ -3,7 +3,7 @@
 // Two tiers:
 //   1. FSEB200_*_batch : device-pointer, stream-ordered, whole-batch entry points -- what the
 //      per-chunk loops of the reference harness (programs/bench.c:353-364 and :389-424) collapse into.
-//      FSEB200_HUF_*_blocks: the same for Huff0 blocks given by per-block device descriptors (common.cuh BlockDescs).
+//      FSEB200_{HUF,FSE,FSEU16}_*_blocks: the same for blocks given by per-block device descriptors (common.cuh BlockDescs).
 //   2. the reference's own one-block-per-call symbols (lib/fse.h, lib/huf.h, lib/hist.h,
 //      lib/fseU16.h) with HOST pointers: they stage the block through a private device workspace and
 //      run the same kernels with a batch of one.  Correct drop-ins for unmodified callers; not the
@@ -29,6 +29,8 @@ cudaError_t launch_fse_decode(const BatchGeom&, void*, const void*, const u64*, 
 cudaError_t launch_fse_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fseu16_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t);
 cudaError_t launch_fseu16_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
+cudaError_t launch_fse_encode_blocks(const BlockDescs&, bool, unsigned, unsigned, cudaStream_t);
+cudaError_t launch_fse_decode_blocks(const BlockDescs&, bool, cudaStream_t);
 cudaError_t launch_hist(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_hist16(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_micro(int, const MicroArgs&, void*, u64*, cudaStream_t);
@@ -216,6 +218,38 @@ FSEB_API size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts
                                               const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
 {
     return huf_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, false, 0, 0, stream);
+}
+namespace {
+size_t fse_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCaps, size_t* dOut, const void* const* dSrcs, const size_t* dSrcSizes,
+                  bool wide, bool compress, unsigned msv, unsigned tlog, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || !dDsts || !dDstCaps || !dOut || !dSrcs || !dSrcSizes) return (size_t)err(E_SRC_WRONG);
+    BlockDescs g;
+    g.dst = (u8* const*)dDsts; g.dstCap = (const u64*)dDstCaps; g.result = (u64*)dOut;
+    g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes; g.nBlocks = (u32)nBlocks;
+    return ok_or_generic(compress ? launch_fse_encode_blocks(g, wide, msv, tlog, (cudaStream_t)stream) : launch_fse_decode_blocks(g, wide, (cudaStream_t)stream));
+}
+}
+FSEB_API size_t FSEB200_FSE_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                            const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return fse_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, false, true, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_FSE_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dResults,
+                                              const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
+{
+    return fse_blocks(nBlocks, dDsts, dDstCapacities, dResults, dCSrcs, dCSrcSizes, false, false, 0, 0, stream);
+}
+FSEB_API size_t FSEB200_FSEU16_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                               const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return fse_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, true, true, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_FSEU16_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dResults,
+                                                 const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
+{
+    return fse_blocks(nBlocks, dDsts, dDstCapacities, dResults, dCSrcs, dCSrcSizes, true, false, 0, 0, stream);
 }
 
 FSEB_API size_t FSEB200_batch_blocks(size_t total, size_t blockSize) { return blockSize ? (total + blockSize - 1) / blockSize : 0; }

@@ -117,4 +117,19 @@ __device__ __forceinline__ const u8* dec_orig(const BlockDescs&, const u8*, u32)
 __device__ __forceinline__ u64 dec_floor(const BatchGeom&, const u8* cbuf, const u8*) { return reinterpret_cast<u64>(cbuf) & ~31ull; }
 __device__ __forceinline__ u64 dec_floor(const BlockDescs&, const u8*, const u8* block) { return reinterpret_cast<u64>(block) & ~31ull; }
 
+// FSE and FSE-U16 blocks: the batch tier's limit is 2^30 bytes per source, capacity and compressed size (U16: 2^29 symbols).
+// The U16 descriptor calls count uncompressed sizes in 16-bit symbols, as FSE_compressU16 / FSE_decompressU16 do; fse_bytes
+// turns such a size into bytes and reports anything above the limit as FSE_BLOCK_MAX + 1, which the kernels answer with
+// srcSize_wrong.  The uncompressed length of a block, in bytes, through either geometry:
+constexpr u64 FSE_BLOCK_MAX = 1ull << 30;
+__device__ __forceinline__ u64 fse_bytes(u64 v, bool wide)
+{
+    if (wide) return v > FSE_BLOCK_MAX / 2 ? FSE_BLOCK_MAX + 1 : 2 * v;
+    return v > FSE_BLOCK_MAX ? FSE_BLOCK_MAX + 1 : v;
+}
+__device__ __forceinline__ u64 fse_enc_len(const BatchGeom& g, u32 b, bool) { return block_len(g, b); }
+__device__ __forceinline__ u64 fse_enc_len(const BlockDescs& g, u32 b, bool wide) { return fse_bytes(g.srcSize[b], wide); }
+__device__ __forceinline__ u64 fse_dec_len(const BatchGeom& g, u32 b, bool) { return block_len(g, b); }
+__device__ __forceinline__ u64 fse_dec_len(const BlockDescs& g, u32 b, bool wide) { return fse_bytes(g.dstCap[b], wide); }
+
 }  // namespace fseb

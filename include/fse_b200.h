@@ -12,8 +12,8 @@
  *   - tables are caller-owned `unsigned[]` with the reference's documented layouts and sizes
  *     (lib/fse.h:295-300, lib/huf.h:136-149).
  *
- * Tier 1 (FSEB200_*_batch) works on DEVICE memory and a CUDA stream, a whole batch per call; for Huff0,
- * FSEB200_HUF_*_blocks does the same for blocks of any size at any address, given by per-block device descriptors.
+ * Tier 1 (FSEB200_*_batch) works on DEVICE memory and a CUDA stream, a whole batch per call; FSEB200_{HUF,FSE,FSEU16}_*_blocks
+ * does the same for blocks of any size at any address, given by per-block device descriptors.
  * Tier 2 (the reference's own names) works on HOST memory, one block per synchronous call, and is
  * implemented by running the same kernels with a batch of one -- a correct drop-in for unmodified
  * callers (programs/bench.c, the fuzzers), not the fast path.
@@ -88,6 +88,40 @@ size_t FSEB200_HUF_compress_blocks(size_t nBlocks, void* const* dDsts, const siz
                                    unsigned maxSymbolValue, unsigned tableLog, void* stream);
 size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                      const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
+
+/* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
+ * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
+ * DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).
+ *   compress:   dCSizes[b] = exactly what FSE_compress2(dDsts[b], dDstCapacities[b], dSrcs[b], dSrcSizes[b], maxSymbolValue,
+ *               tableLog) (U16: FSE_compressU16) returns: 0, 1, a size or an error code; bytes [0, dCSizes[b]) are the
+ *               reference's.  Per-block verdicts come from the kernels: a bad maxSymbolValue / tableLog gives the reference's
+ *               error, and a capacity above 0xFFFFFF00 acts as 0xFFFFFF00.
+ *   decompress: dResults[b] = exactly what FSE_decompress(dDsts[b], dDstCapacities[b], dCSrcs[b], dCSrcSizes[b]) (U16:
+ *               FSE_decompressU16) returns, sizes taken literally: cSize 0 or 1 is corruption_detected (U16: cSize < 2 is
+ *               srcSize_wrong), not "stored", and an error code in dCSrcSizes is not passed through.  Bytes [0, result) are the
+ *               reference's.
+ * Units follow the reference's functions: for U16, dSrcSizes (compress), dDstCapacities and dResults (decompress) count 16-bit
+ * symbols; compressed sizes and capacities are always bytes.
+ * Limits, per block, as the one-block calls of this library: FSE sources, capacities and compressed sizes above 2^30 bytes
+ * give srcSize_wrong, and so do U16 blocks of more than 2^29 symbols.  A U16 block whose symbols sit at an odd address (the
+ * compress source, the decompress destination) gives GENERIC and nothing is written for it; compressed bytes may sit anywhere.
+ * Contract: no destination may overlap another destination, any source or the arrays (sources may overlap each other), and
+ * the output array (dCSizes / dResults) may not overlap the other arrays: the kernels read the sizes again after writing it.  Each
+ * compressed input must be readable up to the end of the 32-byte-aligned sector that holds its last byte (blocks packed back
+ * to back meet this when the buffer has 32 bytes of slack).  Bytes of [dst, dst + capacity) beyond the returned size are
+ * unspecified; nothing outside the destinations is written.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing); srcSize_wrong if nBlocks > 0xFFFFFFFF or an array is NULL
+ * while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_FSE_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                   const void* const* dSrcs, const size_t* dSrcSizes,
+                                   unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_FSE_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dResults,
+                                     const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
+size_t FSEB200_FSEU16_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                      const void* const* dSrcs, const size_t* dSrcSizes,
+                                      unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_FSEU16_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dResults,
+                                        const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
 
 /* Table reuse across blocks (lib/huf.h:191 per block; the shape programs/bench.c:610-633 and HUF_compress4X_repeat,
  * lib/huf_compress.c:664-712, reduce to when the previous table is kept): every block of the batch is coded with ONE
