@@ -4,7 +4,7 @@ Geometry is the one programs/bench.c:530-548 builds: a flat uncompressed buffer 
 `block_size` blocks (last one shorter), compressed block b in the fixed slot `cbuf[b*slot : (b+1)*slot]`,
 `csizes[b]` = the reference's return value for that block (0 = stored raw, 1 = RLE, error codes in-band).
 
-The `*_blocks` calls take per-block descriptors instead (FSEB200_{HUF,FSE,FSEU16}_*_blocks): int64 CUDA tensors of device
+The `*_blocks` calls take per-block descriptors instead (FSEB200_{HUF,HUF_*1X,FSE,FSEU16}_*_blocks): int64 CUDA tensors of device
 addresses and sizes, one entry per block, so blocks of any size may sit anywhere -- e.g. packed back to back.  As in the
 reference's functions, the U16 calls count uncompressed sizes in 16-bit symbols (`block_pointers` gives bytes: halve them)."""
 import torch
@@ -135,6 +135,20 @@ def huf_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=No
                                             csrc_sizes.data_ptr(), _stream_ptr())
     _ret(r, "FSEB200_HUF_decompress_blocks")
     return results
+
+
+def huf_compress1x_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes=None, max_symbol_value=255, table_log=12):
+    """HUF_compress1X (single-stream format) on every block b: src_ptrs[b] / src_sizes[b] into dst_ptrs[b] of capacity
+    dst_caps[b], on the current stream.  Returns csizes (int64; the reference's value per block, error codes as their
+    two's-complement)."""
+    return _codec_blocks("FSEB200_HUF_compress1X_blocks", src_ptrs, (src_ptrs, src_sizes, dst_ptrs, dst_caps), csizes,
+                         (max_symbol_value, table_log))
+
+
+def huf_decompress1x_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=None):
+    """HUF_decompress1X_DCtx (single-stream format) on every block b: csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of
+    dst_sizes[b] bytes, on the current stream.  Returns results (int64; regenerated size or error code per block)."""
+    return _codec_blocks("FSEB200_HUF_decompress1X_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes), results)
 
 
 def _codec_blocks(fn_name, n_ptrs, arrays, out, extra=()):

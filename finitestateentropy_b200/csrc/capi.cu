@@ -23,8 +23,8 @@ namespace fseb {
 cudaError_t launch_huf_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t, u32 flags);
 cudaError_t launch_huf_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_huf_encode_using_ctable(const BatchGeom&, void*, u64*, const void*, const u32*, cudaStream_t);
-cudaError_t launch_huf_encode_blocks(const BlockDescs&, unsigned, unsigned, cudaStream_t);
-cudaError_t launch_huf_decode_blocks(const BlockDescs&, cudaStream_t);
+cudaError_t launch_huf_encode_blocks(const BlockDescs&, int, unsigned, unsigned, cudaStream_t);
+cudaError_t launch_huf_decode_blocks(const BlockDescs&, int, cudaStream_t);
 cudaError_t launch_fse_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t);
 cudaError_t launch_fse_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fseu16_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t);
@@ -197,27 +197,39 @@ FSEB_API size_t FSEB200_HUF_compress4X_usingCTable_batch(void* dCBuf, size_t slo
 
 // Per-block descriptors (see common.cuh BlockDescs): every array and every buffer it points to is device memory, and the host never
 // reads them -- the per-block verdicts (sizes above a block, capacities, parameters) all come from the kernels.
+// nStreams: 4 for the 4X format (HUF_compress2 / HUF_decompress), 1 for the single-stream one (HUF_compress1X / HUF_decompress1X_DCtx).
 namespace {
 size_t huf_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dOut, const void* const* dSrcs, const size_t* dSrcSizes,
-                  bool compress, unsigned msv, unsigned tlog, void* stream)
+                  int nStreams, bool compress, unsigned msv, unsigned tlog, void* stream)
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || !dDsts || !dDstSizes || !dOut || !dSrcs || !dSrcSizes) return (size_t)err(E_SRC_WRONG);
     BlockDescs g;
     g.dst = (u8* const*)dDsts; g.dstCap = (const u64*)dDstSizes; g.result = (u64*)dOut;
     g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes; g.nBlocks = (u32)nBlocks;
-    return ok_or_generic(compress ? launch_huf_encode_blocks(g, msv, tlog, (cudaStream_t)stream) : launch_huf_decode_blocks(g, (cudaStream_t)stream));
+    return ok_or_generic(compress ? launch_huf_encode_blocks(g, nStreams, msv, tlog, (cudaStream_t)stream)
+                                  : launch_huf_decode_blocks(g, nStreams, (cudaStream_t)stream));
 }
 }
 FSEB_API size_t FSEB200_HUF_compress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
                                             const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
-    return huf_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, true, maxSymbolValue, tableLog, stream);
+    return huf_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, 4, true, maxSymbolValue, tableLog, stream);
 }
 FSEB_API size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                               const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
 {
-    return huf_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, false, 0, 0, stream);
+    return huf_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, 4, false, 0, 0, stream);
+}
+FSEB_API size_t FSEB200_HUF_compress1X_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                              const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, 1, true, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_HUF_decompress1X_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                                const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
+{
+    return huf_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, 1, false, 0, 0, stream);
 }
 namespace {
 size_t fse_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCaps, size_t* dOut, const void* const* dSrcs, const size_t* dSrcSizes,

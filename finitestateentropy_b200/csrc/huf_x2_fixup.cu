@@ -20,7 +20,8 @@ namespace hufx {
 
 constexpr int THREADS = 128;
 
-template <class Geo>
+// NS = streams per block of the batch: 4 (HUF_decompress) or 1 (HUF_decompress1X_DCtx)
+template <class Geo, int NS>
 __global__ void __launch_bounds__(THREADS)
 huf_x2_fixup_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, const u64* __restrict__ csizes, u64* __restrict__ results)
 {
@@ -53,7 +54,7 @@ huf_x2_fixup_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, co
             u64 r;
             if (is_err(h)) r = h;                                                   // :934
             else if (h >= cs) r = err(E_SRC_WRONG);                                 // :935
-            else r = cta_huf_decode<d_huf_decode_stream_x2>(true, s_dt, c + h, cs - h, dec_dst(g, dst, bb), n, s_init, s_done);
+            else r = cta_huf_decode<d_huf_decode_stream_x2>(NS == 4, s_dt, c + h, cs - h, dec_dst(g, dst, bb), n, s_init, s_done);
             if (tid == 0) dec_out(g, results, bb) = r;
             __syncthreads();
         }
@@ -63,26 +64,27 @@ huf_x2_fixup_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, co
 }  // namespace hufx
 
 namespace {
-template <class Geo>
+template <class Geo, int NS>
 cudaError_t huf_x2_fixup(const Geo& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream)
 {
     if (g.nBlocks == 0) return cudaSuccess;
     unsigned grid = 2u * (unsigned)device_sm_count(current_device());
     unsigned const need = (g.nBlocks + hufx::THREADS - 1) / hufx::THREADS;
     if (grid > need) grid = need;
-    hufx::huf_x2_fixup_kernel<Geo><<<grid, hufx::THREADS, 0, stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results);
+    hufx::huf_x2_fixup_kernel<Geo, NS><<<grid, hufx::THREADS, 0, stream>>>(g, (u8*)dst, (const u8*)cbuf, csizes, results);
     return cudaGetLastError();
 }
 }  // namespace
 
 cudaError_t launch_huf_x2_fixup(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream)
 {
-    return huf_x2_fixup(g, dst, cbuf, csizes, results, stream);
+    return huf_x2_fixup<BatchGeom, 4>(g, dst, cbuf, csizes, results, stream);
 }
 
-cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, cudaStream_t stream)
+cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream)
 {
-    return huf_x2_fixup(g, nullptr, nullptr, nullptr, nullptr, stream);
+    return nStreams == 1 ? huf_x2_fixup<BlockDescs, 1>(g, nullptr, nullptr, nullptr, nullptr, stream)
+                         : huf_x2_fixup<BlockDescs, 4>(g, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 }  // namespace fseb

@@ -89,6 +89,26 @@ size_t FSEB200_HUF_compress_blocks(size_t nBlocks, void* const* dDsts, const siz
 size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                      const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
 
+/* Tier 1, per-block descriptors (single-stream Huff0, the "1X" format of lib/huf.h:288-335: tree header + one bitstream, no
+ * jump table) -- e.g. the small literal sections a zstd-style caller codes as one stream.  Argument shape, asynchrony,
+ * contract and return value are those of FSEB200_HUF_{compress,decompress}_blocks above; every block builds and carries its
+ * own table.
+ *   compress:   dCSizes[b] = exactly what HUF_compress1X(dDsts[b], dDstCapacities[b], dSrcs[b], dSrcSizes[b], maxSymbolValue,
+ *               tableLog) returns: 0, 1 (the byte in dDsts[b][0]), a size or an error code; bytes [0, dCSizes[b]) are the
+ *               reference's.  srcSize > 128 KB gives srcSize_wrong, a bad maxSymbolValue / tableLog the reference's error, and
+ *               a capacity above 2^32 acts as 0xFFFFFF00.
+ *   decompress: dResults[b] = exactly what HUF_decompress1X_DCtx(dctx, dDsts[b], dDstSizes[b], dCSrcs[b], dCSrcSizes[b])
+ *               returns for a fresh HUF_CREATE_STATIC_DTABLEX2(dctx, HUF_TABLELOG_MAX), sizes taken literally: dstSize 0
+ *               gives dstSize_tooSmall, cSize > dstSize corruption_detected, cSize == dstSize is a raw copy, cSize == 1 RLE,
+ *               anything else is decoded with the decoder (and verdict on malformed input) HUF_selectDecoder picks.
+ *               Deviation: the reference's 1X decoder has no block-size limit; here dstSize > 128 KB gives srcSize_wrong,
+ *               as in FSEB200_HUF_decompress_blocks. */
+size_t FSEB200_HUF_compress1X_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                     const void* const* dSrcs, const size_t* dSrcSizes,
+                                     unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_decompress1X_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                       const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
+
 /* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
  * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
  * DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).

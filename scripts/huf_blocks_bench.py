@@ -5,6 +5,13 @@
   (b) ragged layout  the same stream cut into seeded sizes uniform in [1 KiB, 128 KiB], sources back to back: encode into
                      bound-sized destinations, then decode from the compressed blocks packed back to back (packed outside the
                      timed region) into outputs back to back.  Also the share of streams per decode path and emit path.
+  (c) small layout   the first 256 MiB of the stream cut into seeded sizes uniform in [64 B, 4 KiB], as (b).
+
+A build with the single-stream descriptor calls (FSEB200_HUF_*1X_blocks) is also timed with them: a1_* in layout (a), b1_* in
+(b), c1_* in (c), next to the 4X descriptor calls of the same run (c_* is 4X in layout (c)).  Layouts (b) and (c) decode only
+the blocks that compressed to a Huffman block (1 < cSize < size); every figure is scaled to ms per GiB of uncompressed bytes
+that the call encodes or decodes.  `cpu_ref` is the compiled reference's single-thread HUF_compress1X / HUF_decompress1X_DCtx
+on a sample of layout (a) (oracle/_ref/libfse_ref.so, skipped when it is absent), in the same units.
 
 Builds are libraries given as LABEL=PATH (default: this tree's).  Each run of each build is a child process; builds alternate
 run by run.  Prints one JSON line with the GPU's name, power limit and SM clock, per build and metric the median and range in
@@ -37,16 +44,18 @@ def declare(L):
     L.FSEB200_HUF_compress_batch.restype = sz; L.FSEB200_HUF_compress_batch.argtypes = [vp, sz, vp, vp, sz, sz, u, u, vp]
     L.FSEB200_HUF_decompress_batch.restype = sz; L.FSEB200_HUF_decompress_batch.argtypes = [vp, sz, sz, vp, sz, vp, vp, vp, vp]
     have = hasattr(L, "FSEB200_HUF_compress_blocks")
-    if have:
-        L.FSEB200_HUF_compress_blocks.restype = sz; L.FSEB200_HUF_compress_blocks.argtypes = [sz, vp, vp, vp, vp, vp, u, u, vp]
-        L.FSEB200_HUF_decompress_blocks.restype = sz; L.FSEB200_HUF_decompress_blocks.argtypes = [sz, vp, vp, vp, vp, vp, vp]
-    return have
+    have1x = hasattr(L, "FSEB200_HUF_compress1X_blocks")
+    for suffix, present in (("", have), ("1X", have1x)):
+        if present:
+            f = getattr(L, "FSEB200_HUF_compress%s_blocks" % suffix); f.restype = sz; f.argtypes = [sz, vp, vp, vp, vp, vp, u, u, vp]
+            f = getattr(L, "FSEB200_HUF_decompress%s_blocks" % suffix); f.restype = sz; f.argtypes = [sz, vp, vp, vp, vp, vp, vp]
+    return have, have1x
 
 
-def ragged_sizes(total, seed=7):
+def ragged_sizes(total, seed=7, lo=1024, hi=128 * 1024):
     import numpy as np
     rng = np.random.default_rng(seed)
-    sizes = rng.integers(1024, 128 * 1024 + 1, total // 1024)
+    sizes = rng.integers(lo, hi + 1, total // lo)
     ends = np.cumsum(sizes)
     k = int(np.searchsorted(ends, total))
     sizes = sizes[: k + 1].copy()
@@ -68,11 +77,40 @@ def path_shares(sizes):
     return {k: round(v / nd, 4) for k, v in dec.items()}, {k: round(v / ne, 4) for k, v in emit.items()}
 
 
+def cpu_ref_rates(src_host, nblocks):
+    """the compiled reference's single-thread HUF_compress1X / HUF_decompress1X_DCtx on the first nblocks 32 KB blocks: ms per GiB"""
+    import time
+    import numpy as np
+    path = os.path.join(ROOT, "oracle", "_ref", "libfse_ref.so")
+    if not os.path.exists(path):
+        return None
+    R = C.CDLL(path)
+    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
+    R.HUF_compress1X.restype = sz; R.HUF_compress1X.argtypes = [vp, sz, vp, sz, u, u]
+    R.HUF_decompress1X_DCtx.restype = sz; R.HUF_decompress1X_DCtx.argtypes = [vp, vp, sz, vp, sz]
+    bound = 129 + BLOCK + (BLOCK >> 8) + 8
+    cbuf = np.zeros(nblocks * bound + 64, np.uint8)
+    out = np.zeros(BLOCK + 64, np.uint8)
+    dt = np.zeros(1 + 4096, np.uint32)
+    p = lambda a, o=0: a.ctypes.data + o
+    sizes = []
+    t0 = time.perf_counter()
+    for b in range(nblocks):
+        sizes.append(R.HUF_compress1X(p(cbuf, b * bound), bound, p(src_host, b * BLOCK), BLOCK, 255, 12))
+    t1 = time.perf_counter()
+    for b in range(nblocks):
+        dt[0] = 12 * 0x01000001
+        assert R.HUF_decompress1X_DCtx(p(dt), p(out), BLOCK, p(cbuf, b * bound), sizes[b]) == BLOCK
+    t2 = time.perf_counter()
+    scale = GIB / (nblocks * BLOCK) * 1e3
+    return {"enc1x": round((t1 - t0) * scale, 1), "dec1x": round((t2 - t1) * scale, 1), "sample_blocks": nblocks}
+
+
 def child(lib_path, reps):
     import numpy as np
     import torch
     L = C.CDLL(lib_path)
-    have = declare(L)
+    have, have1x = declare(L)
     dev = torch.device("cuda")
     stream = torch.cuda.current_stream().cuda_stream
     slot = 512 + BLOCK + (BLOCK >> 7) + 12
@@ -114,33 +152,59 @@ def child(lib_path, reps):
         dst.zero_()
         out["a_dec_blocks"] = timed(lambda: L.FSEB200_HUF_decompress_blocks(nb, op.data_ptr(), sn.data_ptr(), res.data_ptr(), dp.data_ptr(), cs2.data_ptr(), stream))
         assert torch.equal(dst, src[:GIB]) and bool((res == BLOCK).all())
-        # (b) ragged
-        sizes = ragged_sizes(GIB)
-        n = len(sizes)
-        offs = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
-        bounds = np.array([129 + s + (s >> 8) + 8 for s in sizes], np.int64)
-        boffs = np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64)
+        if have1x:                                                      # (a) in the single-stream format, into the same slots
+            cs1 = torch.empty_like(cs)
+            out["a1_enc"] = timed(lambda: L.FSEB200_HUF_compress1X_blocks(nb, dp.data_ptr(), dc.data_ptr(), cs1.data_ptr(), sp.data_ptr(), sn.data_ptr(), 255, 12, stream))
+            assert bool(((cs1 > 1) & (cs1 < BLOCK)).all())
+            used = torch.arange(slot, device=dev)[None, :] < cs1[:, None]
+            digest["a1_cbuf"] = hashlib.sha256(cbuf[: nb * slot].view(nb, slot)[used].cpu().numpy().tobytes()).hexdigest()[:16]
+            del used
+            dst.zero_()
+            out["a1_dec"] = timed(lambda: L.FSEB200_HUF_decompress1X_blocks(nb, op.data_ptr(), sn.data_ptr(), res.data_ptr(), dp.data_ptr(), cs1.data_ptr(), stream))
+            assert torch.equal(dst, src[:GIB]) and bool((res == BLOCK).all())
         del cbuf
-        carena = torch.empty(int(bounds.sum()) + 64, dtype=torch.uint8, device=dev)
-        rsp, rsn = t64(src.data_ptr() + offs), t64(sizes)
-        rdp, rdc = t64(carena.data_ptr() + boffs), t64(bounds)
-        rcs = torch.empty(n, dtype=torch.int64, device=dev)
-        out["b_enc"] = timed(lambda: L.FSEB200_HUF_compress_blocks(n, rdp.data_ptr(), rdc.data_ptr(), rcs.data_ptr(), rsp.data_ptr(), rsn.data_ptr(), 255, 12, stream))
-        csz = rcs.cpu().numpy()
-        assert (csz > 1).all() and (csz < np.array(sizes)).all()
-        poffs = np.concatenate([[0], np.cumsum(csz)[:-1]]).astype(np.int64)
-        packed = torch.empty(int(csz.sum()) + 64, dtype=torch.uint8, device=dev)
-        for i in range(n):                                              # packing: outside the timed region
-            packed[poffs[i]: poffs[i] + csz[i]].copy_(carena[boffs[i]: boffs[i] + csz[i]])
-        del carena
-        digest["b_packed"] = hashlib.sha256(packed[: int(csz.sum())].cpu().numpy().tobytes()).hexdigest()[:16]
-        pp = t64(packed.data_ptr() + poffs)
-        od = t64(dst.data_ptr() + offs)
-        rres = torch.empty(n, dtype=torch.int64, device=dev)
-        dst.zero_()
-        out["b_dec"] = timed(lambda: L.FSEB200_HUF_decompress_blocks(n, od.data_ptr(), rsn.data_ptr(), rres.data_ptr(), pp.data_ptr(), rcs.data_ptr(), stream))
-        assert torch.equal(dst, src[:GIB]) and torch.equal(rres, rsn)
-        out["b_blocks"] = n
+
+        def ragged(key, enc, dec, sizes):
+            """encode blocks back to back into bound-sized destinations, pack the Huffman blocks back to back, decode them"""
+            n = len(sizes)
+            total = int(sum(sizes))
+            offs = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
+            bounds = np.array([129 + s + (s >> 8) + 8 for s in sizes], np.int64)
+            boffs = np.concatenate([[0], np.cumsum(bounds)[:-1]]).astype(np.int64)
+            carena = torch.empty(int(bounds.sum()) + 64, dtype=torch.uint8, device=dev)
+            rsp, rsn = t64(src.data_ptr() + offs), t64(sizes)
+            rdp, rdc = t64(carena.data_ptr() + boffs), t64(bounds)
+            rcs = torch.empty(n, dtype=torch.int64, device=dev)
+            out[key + "_enc"] = timed(lambda: enc(n, rdp.data_ptr(), rdc.data_ptr(), rcs.data_ptr(), rsp.data_ptr(), rsn.data_ptr(), 255, 12, stream)) * GIB / total
+            csz = rcs.cpu().numpy()
+            sz_np = np.array(sizes, np.int64)
+            keep = np.nonzero((csz > 1) & (csz < sz_np))[0]             # Huffman blocks (error codes are huge as u64, negative here)
+            kc, kn = csz[keep], sz_np[keep]
+            poffs = np.concatenate([[0], np.cumsum(kc)[:-1]]).astype(np.int64)
+            src_idx = torch.repeat_interleave(t64(boffs[keep] - poffs), t64(kc)) + torch.arange(int(kc.sum()), device=dev)
+            packed = torch.empty(int(kc.sum()) + 64, dtype=torch.uint8, device=dev)
+            packed[: int(kc.sum())] = carena[src_idx]                   # packing: outside the timed region
+            del carena, src_idx
+            digest[key + "_packed"] = hashlib.sha256(packed[: int(kc.sum())].cpu().numpy().tobytes()).hexdigest()[:16]
+            pp, pcs = t64(packed.data_ptr() + poffs), t64(kc)
+            od, on = t64(dst.data_ptr() + offs[keep]), t64(kn)
+            rres = torch.empty(len(keep), dtype=torch.int64, device=dev)
+            dst.zero_()
+            out[key + "_dec"] = timed(lambda: dec(len(keep), od.data_ptr(), on.data_ptr(), rres.data_ptr(), pp.data_ptr(), pcs.data_ptr(), stream)) * GIB / int(kn.sum())
+            assert torch.equal(rres, on)
+            ok = torch.zeros(GIB, dtype=torch.bool, device=dev)
+            ok[torch.repeat_interleave(t64(offs[keep]), t64(kn)) + torch.arange(int(kn.sum()), device=dev) - torch.repeat_interleave(t64(np.concatenate([[0], np.cumsum(kn)[:-1]])), t64(kn))] = True
+            assert torch.equal(dst[ok], src[:GIB][ok])
+            out[key + "_count"] = n
+            out[key + "_huffman_share"] = round(float(kn.sum()) / total, 4)
+
+        layouts = {"b": ragged_sizes(GIB), "c": ragged_sizes(GIB // 4, seed=9, lo=64, hi=4096)}
+        for lay, sizes in layouts.items():
+            ragged(lay, L.FSEB200_HUF_compress_blocks, L.FSEB200_HUF_decompress_blocks, sizes)
+            if have1x:
+                ragged(lay + "1", L.FSEB200_HUF_compress1X_blocks, L.FSEB200_HUF_decompress1X_blocks, sizes)
+        if have1x:
+            out["cpu_ref"] = cpu_ref_rates(src[: 512 * BLOCK].cpu().numpy(), 512)
     print(json.dumps({"ms": out, "digest": digest}))
 
 
@@ -180,11 +244,16 @@ def main():
                                capture_output=True, text=True)
             assert r.returncode == 0, (lab, r.stderr[-3000:])
             runs[lab].append(json.loads(r.stdout.strip().splitlines()[-1]))
+            print(lab, r.stdout.strip().splitlines()[-1], file=sys.stderr)   # every run's raw figures
     summary = {}
     for lab, rs in runs.items():
         ms = {}
         for k in rs[0]["ms"]:
-            if k == "b_blocks":
+            if k.endswith("_count") or k.endswith("_share"):                 # block counts and Huffman shares: the same every run
+                ms[k] = rs[0]["ms"][k]
+                continue
+            if k == "cpu_ref":                                              # medians of the reference's rates
+                ms[k] = rs[0]["ms"][k] and {m: sorted(x["ms"][k][m] for x in rs)[len(rs) // 2] for m in rs[0]["ms"][k]}
                 continue
             v = sorted(x["ms"][k] for x in rs)                           # per GiB: every layout moves 1 GiB uncompressed
             ms[k] = {"median": round(v[len(v) // 2], 3), "min": round(v[0], 3), "max": round(v[-1], 3)}
