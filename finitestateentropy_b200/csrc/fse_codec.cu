@@ -491,8 +491,15 @@ __device__ inline bool warp_encode_front(const EncFront<WIDE>& w, const typename
     if (!WIDE) {
         if (tl > FSE_MAX_TLOG) FRONT_DONE(err(E_TLOG_TOO_LARGE));
         if (tl == 0) FRONT_DONE(err(E_TLOG_TOO_LARGE));               // FSE_WKSP_SIZE_U32(0,..) shifts by -1: the reference (gcc/x86-64) reports tableLog_tooLarge
-        if ((u64)14340 < (u64)1 + (1ull << (tl - 1)) + ((u64)msv + 1) * 2 + 1024) FRONT_DONE(err(E_TLOG_TOO_LARGE));   // :645 vs the stack workspace of :679-685
+        // :645 vs the stack workspace of :679-685.  FSE_WKSP_SIZE_U32 is unsigned 32-bit arithmetic: (msv + 1) * 2 wraps, so
+        // maxSymbolValue 2^32-1 (and 2^31-1) passes the test and compresses as 255
+        u32 const ctWords = 1u + (1u << (tl - 1)) + (msv + 1u) * 2u;  // FSE_CTABLE_SIZE_U32 of the request (:641)
+        if (14340u < ctWords + 1024u) FRONT_DONE(err(E_TLOG_TOO_LARGE));
         if (n <= 1) FRONT_DONE(0);
+        // the scratch after that CTable (:642-643) is 14340 - 4 * ctWords bytes; HIST_count_wksp refuses less than 4096 of it
+        // (hist.c:168).  When the CTable alone exceeds the workspace the size wraps and the reference runs past its stack:
+        // those requests are answered as at maxSymbolValue 255.
+        if (4ull * ctWords <= 14340u && 14340u - 4ull * ctWords < 4096u) FRONT_DONE(err(E_WKSP_TOO_SMALL));
         if (!msv) msv = FSE_MAX_SV;
         if (msv > FSE_MAX_SV) msv = FSE_MAX_SV;                      // HIST_count_wksp clamps (hist.c:171)
     } else {

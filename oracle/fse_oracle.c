@@ -9,11 +9,11 @@
  * Known, documented deviations (all on inputs the reference itself treats as unsupported):
  *   - orc_huf_decode4x1 refuses dstSize < 6 (the reference would write 1 byte out of bounds,
  *     lib/huf_decompress.c:291-296,344-347); HUF_compress never emits such blocks (:565).
- *   - orc_fse_compress2 builds its CTable in private storage.  FSE_compress_wksp sizes CTable+scratch
- *     from the *requested* tableLog (lib/fse_compress.c:641-643) but builds with the one
- *     FSE_optimalTableLog returns (:658,667); for requests of 5..9 on large alphabets the latter is
- *     larger and table and scratch overlap (corrupted stream).  Requests >= 10 (bench.c uses 12,
- *     FSE_compress 11) never alias and are reproduced bit-exactly.
+ *   - orc_fse_compress2 builds its CTable in private storage.  FSE_compress_wksp lays CTable+scratch
+ *     out for the *requested* tableLog and maxSymbolValue (lib/fse_compress.c:641-643) but builds with
+ *     the tableLog FSE_optimalTableLog returns (:658,667); the reference's call can fault on raised
+ *     requests and where the requested CTable alone exceeds its workspace.  Those are answered as the
+ *     same steps done one reference function at a time answer them (tests/table_logs.py:fse_steps).
  *   - orc_fse_decompress_u16 returns `corruption` for an empty payload where the reference
  *     dereferences a NULL stream pointer (lib/fseU16.c:286-287 with lib/bitstream.h:274).
  *
@@ -589,8 +589,15 @@ size_t orc_fse_compress2(void* dst, size_t cap, const void* src, size_t n, unsig
     if (tl > FSE_MAX_TLOG) return ORC_ERROR(ORC_TLOG_TOO_LARGE);
     /* :645 -- FSE_WKSP_SIZE_U32(tl,msv) (lib/fse.h:314) against the 14,340-byte stack workspace of :679-685 */
     if (tl == 0) return ORC_ERROR(ORC_TLOG_TOO_LARGE);   /* the same macro shifts by (0-1): as built (gcc, x86-64) the reference reports tableLog_tooLarge */
-    if ((size_t)14340 < (size_t)1 + ((size_t)1 << (tl - 1)) + ((size_t)msv + 1) * 2 + 1024) return ORC_ERROR(ORC_TLOG_TOO_LARGE);
-    if (n <= 1) return 0;
+    /* the macro is unsigned 32-bit arithmetic: (msv + 1) * 2 wraps, so msv 2^32-1 (and 2^31-1) passes and compresses as 255 */
+    {   u32 const ctWords = 1u + (1u << (tl - 1)) + (msv + 1u) * 2u;   /* FSE_CTABLE_SIZE_U32 of the request (:641) */
+        if (14340u < ctWords + 1024u) return ORC_ERROR(ORC_TLOG_TOO_LARGE);
+        if (n <= 1) return 0;
+        /* :642-643 -- the scratch after that CTable is 14340 - 4*ctWords bytes; HIST_count_wksp refuses less than 4096
+         * (hist.c:168).  Where the CTable alone exceeds the workspace the size wraps and the reference runs past its
+         * stack; those requests are answered as at msv 255. */
+        if (4ull * ctWords <= 14340u && 14340u - 4ull * ctWords < 4096u) return ORC_ERROR(ORC_WKSP_TOO_SMALL);
+    }
     if (!msv) msv = FSE_MAX_SV;
     if (!tl) tl = FSE_DEF_TLOG;
     r = orc_hist_count(count, &msv, src, n);
