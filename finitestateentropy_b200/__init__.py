@@ -66,6 +66,8 @@ def _declare(L):
     sig("FSEB200_HUF_decompress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     sig("FSEB200_HUF_compress1X_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     sig("FSEB200_HUF_decompress1X_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    for name in ("FSEB200_HUF_compress_packed", "FSEB200_HUF_compress1X_packed"):
+        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     for codec in ("FSE", "FSEU16"):
         sig("FSEB200_%s_compress_blocks" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
         sig("FSEB200_%s_decompress_blocks" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
@@ -82,4 +84,5 @@ from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch
                     fseu16_compress_batch, fseu16_decompress_batch, nblocks,
                     huf_compress_blocks, huf_decompress_blocks, block_pointers,
                     huf_compress1x_blocks, huf_decompress1x_blocks,
+                    huf_compress_packed, huf_compress1x_packed, packed_pointers,
                     fse_compress_blocks, fse_decompress_blocks, fseu16_compress_blocks, fseu16_decompress_blocks)

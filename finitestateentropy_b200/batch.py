@@ -151,6 +151,45 @@ def huf_decompress1x_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=
     return _codec_blocks("FSEB200_HUF_decompress1X_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes), results)
 
 
+def huf_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, max_symbol_value=255, table_log=12):
+    """HUF_compress2 on every block b (src_ptrs[b] / src_sizes[b]) at capacity HUF_compressBound, the results stored back to
+    back in `out` (capacity out.numel()), on the current stream.  Returns (out, offsets, csizes): offsets (int64, n + 1 entries)
+    is the prefix sum of the stored lengths, csizes the reference's value per block (dstSize_tooSmall for a block that does not
+    fit `out`).  With out=None, `out` is allocated at sum(src_sizes) + 32 bytes, always enough: reading that sum costs one host
+    synchronisation.  `packed_pointers(out, offsets)` gives the arrays huf_decompress_blocks decodes the buffer with."""
+    return _compress_packed("FSEB200_HUF_compress_packed", src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log)
+
+
+def huf_compress1x_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, max_symbol_value=255, table_log=12):
+    """huf_compress_packed in the single-stream format (HUF_compress1X per block); decode with huf_decompress1x_blocks"""
+    return _compress_packed("FSEB200_HUF_compress1X_packed", src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log)
+
+
+def _compress_packed(fn_name, src_ptrs, src_sizes, out, offsets, csizes, msv, tlog):
+    from . import lib
+    n = _blocks_args(src_ptrs, src_sizes)
+    dev = src_ptrs.device
+    if out is None:
+        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
+    if offsets is None:
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64)
+    assert offsets.numel() == n + 1 and csizes.numel() == n and out.device == dev, (offsets.numel(), csizes.numel(), n)
+    r = getattr(lib(), fn_name)(n, out.data_ptr(), out.numel(), offsets.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
+                                src_sizes.data_ptr(), msv, tlog, _stream_ptr())
+    _ret(r, fn_name)
+    return out, offsets, csizes
+
+
+def packed_pointers(out, offsets):
+    """(ptrs, sizes) of the blocks of a packed buffer: int64 device addresses out + offsets[b] and stored lengths
+    offsets[b + 1] - offsets[b], the compressed-source arrays of huf_decompress_blocks / huf_decompress1x_blocks"""
+    _check(offsets, torch.int64)
+    return offsets[:-1] + out.data_ptr(), offsets[1:] - offsets[:-1]
+
+
 def _codec_blocks(fn_name, n_ptrs, arrays, out, extra=()):
     from . import lib
     if out is None:

@@ -24,6 +24,7 @@ cudaError_t launch_huf_decode(const BatchGeom&, void*, const void*, const u64*, 
 cudaError_t launch_huf_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_huf_encode_using_ctable(const BatchGeom&, void*, u64*, const void*, const u32*, cudaStream_t);
 cudaError_t launch_huf_encode_blocks(const BlockDescs&, int, unsigned, unsigned, cudaStream_t);
+cudaError_t launch_huf_encode_packed(const PackedDescs&, int, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_huf_decode_blocks(const BlockDescs&, int, cudaStream_t);
 cudaError_t launch_fse_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t);
 cudaError_t launch_fse_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
@@ -230,6 +231,29 @@ FSEB_API size_t FSEB200_HUF_decompress1X_blocks(size_t nBlocks, void* const* dDs
                                                 const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
 {
     return huf_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, 1, false, 0, 0, stream);
+}
+// Packed output: the descriptor compress with every block stored back to back in one buffer (common.cuh PackedDescs).
+namespace {
+size_t huf_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes, const void* const* dSrcs,
+                  const size_t* dSrcSizes, int nStreams, unsigned msv, unsigned tlog, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || !dOut || !dOffsets || !dCSizes || !dSrcs || !dSrcSizes) return (size_t)err(E_SRC_WRONG);
+    PackedDescs g;
+    g.out = (u8*)dOut; g.outCap = outCapacity; g.offset = (u64*)dOffsets; g.result = (u64*)dCSizes;
+    g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes; g.nBlocks = (u32)nBlocks;
+    return ok_or_generic(launch_huf_encode_packed(g, nStreams, msv, tlog, (cudaStream_t)stream));
+}
+}
+FSEB_API size_t FSEB200_HUF_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                            const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_packed(nBlocks, dOut, outCapacity, dOffsets, dCSizes, dSrcs, dSrcSizes, 4, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_HUF_compress1X_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                              const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_packed(nBlocks, dOut, outCapacity, dOffsets, dCSizes, dSrcs, dSrcSizes, 1, maxSymbolValue, tableLog, stream);
 }
 namespace {
 size_t fse_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCaps, size_t* dOut, const void* const* dSrcs, const size_t* dSrcSizes,

@@ -81,6 +81,32 @@ __host__ __forceinline__ BlockDescs slice(const BlockDescs& g, u32 b0, u32 n)   
     return s;
 }
 
+// -------------------------------------------------------------------------------------------
+// Packed geometry (Huff0 compress only): sources by descriptor, outputs back to back in one buffer.  Block b is stored at
+// out + offset[b], offset[] being the exclusive prefix sum of the stored lengths (include/fse_b200.h); its capacity is
+// HUF_compressBound(srcSize), so its verdict is that of the reference at that capacity.  `offset` has nBlocks + 1 entries;
+// a slice keeps `out` and shifts `offset`, so offset[0] of a slice is the running total of the blocks before it.
+// -------------------------------------------------------------------------------------------
+struct PackedDescs {
+    static constexpr bool DESCS = true;
+    u8* out;
+    u64 outCap;
+    u64* offset;
+    u64* result;
+    const u8* const* src;
+    const u64* srcSize;
+    u32 nBlocks;
+};
+__host__ __forceinline__ PackedDescs slice(const PackedDescs& g, u32 b0, u32 n)
+{
+    PackedDescs s = g;
+    s.offset += b0; s.result += b0; s.src += b0; s.srcSize += b0; s.nBlocks = n;
+    return s;
+}
+// bytes a block takes in the packed output, from its compress verdict: the compressed size, the RLE byte, a raw copy of the
+// source when the verdict is 0 (0 bytes for an empty block), nothing for an error
+__host__ __device__ __forceinline__ u64 packed_len(u64 v, u64 n) { return is_err(v) ? 0 : (v ? v : n); }
+
 // The Huff0 kernels locate a block only through these accessors, one set per geometry.  The uniform geometry's pointer
 // arguments are the batch's buffers; the descriptor geometry ignores them (its launchers pass nullptr).
 // A size above what any Huff0 block can have is reported as HUF_BLOCK_MAX + 1: every verdict the kernels derive from it
@@ -98,6 +124,12 @@ __device__ __forceinline__ u32 enc_len(const BlockDescs& g, u32 b) { return clam
 __device__ __forceinline__ u8* enc_dst(const BlockDescs& g, u8*, u32 b) { return g.dst[b]; }
 __device__ __forceinline__ u64 enc_cap(const BlockDescs& g, u32 b) { u64 const c = g.dstCap[b]; return c > 0xFFFFFF00ull ? 0xFFFFFF00ull : c; }   // as one_block_compress
 __device__ __forceinline__ u64& enc_out(const BlockDescs& g, u64*, u32 b) { return g.result[b]; }
+// packed: enc_dst is valid only once the placement kernel has written offset[b] (the emit kernel's use)
+__device__ __forceinline__ const u8* enc_src(const PackedDescs& g, const u8*, u32 b) { return g.src[b]; }
+__device__ __forceinline__ u32 enc_len(const PackedDescs& g, u32 b) { return clamp_len(g.srcSize[b]); }
+__device__ __forceinline__ u8* enc_dst(const PackedDescs& g, u8*, u32 b) { return g.out + g.offset[b]; }
+__device__ __forceinline__ u64 enc_cap(const PackedDescs& g, u32 b) { u64 const n = enc_len(g, b); return 129 + n + (n >> 8) + 8; }   // HUF_compressBound
+__device__ __forceinline__ u64& enc_out(const PackedDescs& g, u64*, u32 b) { return g.result[b]; }
 
 // decoder: compressed source, its size, the output, the regenerated size, the result; `orig` (stored blocks) is uniform-only
 __device__ __forceinline__ const u8* dec_src(const BatchGeom& g, const u8* cbuf, u32 b) { return cbuf + (u64)b * g.slot; }

@@ -109,6 +109,36 @@ size_t FSEB200_HUF_compress1X_blocks(size_t nBlocks, void* const* dDsts, const s
 size_t FSEB200_HUF_decompress1X_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                        const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
 
+/* Tier 1, per-block descriptors with packed output (Huff0, 4X and 1X): the blocks given by dSrcs / dSrcSizes are compressed and
+ * stored back to back in one buffer, each at an offset the call computes on the device -- no per-block reservation, no
+ * compaction pass, and the stream decodes with the descriptor decoders above.  Per block b, with n = dSrcSizes[b]:
+ *   dCSizes[b]  = exactly what HUF_compress2(dst, HUF_compressBound(n), src, n, maxSymbolValue, tableLog) returns (the 1X call:
+ *                 HUF_compress1X): 0, 1, a size or an error code -- except for a block that does not fit (below).
+ *   stored length L[b]: dCSizes[b] >= 2: dCSizes[b], the reference's compressed bytes; 1: 1, the byte src[0] (RLE); 0: n, a raw
+ *                 copy of the source (0 bytes for an empty block); an error code: 0, nothing stored.
+ *                 L[b] <= n always (a compressed block is shorter than n - 1 bytes, lib/huf_compress.c:625), so an outCapacity
+ *                 of sum(n) always holds every block; add 32 bytes of slack for the decoders' sector reads.
+ *   dOffsets    has nBlocks + 1 entries: dOffsets[b] = L[0] + ... + L[b-1], dOffsets[nBlocks] = the total.  It is written in
+ *                 full even when blocks do not fit, so a too-small call still tells the size it needs.
+ *   capacity    block b is stored at dOut + dOffsets[b] only if dOffsets[b] + L[b] <= outCapacity; otherwise dCSizes[b] =
+ *                 dstSize_tooSmall and nothing is written for it (a block whose value is an error code keeps it).  Nothing
+ *                 outside [dOut, dOut + min(total, outCapacity)) is ever written.
+ * Decoding: FSEB200_HUF_decompress_blocks (1X: FSEB200_HUF_decompress1X_blocks) with dCSrcs[b] = dOut + dOffsets[b],
+ * dCSrcSizes[b] = L[b] = dOffsets[b+1] - dOffsets[b] and dDstSizes[b] = n regenerates every non-empty block whose dCSizes[b]
+ * is not an error code (HUF_decompress reads cSize == dstSize as a raw copy and cSize == 1 as RLE, lib/huf.h:60-63) -- with the
+ * reference's own exception: it cannot decode a few of its compressed blocks (a code of length 1 at tableLog 12 is written as
+ * weight 12, which HUF_readStats rejects, entropy_common.c:191), and the decoders return its verdict for them.
+ * All arrays and buffers are in DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays.
+ * Contract: dOut, dOffsets and dCSizes overlap no source and no other array; sources may overlap each other.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing and writes nothing, not even dOffsets[0]); srcSize_wrong if
+ * nBlocks > 0xFFFFFFFF or a pointer is NULL while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_HUF_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                   const void* const* dSrcs, const size_t* dSrcSizes,
+                                   unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_compress1X_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                     const void* const* dSrcs, const size_t* dSrcSizes,
+                                     unsigned maxSymbolValue, unsigned tableLog, void* stream);
+
 /* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
  * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
  * DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).

@@ -8,7 +8,14 @@
   (c) small layout   the first 256 MiB of the stream cut into seeded sizes uniform in [64 B, 4 KiB], as (b).
 
 A build with the single-stream descriptor calls (FSEB200_HUF_*1X_blocks) is also timed with them: a1_* in layout (a), b1_* in
-(b), c1_* in (c), next to the 4X descriptor calls of the same run (c_* is 4X in layout (c)).  Layouts (b) and (c) decode only
+(b), c1_* in (c), next to the 4X descriptor calls of the same run (c_* is 4X in layout (c)).
+
+A build with the packed calls (FSEB200_HUF_compress[1X]_packed) times them right after the descriptor encode of the same layout
+and format, on the same blocks (*_enc_packed, e.g. a_enc_packed next to a_enc_blocks, b1_enc_packed next to b1_enc), then decodes
+every block from the packed buffer with the descriptor decoder and checks the source comes back (*_packed_decoded digests, equal
+to a_source).  *_packed_share is packed bytes per source byte.  Layout (d) is 1 GiB of random bytes in 32 KB blocks, every block
+raw: d_enc / d1_enc is the descriptor encode (which leaves raw blocks to the caller), d_enc_packed / d1_enc_packed the packed
+one (copy included), d_copy a plain device-to-device copy of the same GiB.  Layouts (b) and (c) decode only
 the blocks that compressed to a Huffman block (1 < cSize < size); every figure is scaled to ms per GiB of uncompressed bytes
 that the call encodes or decodes.  `cpu_ref` is the compiled reference's single-thread HUF_compress1X / HUF_decompress1X_DCtx
 on a sample of layout (a) (oracle/_ref/libfse_ref.so, skipped when it is absent), in the same units.
@@ -49,7 +56,11 @@ def declare(L):
         if present:
             f = getattr(L, "FSEB200_HUF_compress%s_blocks" % suffix); f.restype = sz; f.argtypes = [sz, vp, vp, vp, vp, vp, u, u, vp]
             f = getattr(L, "FSEB200_HUF_decompress%s_blocks" % suffix); f.restype = sz; f.argtypes = [sz, vp, vp, vp, vp, vp, vp]
-    return have, have1x
+    have_packed = hasattr(L, "FSEB200_HUF_compress_packed")
+    if have_packed:
+        for suffix in ("", "1X"):
+            f = getattr(L, "FSEB200_HUF_compress%s_packed" % suffix); f.restype = sz; f.argtypes = [sz, vp, sz, vp, vp, vp, vp, u, u, vp]
+    return have, have1x, have_packed
 
 
 def ragged_sizes(total, seed=7, lo=1024, hi=128 * 1024):
@@ -110,7 +121,7 @@ def child(lib_path, reps):
     import numpy as np
     import torch
     L = C.CDLL(lib_path)
-    have, have1x = declare(L)
+    have, have1x, have_packed = declare(L)
     dev = torch.device("cuda")
     stream = torch.cuda.current_stream().cuda_stream
     slot = 512 + BLOCK + (BLOCK >> 7) + 12
@@ -164,7 +175,35 @@ def child(lib_path, reps):
             assert torch.equal(dst, src[:GIB]) and bool((res == BLOCK).all())
         del cbuf
 
-        def ragged(key, enc, dec, sizes):
+        def sha(t):
+            return hashlib.sha256(t.cpu().numpy().tobytes()).hexdigest()[:16]
+
+        def pack_run(key, fn, dec, sp, sn, offs, total):
+            """the packed call on blocks (sp, sn) into one buffer, then every block decoded from it with the descriptor decoder"""
+            n = sn.numel()
+            pout = torch.empty(total + 32, dtype=torch.uint8, device=dev)
+            poffs = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            pcs = torch.empty(n, dtype=torch.int64, device=dev)
+            out[key + "_enc_packed"] = timed(lambda: fn(n, pout.data_ptr(), pout.numel(), poffs.data_ptr(), pcs.data_ptr(), sp.data_ptr(),
+                                                        sn.data_ptr(), 255, 12, stream)) * GIB / total
+            used = int(poffs[-1])
+            out[key + "_packed_share"] = round(used / total, 4)           # packed bytes per source byte
+            digest[key + "_packed_out"] = sha(pout[:used])
+            dst.zero_()
+            pres = torch.empty(n, dtype=torch.int64, device=dev)
+            # the descriptor arrays stay referenced until the call is enqueued: a temporary freed while the argument list is built
+            # would hand its memory to the next one
+            od, cp, cl = t64(dst.data_ptr() + offs), poffs[:-1] + pout.data_ptr(), poffs[1:] - poffs[:-1]
+            assert dec(n, od.data_ptr(), sn.data_ptr(), pres.data_ptr(), cp.data_ptr(), cl.data_ptr(), stream) == 0
+            assert torch.equal(pres, sn) and torch.equal(dst[:total], src[:total])
+            digest[key + "_packed_decoded"] = sha(dst[:total])
+
+        if have_packed:                                                 # (a) packed, next to a_enc_blocks / a1_enc of this run
+            pack_run("a", L.FSEB200_HUF_compress_packed, L.FSEB200_HUF_decompress_blocks, sp, sn, b * BLOCK, GIB)
+            pack_run("a1", L.FSEB200_HUF_compress1X_packed, L.FSEB200_HUF_decompress1X_blocks, sp, sn, b * BLOCK, GIB)
+            digest["a_source"] = sha(src[:GIB])
+
+        def ragged(key, enc, dec, sizes, pk=None):
             """encode blocks back to back into bound-sized destinations, pack the Huffman blocks back to back, decode them"""
             n = len(sizes)
             total = int(sum(sizes))
@@ -197,14 +236,32 @@ def child(lib_path, reps):
             assert torch.equal(dst[ok], src[:GIB][ok])
             out[key + "_count"] = n
             out[key + "_huffman_share"] = round(float(kn.sum()) / total, 4)
+            if pk is not None:
+                del ok
+                pack_run(key, pk, dec, rsp, rsn, offs, total)
 
         layouts = {"b": ragged_sizes(GIB), "c": ragged_sizes(GIB // 4, seed=9, lo=64, hi=4096)}
         for lay, sizes in layouts.items():
-            ragged(lay, L.FSEB200_HUF_compress_blocks, L.FSEB200_HUF_decompress_blocks, sizes)
+            ragged(lay, L.FSEB200_HUF_compress_blocks, L.FSEB200_HUF_decompress_blocks, sizes,
+                   L.FSEB200_HUF_compress_packed if have_packed else None)
             if have1x:
-                ragged(lay + "1", L.FSEB200_HUF_compress1X_blocks, L.FSEB200_HUF_decompress1X_blocks, sizes)
+                ragged(lay + "1", L.FSEB200_HUF_compress1X_blocks, L.FSEB200_HUF_decompress1X_blocks, sizes,
+                       L.FSEB200_HUF_compress1X_packed if have_packed else None)
         if have1x:
             out["cpu_ref"] = cpu_ref_rates(src[: 512 * BLOCK].cpu().numpy(), 512)
+        if have_packed:                                                 # (d) 1 GiB of random bytes in 32 KB blocks: every block raw
+            gen = torch.Generator(device=dev)
+            gen.manual_seed(11)
+            src[:GIB] = torch.randint(0, 256, (GIB,), dtype=torch.uint8, device=dev, generator=gen)
+            cbuf = torch.empty(nb * slot + 64, dtype=torch.uint8, device=dev)
+            ddp = t64(cbuf.data_ptr() + b * slot)
+            for key, enc, pk, dec in (("d", L.FSEB200_HUF_compress_blocks, L.FSEB200_HUF_compress_packed, L.FSEB200_HUF_decompress_blocks),
+                                      ("d1", L.FSEB200_HUF_compress1X_blocks, L.FSEB200_HUF_compress1X_packed, L.FSEB200_HUF_decompress1X_blocks)):
+                out[key + "_enc"] = timed(lambda: enc(nb, ddp.data_ptr(), dc.data_ptr(), cs2.data_ptr(), sp.data_ptr(), sn.data_ptr(), 255, 12, stream))
+                assert bool((cs2 == 0).all())                           # the descriptor call leaves the raw blocks to its caller
+                pack_run(key, pk, dec, sp, sn, b * BLOCK, GIB)
+            out["d_copy"] = timed(lambda: dst.copy_(src[:GIB]))           # a plain device-to-device copy of the same bytes
+            del cbuf
     print(json.dumps({"ms": out, "digest": digest}))
 
 
