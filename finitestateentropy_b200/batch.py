@@ -226,3 +226,74 @@ def fseu16_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_symbols, resul
     """FSE_decompressU16 on every block b: csrc_ptrs[b] / csrc_sizes[b] bytes into dst_ptrs[b] (2-byte aligned) of room for
     dst_symbols[b] symbols, on the current stream.  Returns results (int64; regenerated symbols or error code per block)."""
     return _codec_blocks("FSEB200_FSEU16_decompress_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_symbols), results)
+
+
+def fse_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, work=None, max_symbol_value=255, table_log=12):
+    """FSE_compress2 on every block b (src_ptrs[b] / src_sizes[b] bytes) at capacity FSE_compressBound, the results stored back
+    to back in `out` (capacity out.numel()), raw and RLE blocks included, on the current stream.  `work` (uint8) holds each
+    block's staging slot.  Returns (out, offsets, csizes): offsets (int64, n + 1 entries) is the prefix sum of the stored lengths,
+    csizes the reference's value per block (dstSize_tooSmall / workSpace_tooSmall for a block that does not fit `out` / `work`).
+    With out or work None they are sized from sum(src_sizes) -- out at that sum + 32 bytes, work by fse_packed_workspace, both
+    always enough: reading the sum costs one host synchronisation.  Decode with fse_decompress_packed."""
+    return _fse_compress_packed("FSEB200_FSE_compress_packed", 1, src_ptrs, src_sizes, out, offsets, csizes, work,
+                                max_symbol_value, table_log)
+
+
+def fseu16_compress_packed(src_ptrs, src_symbols, out=None, offsets=None, csizes=None, work=None, max_symbol_value=0, table_log=12):
+    """fse_compress_packed for FSE_compressU16: src_symbols[b] 16-bit symbols at src_ptrs[b] (2-byte aligned); `out` and `work`
+    default to 2 * sum(src_symbols) + 32 bytes and the workspace of 2 * sum(src_symbols) source bytes"""
+    return _fse_compress_packed("FSEB200_FSEU16_compress_packed", 2, src_ptrs, src_symbols, out, offsets, csizes, work,
+                                max_symbol_value, table_log)
+
+
+def fse_packed_workspace(n_blocks, src_bytes):
+    """bytes of workspace that never run short for n_blocks blocks of src_bytes source bytes in all (U16: 2 * symbols)"""
+    from . import lib
+    return int(lib().FSEB200_FSE_packed_workspace(n_blocks, src_bytes))
+
+
+def _fse_compress_packed(fn_name, unit, src_ptrs, src_sizes, out, offsets, csizes, work, msv, tlog):
+    from . import lib
+    n = _blocks_args(src_ptrs, src_sizes)
+    dev = src_ptrs.device
+    if out is None or work is None:
+        src_bytes = unit * int(src_sizes.sum().item())                                  # .item(): the host sync
+        if out is None:
+            out = torch.empty(src_bytes + 32, dtype=torch.uint8, device=dev)
+        if work is None:
+            work = torch.empty(max(fse_packed_workspace(n, src_bytes), 1), dtype=torch.uint8, device=dev)
+    if offsets is None:
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    _check(out, torch.uint8); _check(work, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64)
+    assert offsets.numel() == n + 1 and csizes.numel() == n and out.device == dev and work.device == dev, (offsets.numel(), csizes.numel(), n)
+    r = getattr(lib(), fn_name)(n, out.data_ptr(), out.numel(), offsets.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
+                                src_sizes.data_ptr(), msv, tlog, work.data_ptr(), work.numel(), _stream_ptr())
+    _ret(r, fn_name)
+    return out, offsets, csizes
+
+
+def fse_decompress_packed(packed, offsets, dst_ptrs, dst_sizes, results=None):
+    """every block of a packed FSE buffer (fse_compress_packed's out and offsets) into dst_ptrs[b], regenerating dst_sizes[b]
+    bytes, on the current stream: a stored length equal to the size is a raw copy, one byte an RLE block, anything else is
+    FSE_decompress'ed.  Returns results (int64; the regenerated size or an error code per block)."""
+    return _fse_decompress_packed("FSEB200_FSE_decompress_packed", packed, offsets, dst_ptrs, dst_sizes, results)
+
+
+def fseu16_decompress_packed(packed, offsets, dst_ptrs, dst_symbols, results=None):
+    """fse_decompress_packed for FSE-U16: dst_symbols[b] 16-bit symbols into dst_ptrs[b] (2-byte aligned); results in symbols"""
+    return _fse_decompress_packed("FSEB200_FSEU16_decompress_packed", packed, offsets, dst_ptrs, dst_symbols, results)
+
+
+def _fse_decompress_packed(fn_name, packed, offsets, dst_ptrs, dst_sizes, results):
+    from . import lib
+    n = _blocks_args(dst_ptrs, dst_sizes)
+    if results is None:
+        results = torch.empty(n, dtype=torch.int64, device=dst_ptrs.device)
+    _check(packed, torch.uint8); _check(offsets, torch.int64); _check(results, torch.int64)
+    assert offsets.numel() == n + 1 and results.numel() == n and packed.device == dst_ptrs.device, (offsets.numel(), results.numel(), n)
+    r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), packed.data_ptr(),
+                                offsets.data_ptr(), _stream_ptr())
+    _ret(r, fn_name)
+    return results

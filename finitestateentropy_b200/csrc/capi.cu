@@ -32,6 +32,8 @@ cudaError_t launch_fseu16_decode(const BatchGeom&, void*, const void*, const u64
 cudaError_t launch_fseu16_encode(const BatchGeom&, void*, u64*, const void*, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fse_encode_blocks(const BlockDescs&, bool, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fse_decode_blocks(const BlockDescs&, bool, cudaStream_t);
+cudaError_t launch_fse_compress_packed(u8*, u64, u64*, u64*, const u8* const*, const u64*, u32, u8*, u64, bool, unsigned, unsigned, cudaStream_t);
+cudaError_t launch_fse_decompress_packed(u8* const*, const u64*, u64*, const u8*, const u64*, u32, bool, cudaStream_t);
 cudaError_t launch_hist(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_hist16(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_micro(int, const MicroArgs&, void*, u64*, cudaStream_t);
@@ -286,6 +288,50 @@ FSEB_API size_t FSEB200_FSEU16_decompress_blocks(size_t nBlocks, void* const* dD
                                                  const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
 {
     return fse_blocks(nBlocks, dDsts, dDstCapacities, dResults, dCSrcs, dCSrcSizes, true, false, 0, 0, stream);
+}
+
+// Packed FSE / FSE-U16 blocks (include/fse_b200.h): the descriptor codecs with every block stored back to back in one buffer.
+namespace {
+size_t fse_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes, const void* const* dSrcs,
+                  const size_t* dSrcSizes, unsigned msv, unsigned tlog, void* dWork, size_t workSize, bool wide, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || !dOut || !dOffsets || !dCSizes || !dSrcs || !dSrcSizes || !dWork) return (size_t)err(E_SRC_WRONG);
+    return ok_or_generic(launch_fse_compress_packed((u8*)dOut, outCapacity, (u64*)dOffsets, (u64*)dCSizes, (const u8* const*)dSrcs,
+                                                    (const u64*)dSrcSizes, (u32)nBlocks, (u8*)dWork, workSize, wide, msv, tlog,
+                                                    (cudaStream_t)stream));
+}
+size_t fse_unpacked(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults, const void* dIn,
+                    const size_t* dOffsets, bool wide, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || !dDsts || !dDstSizes || !dResults || !dIn || !dOffsets) return (size_t)err(E_SRC_WRONG);
+    return ok_or_generic(launch_fse_decompress_packed((u8* const*)dDsts, (const u64*)dDstSizes, (u64*)dResults, (const u8*)dIn,
+                                                      (const u64*)dOffsets, (u32)nBlocks, wide, (cudaStream_t)stream));
+}
+}
+FSEB_API size_t FSEB200_FSE_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                            const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog,
+                                            void* dWork, size_t workSize, void* stream)
+{
+    return fse_packed(nBlocks, dOut, outCapacity, dOffsets, dCSizes, dSrcs, dSrcSizes, maxSymbolValue, tableLog, dWork, workSize, false, stream);
+}
+FSEB_API size_t FSEB200_FSEU16_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                               const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog,
+                                               void* dWork, size_t workSize, void* stream)
+{
+    return fse_packed(nBlocks, dOut, outCapacity, dOffsets, dCSizes, dSrcs, dSrcSizes, maxSymbolValue, tableLog, dWork, workSize, true, stream);
+}
+FSEB_API size_t FSEB200_FSE_packed_workspace(size_t nBlocks, size_t srcBytes) { return srcBytes + (srcBytes >> 7) + 524 * nBlocks; }
+FSEB_API size_t FSEB200_FSE_decompress_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                              const void* dIn, const size_t* dOffsets, void* stream)
+{
+    return fse_unpacked(nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, false, stream);
+}
+FSEB_API size_t FSEB200_FSEU16_decompress_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                                 const void* dIn, const size_t* dOffsets, void* stream)
+{
+    return fse_unpacked(nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, true, stream);
 }
 
 FSEB_API size_t FSEB200_batch_blocks(size_t total, size_t blockSize) { return blockSize ? (total + blockSize - 1) / blockSize : 0; }

@@ -37,6 +37,7 @@
 #include "fse_dev.cuh"
 #include "sink_dev.cuh"
 #include "huf_build_dev.cuh"
+#include "pack_dev.cuh"
 
 namespace fseb {
 namespace hufe {
@@ -618,108 +619,27 @@ huf_emit_kernel(Geo g, u8* __restrict__ cbuf, const u8* __restrict__ src, const 
 
 // ---------------------------------------------------------------------------------------------
 // Packed output (PackedDescs): the plan kernel has settled every block's verdict, so every block's stored length is known
-// before anything is written.  Between plan and emit, a device-wide exclusive scan of the stored lengths gives each block its
-// offset, and placement settles what the plan kernel left open: the capacity verdict (the plan is made final, emit skips the
-// block), the RLE byte and the raw copy of a block whose verdict is 0.  The scan is reduce-then-scan over tiles of PACK_TILE
-// blocks -- the tiles' sums, their exclusive scan in one CTA starting from the total of the sub-batches before, then the scan
-// inside each tile -- in u64, so totals above 2^32 and batches of up to 2^32 - 1 blocks are exact.
+// before anything is written.  Between plan and emit, a device-wide exclusive scan of the stored lengths (pack_dev.cuh) gives
+// each block its offset, and placement settles what the plan kernel left open: the capacity verdict (the plan is made final,
+// emit skips the block), the RLE byte and the raw copy of a block whose verdict is 0.  The scan starts each sub-batch from the
+// total of the sub-batches before.
 // ---------------------------------------------------------------------------------------------
-constexpr int PACK_THREADS = 256, PACK_ITEMS = 8, PACK_SCAN_THREADS = 1024, COPY_THREADS = 256, COPY_UNROLL = 4;
-constexpr u32 PACK_TILE = PACK_THREADS * PACK_ITEMS;
-
-// exclusive prefix of v over the CTA's NT threads in `excl`; returns the CTA's total.  sm: NT / 32 + 1 words.
-template <int NT>
-__device__ __forceinline__ u64 cta_exclusive_scan(u64 v, u64& excl, u64* sm)
-{
-    static_assert(NT % 32 == 0 && NT <= 1024, "one warp scans the warp totals");
-    unsigned const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    u64 incl = v;
-    #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { u64 const t = __shfl_up_sync(FULL, incl, d); if (lane >= (unsigned)d) incl += t; }
-    if (lane == 31) sm[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-        u64 const w = lane < NT / 32 ? sm[lane] : 0;
-        u64 wi = w;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { u64 const t = __shfl_up_sync(FULL, wi, d); if (lane >= (unsigned)d) wi += t; }
-        if (lane < NT / 32) sm[lane] = wi - w;
-        if (lane == NT / 32 - 1) sm[NT / 32] = wi;
-    }
-    __syncthreads();
-    excl = sm[warp] + incl - v;
-    u64 const total = sm[NT / 32];
-    __syncthreads();                                                // sm is free for the next call
-    return total;
-}
-
-// step 1: the stored length of each tile of blocks
-__global__ void __launch_bounds__(PACK_THREADS)
-huf_pack_sums_kernel(PackedDescs g, u64* __restrict__ tileSum)
-{
-    __shared__ u64 sm[PACK_THREADS / 32 + 1];
-    u64 const first = (u64)blockIdx.x * PACK_TILE + threadIdx.x * PACK_ITEMS;
-    u64 s = 0;
-    #pragma unroll
-    for (int i = 0; i < PACK_ITEMS; i++) { u64 const b = first + i; if (b < g.nBlocks) s += packed_len(g.result[b], g.srcSize[b]); }
-    u64 excl;
-    u64 const t = cta_exclusive_scan<PACK_THREADS>(s, excl, sm);
-    if (threadIdx.x == 0) tileSum[blockIdx.x] = t;
-}
-
-// step 2, one CTA: tile sums -> tile offsets (in place), from *carryIn (the sub-batches before; nullptr: 0); the grand total
-// goes to *totalOut, which is offset[nBlocks] of the sub-batch
-__global__ void __launch_bounds__(PACK_SCAN_THREADS)
-huf_pack_scan_tiles_kernel(u64* __restrict__ tileSum, u32 nTiles, const u64* __restrict__ carryIn, u64* __restrict__ totalOut)
-{
-    __shared__ u64 sm[PACK_SCAN_THREADS / 32 + 1];
-    u64 run = carryIn ? *carryIn : 0;
-    for (u32 t0 = 0; t0 < nTiles; t0 += PACK_SCAN_THREADS) {
-        u32 const t = t0 + threadIdx.x;
-        u64 const v = t < nTiles ? tileSum[t] : 0;
-        u64 excl;
-        u64 const tot = cta_exclusive_scan<PACK_SCAN_THREADS>(v, excl, sm);
-        if (t < nTiles) tileSum[t] = run + excl;
-        run += tot;
-    }
-    if (threadIdx.x == 0) *totalOut = run;
-}
-
-// step 3: offsets inside each tile, the capacity verdict, the RLE bytes
-__global__ void __launch_bounds__(PACK_THREADS)
-huf_pack_place_kernel(PackedDescs g, const u64* __restrict__ tileOff, Plan* __restrict__ plans)
-{
-    __shared__ u64 sm[PACK_THREADS / 32 + 1];
-    u64 const first = (u64)blockIdx.x * PACK_TILE + threadIdx.x * PACK_ITEMS;
-    u64 v[PACK_ITEMS], len[PACK_ITEMS], s = 0;
-    #pragma unroll
-    for (int i = 0; i < PACK_ITEMS; i++) {
-        u64 const b = first + i;
-        bool const in = b < g.nBlocks;
-        v[i] = in ? g.result[b] : 0;
-        len[i] = in ? packed_len(v[i], g.srcSize[b]) : 0;
-        s += len[i];
-    }
-    u64 excl;
-    cta_exclusive_scan<PACK_THREADS>(s, excl, sm);
-    u64 off = tileOff[blockIdx.x] + excl;
-    #pragma unroll
-    for (int i = 0; i < PACK_ITEMS; i++) {
-        u64 const b = first + i;
-        if (b >= g.nBlocks) break;
+struct HufPlace {
+    typedef PackedDescs Geo;
+    typedef Plan* Aux;
+    static __device__ __forceinline__ u64 value(const PackedDescs& g, u64 b) { return g.result[b]; }
+    static __device__ __forceinline__ u64 len(const PackedDescs& g, u64 b, u64 v) { return packed_len(v, g.srcSize[b]); }
+    // the capacity verdict (nothing is written for a block that does not fit), the RLE byte
+    static __device__ __forceinline__ void place(const PackedDescs& g, Plan* plans, u64 b, u64 v, u64 off, u64 len)
+    {
         g.offset[b] = off;
-        if (!is_err(v[i]) && off + len[i] > g.outCap) { g.result[b] = err(E_DST_TOO_SMALL); plans[b].state = 1; }   // nothing is written for it
-        else if (v[i] == 1) g.out[off] = g.src[b][0];
-        off += len[i];
+        if (!is_err(v) && off + len > g.outCap) { g.result[b] = err(E_DST_TOO_SMALL); plans[b].state = 1; }
+        else if (v == 1) g.out[off] = g.src[b][0];
     }
-}
+};
 
-// step 4: raw copy of every block whose verdict is 0, one CTA per block.  The destination's 16-byte aligned interior is
-// written in whole 16-byte stores, the bytes before and after it one by one.  Every interior chunk's source bytes sit at
-// the same misalignment sh in the source, so they are the bytes [sh, sh + 16) of two consecutive aligned 16-byte source
-// pieces: a lane loads one piece, takes the next from its neighbour lane, and funnel-shifts the pair.  A piece is loaded
-// only if it holds a byte of the source.
-__global__ void __launch_bounds__(COPY_THREADS)
+// raw copy of every block whose verdict is 0, one CTA per block
+__global__ void __launch_bounds__(pack::COPY_THREADS)
 huf_pack_raw_kernel(PackedDescs g)
 {
     u32 const b = blockIdx.x;
@@ -728,42 +648,7 @@ huf_pack_raw_kernel(PackedDescs g)
     if (n == 0) return;
     const u8* const s = g.src[b];
     u8* const d = g.out + g.offset[b];
-    u32 const tid = threadIdx.x, lane = tid & 31u;
-    u32 const head = min((u32)(-reinterpret_cast<u64>(d) & 15), n);
-    u32 const nChunks = (n - head) / 16, tailBeg = head + 16 * nChunks;
-    if (tid < head) d[tid] = s[tid];
-    if (tid < n - tailBeg) d[tailBeg + tid] = s[tailBeg + tid];
-    u64 const sa = reinterpret_cast<u64>(s) + head;                 // source of chunk 0
-    u32 const sh = (u32)(sa & 15), q = sh >> 2, r = 8 * (sh & 3);
-    const uint4* const sp = reinterpret_cast<const uint4*>(sa - sh);    // chunk k: pieces k and k + 1 (k alone when sh == 0)
-    uint4* const dp = reinterpret_cast<uint4*>(d + head);
-    u32 const lastPiece = nChunks - (sh == 0);                      // pieces [0, lastPiece] hold source bytes (none if nChunks == 0)
-    auto ld = [&](u32 k) { return (nChunks && k <= lastPiece) ? __ldg(sp + k) : make_uint4(0, 0, 0, 0); };
-    #pragma unroll 1
-    for (u32 k0 = 0; k0 < nChunks; k0 += COPY_THREADS * COPY_UNROLL) {   // CTA-uniform: every lane takes part in the shuffles
-        uint4 a[COPY_UNROLL], c[COPY_UNROLL];
-        #pragma unroll
-        for (int j = 0; j < COPY_UNROLL; j++) {
-            u32 const k = k0 + j * COPY_THREADS + tid;
-            a[j] = ld(k);
-            c[j] = (lane == 31 && sh) ? ld(k + 1) : make_uint4(0, 0, 0, 0);
-        }
-        #pragma unroll
-        for (int j = 0; j < COPY_UNROLL; j++) {
-            u32 const k = k0 + j * COPY_THREADS + tid;
-            uint4 nx;
-            nx.x = __shfl_down_sync(FULL, a[j].x, 1); nx.y = __shfl_down_sync(FULL, a[j].y, 1);
-            nx.z = __shfl_down_sync(FULL, a[j].z, 1); nx.w = __shfl_down_sync(FULL, a[j].w, 1);
-            if (lane == 31) nx = c[j];
-            if (k >= nChunks) continue;
-            u32 const x[8] = { a[j].x, a[j].y, a[j].z, a[j].w, nx.x, nx.y, nx.z, nx.w };
-            u32 y[5];
-            #pragma unroll
-            for (int i = 0; i < 5; i++) y[i] = q == 0 ? x[i] : q == 1 ? x[i + 1] : q == 2 ? x[i + 2] : x[i + 3];
-            dp[k] = make_uint4(__funnelshift_r(y[0], y[1], r), __funnelshift_r(y[1], y[2], r),
-                               __funnelshift_r(y[2], y[3], r), __funnelshift_r(y[3], y[4], r));
-        }
-    }
+    pack::cta_copy<pack::COPY_THREADS, pack::COPY_UNROLL>(d, s, n);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -876,7 +761,7 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
     u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch
     if constexpr (packed) {
-        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * (((size_t)step + hufe::PACK_TILE - 1) / hufe::PACK_TILE), &e);
+        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * (((size_t)step + pack::PACK_TILE - 1) / pack::PACK_TILE), &e);
         if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
     }
     for (u32 b0 = 0; b0 < g.nBlocks; b0 += step) {
@@ -885,12 +770,12 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
         unsigned const grid = (sb.g.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
         hufe::huf_plan_kernel<Geo, NS><<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(sb.g, sb.cbuf, cs, sb.src, msv, tlog, plans + b0);
         if constexpr (packed) {                                     // offsets, capacity verdicts, RLE bytes, raw copies; then emit
-            unsigned const tiles = (sb.g.nBlocks + hufe::PACK_TILE - 1) / hufe::PACK_TILE;
-            hufe::huf_pack_sums_kernel<<<tiles, hufe::PACK_THREADS, 0, stream>>>(sb.g, tileSum);
-            hufe::huf_pack_scan_tiles_kernel<<<1, hufe::PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, b0 ? sb.g.offset : nullptr,
-                                                                                         sb.g.offset + sb.g.nBlocks);
-            hufe::huf_pack_place_kernel<<<tiles, hufe::PACK_THREADS, 0, stream>>>(sb.g, tileSum, plans + b0);
-            hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, hufe::COPY_THREADS, 0, stream>>>(sb.g);
+            unsigned const tiles = (sb.g.nBlocks + pack::PACK_TILE - 1) / pack::PACK_TILE;
+            pack::pack_sums_kernel<hufe::HufPlace><<<tiles, pack::PACK_THREADS, 0, stream>>>(sb.g, tileSum);
+            pack::pack_scan_tiles_kernel<<<1, pack::PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, b0 ? sb.g.offset : nullptr,
+                                                                                     sb.g.offset + sb.g.nBlocks);
+            pack::pack_place_kernel<hufe::HufPlace><<<tiles, pack::PACK_THREADS, 0, stream>>>(sb.g, tileSum, plans + b0);
+            hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g);
         }
         hufe::huf_emit_kernel<Geo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);
     }

@@ -173,6 +173,59 @@ size_t FSEB200_FSEU16_compress_blocks(size_t nBlocks, void* const* dDsts, const 
 size_t FSEB200_FSEU16_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dResults,
                                         const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream);
 
+/* Tier 1, per-block descriptors with packed output (FSE, FSE-U16): the blocks given by dSrcs / dSrcSizes are compressed and
+ * stored back to back in one buffer, each at an offset the call computes on the device, raw and RLE blocks included; the
+ * *_decompress_packed calls regenerate every block from that buffer and its offsets.  Let u be the unit (1 for FSE, 2 for
+ * U16) and, per block b, n = dSrcSizes[b] (U16: symbols).
+ *   dCSizes[b]  = exactly what FSE_compress2(dst, FSE_compressBound(n), src, n, maxSymbolValue, tableLog) returns (U16:
+ *                 FSE_compressU16(dst, FSE_compressBound(2n), ...)): 0, 1, a size or an error code -- except for a block
+ *                 that does not fit the workspace or the output (below).
+ *   stored length L[b]: dCSizes[b] >= 2: dCSizes[b], the reference's compressed bytes; 1: u, the symbol src[0] as it lies in
+ *                 memory (RLE); 0: u * n, a raw copy of the source (0 bytes for an empty block); an error code: 0, nothing.
+ *                 L[b] <= u * n always (FSE answers 0 once the output reaches n - 1 bytes, U16 at 2(n - 1), and U16 returns
+ *                 n itself for n <= 1), so an outCapacity of u * sum(n) always holds every block; add 32 bytes of slack for
+ *                 the decoders' sector reads.
+ *   dOffsets    has nBlocks + 1 entries: dOffsets[b] = L[0] + ... + L[b-1], dOffsets[nBlocks] = the total.  It is written in
+ *                 full even when blocks do not fit, so a too-small call still tells the size it needs.
+ *   capacity    block b is stored at dOut + dOffsets[b] only if dOffsets[b] + L[b] <= outCapacity; otherwise dCSizes[b] =
+ *                 dstSize_tooSmall and nothing is written for it (a block whose value is an error code keeps it).  Nothing
+ *                 outside [dOut, dOut + min(total, outCapacity)) is ever written.
+ *   workspace   an FSE block's size is known only once it is coded, so each block is first coded into a staging slot of
+ *                 FSE_compressBound(u * n) bytes in dWork; the slots are laid out back to back in block order.  A block the
+ *                 limits below settle takes no slot.  Block b is coded only if its slot ends at or before workSize;
+ *                 otherwise dCSizes[b] = workSpace_tooSmall and nothing is stored for it.  FSEB200_FSE_packed_workspace gives
+ *                 a size that never runs short; dWork beyond workSize is never touched.
+ * Limits, as the descriptor calls above: an FSE source above 2^30 bytes and a U16 source above 2^29 symbols give
+ * srcSize_wrong, a U16 source at an odd address GENERIC.
+ * Decompress, per block b, with L = dOffsets[b+1] - dOffsets[b] and n = dDstSizes[b] (the regenerated size, U16: symbols;
+ * not a capacity):
+ *   1. the descriptor decoder's limit and alignment verdicts come first: L or n above the limits gives srcSize_wrong, a U16
+ *      destination at an odd address GENERIC, and nothing is written;
+ *   2. L == u * n: a raw copy; the result is n (n == 0 included);
+ *   3. otherwise L == u: RLE, n copies of the unit at dIn + dOffsets[b]; the result is n;
+ *   4. otherwise exactly what FSEB200_FSE{,U16}_decompress_blocks returns for source dIn + dOffsets[b], cSize L and
+ *      capacity n -- for L == 0 (a block whose value was an error) corruption_detected, U16 srcSize_wrong.
+ *   Rules 2 and 3 never capture a compressed block: an FSE one has 2 <= L < n - 1, and a U16 one is never 2 or 2n bytes long.
+ * All arrays and buffers are in DEVICE memory; the calls are asynchronous on `stream` and the host never reads the arrays.
+ * Contract: compress: dOut, dOffsets, dCSizes and dWork overlap no source and no other array; sources may overlap each other.
+ * Decompress: dIn must be readable up to the end of the 32-byte sector that holds each block's last byte; no destination may
+ * overlap another destination, dIn or the arrays.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing and writes nothing); srcSize_wrong if nBlocks > 0xFFFFFFFF
+ * or a pointer is NULL while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_FSE_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                   const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog,
+                                   void* dWork, size_t workSize, void* stream);
+size_t FSEB200_FSEU16_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
+                                      const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog,
+                                      void* dWork, size_t workSize, void* stream);
+/* Host-side, no device work: srcBytes + (srcBytes >> 7) + 524 * nBlocks, at least the sum of FSE_compressBound over any batch
+ * of nBlocks blocks of srcBytes source bytes in all (U16: 2 * sum(n)). */
+size_t FSEB200_FSE_packed_workspace(size_t nBlocks, size_t srcBytes);
+size_t FSEB200_FSE_decompress_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                     const void* dIn, const size_t* dOffsets, void* stream);
+size_t FSEB200_FSEU16_decompress_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                        const void* dIn, const size_t* dOffsets, void* stream);
+
 /* Table reuse across blocks (lib/huf.h:191 per block; the shape programs/bench.c:610-633 and HUF_compress4X_repeat,
  * lib/huf_compress.c:664-712, reduce to when the previous table is kept): every block of the batch is coded with ONE
  * caller-supplied table -- dCTable = 256 HUF_CElt cells in DEVICE memory, the layout HUF_buildCTable produces.

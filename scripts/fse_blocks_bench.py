@@ -6,12 +6,20 @@
   (b) ragged layout  the same stream cut into seeded sizes uniform in [1 KiB, 128 KiB] (U16: even byte counts), sources back
                      to back: encode into bound-sized destinations, then decode from the compressed blocks packed back to back
                      (packed outside the timed region) into outputs back to back.  Also the share of blocks per encode kernel.
+  (c) random layout  FSE only: 1 GiB of random bytes in 32 KB blocks, every block raw.  c_enc_blocks is the descriptor encode
+                     (which leaves raw blocks to the caller), c_copy a plain device-to-device copy of the same GiB.  (A U16
+                     block is never raw: its symbols hold at most log2(287) bits of 16.)
+
+The packed calls (FSEB200_FSE{,U16}_{compress,decompress}_packed) are timed alternated with the descriptor calls on the same
+blocks: *_pk_enc_packed next to *_pk_enc_blocks (descriptor encode into bound-sized destinations), *_pk_dec_packed next to
+*_pk_dec_blocks (descriptor decode of the same compressed bytes); c_enc_packed / c_dec_packed for layout (c).  The packed buffer
+must equal the compressed blocks packed back to back (a_compressed, b_packed digests) and decode to the source.
 
 Each run is a child process per codec; within a child the uniform and descriptor calls alternate, each metric the median of
 --reps timed calls.  Prints one JSON line with the GPU's name, power limit and SM clock, per codec and metric the median and
 range over runs in ms per GiB, and digests of the compressed and decoded bytes.
 
-    python scripts/fse_blocks_bench.py --runs 5
+    python scripts/fse_blocks_bench.py --runs 5 [--codecs fse]
 """
 import argparse
 import ctypes as C
@@ -33,9 +41,11 @@ def declare(L):
     L.FSEB200_genU16.restype = sz; L.FSEB200_genU16.argtypes = [vp, sz, sz, u, C.c_double, u, vp]
     for codec in ("FSE", "FSEU16"):
         for name, args in (("compress_batch", [vp, sz, vp, vp, sz, sz, u, u, vp]), ("decompress_batch", [vp, sz, sz, vp, sz, vp, vp, vp, vp]),
-                           ("compress_blocks", [sz, vp, vp, vp, vp, vp, u, u, vp]), ("decompress_blocks", [sz, vp, vp, vp, vp, vp, vp])):
+                           ("compress_blocks", [sz, vp, vp, vp, vp, vp, u, u, vp]), ("decompress_blocks", [sz, vp, vp, vp, vp, vp, vp]),
+                           ("compress_packed", [sz, vp, sz, vp, vp, vp, vp, u, u, vp, sz, vp]), ("decompress_packed", [sz, vp, vp, vp, vp, vp, vp])):
             f = getattr(L, "FSEB200_%s_%s" % (codec, name))
             f.restype = sz; f.argtypes = args
+    L.FSEB200_FSE_packed_workspace.restype = sz; L.FSEB200_FSE_packed_workspace.argtypes = [sz, sz]
 
 
 def fbound(n):
@@ -86,7 +96,8 @@ def child(codec, reps):
           (lambda: L.FSEB200_probagen(src.data_ptr(), GIB, 0, 0.80, stream))
     assert gen() == 0
     nb = GIB // BLOCK
-    f = {k: getattr(L, "FSEB200_%s_%s" % (name, k)) for k in ("compress_batch", "decompress_batch", "compress_blocks", "decompress_blocks")}
+    f = {k: getattr(L, "FSEB200_%s_%s" % (name, k)) for k in ("compress_batch", "decompress_batch", "compress_blocks", "decompress_blocks",
+                                                               "compress_packed", "decompress_packed")}
 
     def t64(a):
         return torch.tensor(np.asarray(a, dtype=np.int64), device=dev)
@@ -100,6 +111,28 @@ def child(codec, reps):
                 a.record(); fn(); b.record(); b.synchronize()
                 ts.append(a.elapsed_time(b))
         return sorted(ta)[len(ta) // 2], sorted(tb)[len(tb) // 2]
+
+    class Packed:
+        """one packed buffer for n blocks of `nbytes` source bytes in all, and its calls"""
+        def __init__(self, n, sp, sn, nbytes):
+            self.n, self.sp, self.sn = n, sp, sn
+            self.out = torch.empty(nbytes + 32, dtype=torch.uint8, device=dev)
+            self.wsz = L.FSEB200_FSE_packed_workspace(n, nbytes)
+            self.work = torch.empty(self.wsz, dtype=torch.uint8, device=dev)
+            self.offs = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            self.cs = torch.empty(n, dtype=torch.int64, device=dev)
+            self.res = torch.empty(n, dtype=torch.int64, device=dev)
+
+        def enc(self):
+            assert f["compress_packed"](self.n, self.out.data_ptr(), self.out.numel(), self.offs.data_ptr(), self.cs.data_ptr(),
+                                        self.sp.data_ptr(), self.sn.data_ptr(), msv, 12, self.work.data_ptr(), self.wsz, stream) == 0
+
+        def dec(self, dptrs):
+            assert f["decompress_packed"](self.n, dptrs.data_ptr(), self.sn.data_ptr(), self.res.data_ptr(), self.out.data_ptr(),
+                                          self.offs.data_ptr(), stream) == 0
+
+        def digest(self):
+            return hashlib.sha256(self.out[: int(self.offs[-1])].cpu().numpy().tobytes()).hexdigest()[:16]
 
     out, digest = {}, {}
     cbuf = torch.zeros(nb * slot + 64, dtype=torch.uint8, device=dev)
@@ -117,7 +150,11 @@ def child(codec, reps):
     h2 = hashlib.sha256(cbuf2[: nb * slot].view(nb, slot)[used].cpu().numpy().tobytes()).hexdigest()[:16]
     assert h1 == h2
     digest["a_compressed"] = h1
-    del used, cbuf2
+    pka = Packed(nb, sp, sn, GIB)
+    out["a_pk_enc_blocks"], out["a_pk_enc_packed"] = timed_pair(
+        lambda: f["compress_blocks"](nb, dp.data_ptr(), dc.data_ptr(), cs2.data_ptr(), sp.data_ptr(), sn.data_ptr(), msv, 12, stream), pka.enc)
+    assert torch.equal(pka.cs, cs) and pka.digest() == h1
+    del used, cbuf2, pka.work
     dst = torch.zeros(GIB, dtype=torch.uint8, device=dev)
     dst2 = torch.zeros(GIB, dtype=torch.uint8, device=dev)
     res, res2 = torch.empty(nb, dtype=torch.int64, device=dev), torch.empty(nb, dtype=torch.int64, device=dev)
@@ -127,7 +164,14 @@ def child(codec, reps):
         lambda: f["decompress_blocks"](nb, op.data_ptr(), sn.data_ptr(), res2.data_ptr(), cp.data_ptr(), cs.data_ptr(), stream))
     assert torch.equal(dst, src[:GIB]) and torch.equal(dst2, src[:GIB]) and torch.equal(res // w, res2)
     digest["a_decoded"] = hashlib.sha256(dst.cpu().numpy().tobytes()).hexdigest()[:16]
-    del cbuf, dst2
+    dst.zero_()
+    da = t64(dst.data_ptr() + b * BLOCK)
+    out["a_pk_dec_blocks"], out["a_pk_dec_packed"] = timed_pair(
+        lambda: f["decompress_blocks"](nb, op.data_ptr(), sn.data_ptr(), res2.data_ptr(), cp.data_ptr(), cs.data_ptr(), stream),
+        lambda: pka.dec(da))
+    assert torch.equal(dst, src[:GIB]) and torch.equal(pka.res, sn)
+    digest["a_pk_decoded"] = hashlib.sha256(dst.cpu().numpy().tobytes()).hexdigest()[:16]
+    del cbuf, dst2, pka
     # (b) ragged
     sizes = ragged_sizes(GIB, wide)
     n = len(sizes)
@@ -140,6 +184,10 @@ def child(codec, reps):
     rcs = torch.empty(n, dtype=torch.int64, device=dev)
     enc = lambda: f["compress_blocks"](n, rdp.data_ptr(), rdc.data_ptr(), rcs.data_ptr(), rsp.data_ptr(), rsn.data_ptr(), msv, 12, stream)   # noqa: E731
     out["b_enc"], _ = timed_pair(enc, lambda: None)
+    pkb = Packed(n, rsp, rsn, GIB)
+    out["b_pk_enc_blocks"], out["b_pk_enc_packed"] = timed_pair(enc, pkb.enc)
+    assert torch.equal(pkb.cs, rcs)
+    del pkb.work
     csz = rcs.cpu().numpy()
     assert (csz > 1).all() and (csz < np.array(sizes)).all()
     poffs = np.concatenate([[0], np.cumsum(csz)[:-1]]).astype(np.int64)
@@ -154,6 +202,25 @@ def child(codec, reps):
     dec = lambda: f["decompress_blocks"](n, od.data_ptr(), rsn.data_ptr(), rres.data_ptr(), pp.data_ptr(), rcs.data_ptr(), stream)   # noqa: E731
     out["b_dec"], _ = timed_pair(dec, lambda: None)
     assert torch.equal(dst, src[:GIB]) and torch.equal(rres, rsn)
+    dst.zero_()
+    out["b_pk_dec_blocks"], out["b_pk_dec_packed"] = timed_pair(dec, lambda: pkb.dec(od))
+    assert torch.equal(dst, src[:GIB]) and torch.equal(pkb.res, rsn) and pkb.digest() == digest["b_packed"]
+    digest["b_pk_decoded"] = hashlib.sha256(dst.cpu().numpy().tobytes()).hexdigest()[:16]
+    del pkb, packed
+    if not wide:                                                        # (c) random bytes: every block raw
+        rnd = torch.randint(0, 256, (GIB,), dtype=torch.uint8, device=dev, generator=torch.Generator(device=dev).manual_seed(5))
+        rp = t64(rnd.data_ptr() + b * BLOCK)
+        cbuf = torch.empty(nb * slot + 64, dtype=torch.uint8, device=dev)
+        dp = t64(cbuf.data_ptr() + b * slot)
+        pkc = Packed(nb, rp, sn, GIB)
+        out["c_enc_blocks"], out["c_enc_packed"] = timed_pair(
+            lambda: f["compress_blocks"](nb, dp.data_ptr(), dc.data_ptr(), cs2.data_ptr(), rp.data_ptr(), sn.data_ptr(), msv, 12, stream), pkc.enc)
+        assert bool((cs2 == 0).all()) and bool((pkc.cs == 0).all()) and torch.equal(pkc.out[:GIB], rnd)
+        del cbuf, pkc.work
+        out["c_copy"], out["c_dec_packed"] = timed_pair(lambda: dst.copy_(rnd), lambda: pkc.dec(da))
+        assert torch.equal(dst, rnd) and torch.equal(pkc.res, sn)
+        digest["c_source"] = hashlib.sha256(rnd.cpu().numpy().tobytes()).hexdigest()[:16]
+        digest["c_pk_decoded"] = hashlib.sha256(dst.cpu().numpy().tobytes()).hexdigest()[:16]
     print(json.dumps({"ms": out, "digest": digest, "blocks": n}))
 
 
@@ -168,11 +235,12 @@ def main():
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--reps", type=int, default=3, help="timed calls per metric and run (median taken)")
     ap.add_argument("--child", default=None, choices=("fse", "u16"))
+    ap.add_argument("--codecs", default="fse,u16", help="comma-separated subset of fse,u16")
     a = ap.parse_args()
     if a.child:
         child(a.child, a.reps)
         return
-    runs = {"fse": [], "u16": []}
+    runs = {c: [] for c in a.codecs.split(",")}
     info_before = gpu_info()
     for _ in range(a.runs):
         for codec in runs:
