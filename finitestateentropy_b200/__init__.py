@@ -74,6 +74,10 @@ def _declare(L):
         sig("FSEB200_%s_compress_packed" % codec, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp, c_sz, c_vp)
         sig("FSEB200_%s_decompress_packed" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     sig("FSEB200_FSE_packed_workspace", c_sz, c_sz, c_sz)
+    for name in ("FSEB200_HUF_decompress_packed", "FSEB200_HUF_decompress1X_packed"):
+        sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_compress_host_packed", c_sz, C.c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_sz, C.c_uint, C.c_uint)
+    sig("FSEB200_decompress_host_packed", c_sz, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz)
     for name in ("FSEB200_HUF_compress_batch", "FSEB200_FSE_compress_batch", "FSEB200_FSE_decompress_batch",
                  "FSEB200_FSEU16_compress_batch", "FSEB200_FSEU16_decompress_batch"):
         if hasattr(L, name):
@@ -90,4 +94,5 @@ from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch
                     huf_compress_packed, huf_compress1x_packed, packed_pointers,
                     fse_compress_blocks, fse_decompress_blocks, fseu16_compress_blocks, fseu16_decompress_blocks,
                     fse_compress_packed, fseu16_compress_packed, fse_decompress_packed, fseu16_decompress_packed,
-                    fse_packed_workspace)
+                    fse_packed_workspace, huf_decompress_packed, huf_decompress1x_packed,
+                    host_compress_packed, host_decompress_packed)

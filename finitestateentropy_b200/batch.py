@@ -278,15 +278,27 @@ def fse_decompress_packed(packed, offsets, dst_ptrs, dst_sizes, results=None):
     """every block of a packed FSE buffer (fse_compress_packed's out and offsets) into dst_ptrs[b], regenerating dst_sizes[b]
     bytes, on the current stream: a stored length equal to the size is a raw copy, one byte an RLE block, anything else is
     FSE_decompress'ed.  Returns results (int64; the regenerated size or an error code per block)."""
-    return _fse_decompress_packed("FSEB200_FSE_decompress_packed", packed, offsets, dst_ptrs, dst_sizes, results)
+    return _decompress_packed("FSEB200_FSE_decompress_packed", packed, offsets, dst_ptrs, dst_sizes, results)
 
 
 def fseu16_decompress_packed(packed, offsets, dst_ptrs, dst_symbols, results=None):
     """fse_decompress_packed for FSE-U16: dst_symbols[b] 16-bit symbols into dst_ptrs[b] (2-byte aligned); results in symbols"""
-    return _fse_decompress_packed("FSEB200_FSEU16_decompress_packed", packed, offsets, dst_ptrs, dst_symbols, results)
+    return _decompress_packed("FSEB200_FSEU16_decompress_packed", packed, offsets, dst_ptrs, dst_symbols, results)
 
 
-def _fse_decompress_packed(fn_name, packed, offsets, dst_ptrs, dst_sizes, results):
+def huf_decompress_packed(packed, offsets, dst_ptrs, dst_sizes, results=None):
+    """every block of a packed Huff0 buffer (huf_compress_packed's out and offsets) into dst_ptrs[b], regenerating dst_sizes[b]
+    bytes, on the current stream: exactly huf_decompress_blocks on packed_pointers(packed, offsets), except that an empty block
+    (size 0, nothing stored) gives 0.  Returns results (int64; the regenerated size or an error code per block)."""
+    return _decompress_packed("FSEB200_HUF_decompress_packed", packed, offsets, dst_ptrs, dst_sizes, results)
+
+
+def huf_decompress1x_packed(packed, offsets, dst_ptrs, dst_sizes, results=None):
+    """huf_decompress_packed in the single-stream format (huf_compress1x_packed's buffers, huf_decompress1x_blocks per block)"""
+    return _decompress_packed("FSEB200_HUF_decompress1X_packed", packed, offsets, dst_ptrs, dst_sizes, results)
+
+
+def _decompress_packed(fn_name, packed, offsets, dst_ptrs, dst_sizes, results):
     from . import lib
     n = _blocks_args(dst_ptrs, dst_sizes)
     if results is None:
@@ -297,3 +309,80 @@ def _fse_decompress_packed(fn_name, packed, offsets, dst_ptrs, dst_sizes, result
                                 offsets.data_ptr(), _stream_ptr())
     _ret(r, fn_name)
     return results
+
+
+# Host-buffer packed calls (FSEB200_{compress,decompress}_host_packed): name -> (C codec number, bytes per symbol, default
+# maxSymbolValue)
+HOST_CODECS = {"fse": (0, 1, 255), "huf": (1, 1, 255), "fseu16": (2, 2, 0), "huf1x": (3, 1, 255)}
+_NONEMPTY = None
+
+
+def _host_ptr(t):
+    """t's address; an empty tensor has none, and the C calls refuse NULL, so it stands in with a 1-byte buffer"""
+    global _NONEMPTY
+    if t.numel():
+        return t.data_ptr()
+    if _NONEMPTY is None:
+        _NONEMPTY = torch.zeros(8, dtype=torch.uint8)
+    return _NONEMPTY.data_ptr()
+
+
+def _host_check(t, dtype):
+    assert t.device.type == "cpu" and t.is_contiguous() and t.dtype == dtype, (t.device, t.dtype, t.is_contiguous())
+
+
+def _host_sizes(sizes):
+    sizes = torch.as_tensor(sizes, dtype=torch.int64)
+    _host_check(sizes, torch.int64)
+    return sizes
+
+
+def host_compress_packed(src, sizes, codec, out=None, offsets=None, csizes=None, max_symbol_value=None, table_log=12):
+    """The packed compress of `codec` ("fse", "huf", "huf1x" or "fseu16") on HOST memory: block b is sizes[b] symbols of `src`
+    (a CPU uint8 tensor, pinned or pageable; U16 symbols as little-endian byte pairs) right after block b - 1.  `out` (capacity
+    out.numel()), offsets (int64, n + 1 entries) and csizes (int64) are what the device packed call gives for the same blocks;
+    with out=None it is allocated at unit * sum(sizes) + 32 bytes, always enough.  Synchronous.  Returns (out, offsets, csizes)."""
+    from . import lib
+    cid, unit, msv = HOST_CODECS[codec]
+    msv = msv if max_symbol_value is None else max_symbol_value
+    sizes = _host_sizes(sizes)
+    n = sizes.numel()
+    total = unit * int(sizes.sum())
+    _host_check(src, torch.uint8)
+    assert src.numel() >= total, (src.numel(), total)
+    if out is None:
+        out = torch.empty(total + 32, dtype=torch.uint8)
+    if offsets is None:
+        offsets = torch.empty(n + 1, dtype=torch.int64)
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64)
+    _host_check(out, torch.uint8); _host_check(offsets, torch.int64); _host_check(csizes, torch.int64)
+    assert offsets.numel() == n + 1 and csizes.numel() == n, (offsets.numel(), csizes.numel(), n)
+    r = lib().FSEB200_compress_host_packed(cid, _host_ptr(out), out.numel(), offsets.data_ptr(), _host_ptr(csizes), _host_ptr(src),
+                                           _host_ptr(sizes), n, msv, table_log)
+    _ret(r, "FSEB200_compress_host_packed")
+    return out, offsets, csizes
+
+
+def host_decompress_packed(packed, offsets, dst_sizes, codec, out=None, results=None):
+    """The packed decompress of `codec` on HOST memory: every block of `packed` (a CPU uint8 tensor, host_compress_packed's out)
+    located by `offsets`, regenerating dst_sizes[b] symbols; block b lands in `out` right after block b - 1, as in the source.
+    With out=None it is allocated at unit * sum(dst_sizes) bytes.  results (int64) equals the device packed decompress's.
+    Synchronous.  Returns (out, results)."""
+    from . import lib
+    cid, unit, _ = HOST_CODECS[codec]
+    dst_sizes = _host_sizes(dst_sizes)
+    n = dst_sizes.numel()
+    total = unit * int(dst_sizes.sum())
+    _host_check(packed, torch.uint8); _host_check(offsets, torch.int64)
+    assert offsets.numel() == n + 1 and packed.numel() >= int(offsets[-1]), (offsets.numel(), n, packed.numel())
+    if out is None:
+        out = torch.empty(total, dtype=torch.uint8)
+    if results is None:
+        results = torch.empty(n, dtype=torch.int64)
+    _host_check(out, torch.uint8); _host_check(results, torch.int64)
+    assert out.numel() >= total and results.numel() == n, (out.numel(), total, results.numel(), n)
+    r = lib().FSEB200_decompress_host_packed(cid, _host_ptr(out), _host_ptr(dst_sizes), _host_ptr(results), _host_ptr(packed),
+                                             offsets.data_ptr(), n)
+    _ret(r, "FSEB200_decompress_host_packed")
+    return out, results

@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <vector>
 
 namespace fseb {
 cudaError_t launch_huf_decode(const BatchGeom&, void*, const void*, const u64*, u64*, const void*, cudaStream_t, u32 flags);
@@ -34,6 +35,7 @@ cudaError_t launch_fse_encode_blocks(const BlockDescs&, bool, unsigned, unsigned
 cudaError_t launch_fse_decode_blocks(const BlockDescs&, bool, cudaStream_t);
 cudaError_t launch_fse_compress_packed(u8*, u64, u64*, u64*, const u8* const*, const u64*, u32, u8*, u64, bool, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fse_decompress_packed(u8* const*, const u64*, u64*, const u8*, const u64*, u32, bool, cudaStream_t);
+cudaError_t launch_huf_decompress_packed(u8* const*, const u64*, u64*, const u8*, const u64*, u32, int, cudaStream_t);
 cudaError_t launch_hist(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_hist16(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_micro(int, const MicroArgs&, void*, u64*, cudaStream_t);
@@ -256,6 +258,27 @@ FSEB_API size_t FSEB200_HUF_compress1X_packed(size_t nBlocks, void* dOut, size_t
                                               const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
     return huf_packed(nBlocks, dOut, outCapacity, dOffsets, dCSizes, dSrcs, dSrcSizes, 1, maxSymbolValue, tableLog, stream);
+}
+// Packed decompress: the descriptor decoder on dIn + dOffsets[b] / dOffsets[b+1] - dOffsets[b], an empty block answered with 0.
+namespace {
+size_t huf_unpacked(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults, const void* dIn,
+                    const size_t* dOffsets, int nStreams, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || !dDsts || !dDstSizes || !dResults || !dIn || !dOffsets) return (size_t)err(E_SRC_WRONG);
+    return ok_or_generic(launch_huf_decompress_packed((u8* const*)dDsts, (const u64*)dDstSizes, (u64*)dResults, (const u8*)dIn,
+                                                      (const u64*)dOffsets, (u32)nBlocks, nStreams, (cudaStream_t)stream));
+}
+}
+FSEB_API size_t FSEB200_HUF_decompress_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                              const void* dIn, const size_t* dOffsets, void* stream)
+{
+    return huf_unpacked(nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, 4, stream);
+}
+FSEB_API size_t FSEB200_HUF_decompress1X_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                                const void* dIn, const size_t* dOffsets, void* stream)
+{
+    return huf_unpacked(nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, 1, stream);
 }
 namespace {
 size_t fse_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCaps, size_t* dOut, const void* const* dSrcs, const size_t* dSrcSizes,
@@ -1075,4 +1098,228 @@ FSEB_API size_t FSEB200_decompress_host(int codec, void* hDst, size_t dstTotal, 
         }
     }
     return 0;
+}
+
+// ================================================================================================
+// tier 1b, packed: blocks of any size on HOST buffers through the packed device calls, so the stream a host program keeps is
+// the one the device packed calls produce -- one buffer and its offsets, raw and RLE blocks stored in place -- and decodes
+// without the original.  Chunks of blocks, cut by a byte budget, run on alternating streams as in the slot form above; inside a
+// chunk the device packed calls run unchanged on chunk-local offsets with room for every block, and the host turns the results
+// into the whole batch's: global offsets, the capacity rule, only the stored bytes copied down.
+// codec: 0 = FSE, 1 = Huff0 4X, 2 = FSE-U16, 3 = Huff0 1X.
+// ================================================================================================
+namespace {
+struct PackedPipe {
+    enum { NS = 3 };
+    cudaStream_t st[NS] = {};
+    u8* dA[NS] = {};              // uncompressed side
+    u8* dB[NS] = {};              // packed side
+    u8* dW[NS] = {};              // FSE staging slots
+    u64* dD[NS] = {};             // per-block arrays: pointers, sizes, offsets (n + 1), values
+    u64* hD[NS] = {};             // their pinned host images
+    size_t capA = 0, capB = 0, capW = 0, capD = 0, capH = 0;
+    std::mutex mu;
+    template <typename T> static cudaError_t grow(T* (&p)[NS], size_t& cap, size_t need, bool host)
+    {
+        if (need <= cap) return cudaSuccess;
+        for (int i = 0; i < NS; i++) {
+            if (p[i]) { cudaError_t const e = host ? cudaFreeHost(p[i]) : cudaFree(p[i]); p[i] = nullptr; if (e != cudaSuccess) return e; }
+        }
+        cap = 0;
+        for (int i = 0; i < NS; i++) {
+            cudaError_t const e = host ? cudaMallocHost((void**)&p[i], need) : cudaMalloc((void**)&p[i], need);
+            if (e != cudaSuccess) return e;
+        }
+        cap = need;
+        return cudaSuccess;
+    }
+    // `a`, `b`, `w` bytes, `d` words per slot; the packed side gets the decoders' slack
+    cudaError_t ensure(size_t a, size_t b, size_t w, size_t d)
+    {
+        cudaError_t e = cudaSuccess;
+        for (int i = 0; i < NS && e == cudaSuccess; i++) if (!st[i]) e = cudaStreamCreateWithFlags(&st[i], cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = grow(dA, capA, a + 256, false);
+        if (e == cudaSuccess) e = grow(dB, capB, b + 256, false);
+        if (e == cudaSuccess && w) e = grow(dW, capW, w, false);
+        if (e == cudaSuccess) e = grow(dD, capD, d * sizeof(u64), false);
+        if (e == cudaSuccess) e = grow(hD, capH, d * sizeof(u64), true);
+        return e;
+    }
+    // waits for every stream, also after a failure; the first error
+    cudaError_t drain()
+    {
+        cudaError_t first = cudaSuccess;
+        for (int i = 0; i < NS; i++) if (st[i]) { cudaError_t const e = cudaStreamSynchronize(st[i]); if (first == cudaSuccess) first = e; }
+        return first;
+    }
+};
+PackedPipe& ppipe() { static PackedPipe p[MAX_DEVICES]; return p[current_device()]; }
+
+// Bytes per pipeline chunk (FSEB200_HOST_PACKED_CHUNK_BYTES, default 64 MiB).  A block counts its bytes plus 512 for its
+// descriptors and staging overhead, so a chunk of tiny blocks stays bounded too; a block above the budget is a chunk of its own.
+size_t chunk_budget()
+{
+    static size_t const v = [] { const char* e = std::getenv("FSEB200_HOST_PACKED_CHUNK_BYTES"); long long n = e ? std::atoll(e) : 64ll << 20; return (size_t)(n < 1 ? 1 : n); }();
+    return v;
+}
+constexpr u64 BLOCK_OVERHEAD = 512;
+
+struct HostChunk { size_t b0, b1; u64 a0, a1; };   // blocks [b0, b1); uncompressed bytes [a0, a1) of the batch
+
+// chunks of blocks whose weight (uncompressed bytes + the packed bytes `packed(b)` + BLOCK_OVERHEAD) stays within the budget
+template <typename F>
+std::vector<HostChunk> cut_chunks(const size_t* sizes, size_t nBlocks, u64 unit, F packed)
+{
+    std::vector<HostChunk> out;
+    size_t const budget = chunk_budget();
+    HostChunk c = { 0, 0, 0, 0 };
+    u64 w = 0;
+    for (size_t b = 0; b < nBlocks; b++) {
+        u64 const bytes = unit * sizes[b], wb = bytes + packed(b) + BLOCK_OVERHEAD;
+        if (c.b1 > c.b0 && w + wb > budget) { out.push_back(c); c = { b, b, c.a1, c.a1 }; w = 0; }
+        c.b1 = b + 1; c.a1 += bytes; w += wb;
+    }
+    out.push_back(c);
+    return out;
+}
+}
+
+FSEB_API size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
+                                             const void* hSrc, const size_t* hSrcSizes, size_t nBlocks,
+                                             unsigned maxSymbolValue, unsigned tableLog)
+{
+    if (codec < 0 || codec > 3 || nBlocks > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    if (nBlocks == 0) return 0;
+    if (!hOut || !hOffsets || !hCSizes || !hSrc || !hSrcSizes) return (size_t)err(E_SRC_WRONG);
+    bool const fse = codec == 0 || codec == 2, wide = codec == 2;
+    u64 const unit = wide ? 2 : 1;
+    std::vector<HostChunk> const chunks = cut_chunks(hSrcSizes, nBlocks, unit, [](size_t) { return (u64)0; });
+    size_t maxA = 0, maxW = 0, maxD = 0;
+    for (const HostChunk& c : chunks) {
+        size_t const cb = c.b1 - c.b0, a = (size_t)(c.a1 - c.a0);
+        maxA = a > maxA ? a : maxA;
+        maxD = 4 * cb + 1 > maxD ? 4 * cb + 1 : maxD;
+        if (fse) { size_t const w = FSEB200_FSE_packed_workspace(cb, a); maxW = w > maxW ? w : maxW; }
+    }
+    PackedPipe& P = ppipe();
+    std::lock_guard<std::mutex> lock(P.mu);
+    cudaError_t e = P.ensure(maxA, maxA, maxW, maxD);             // a block stores at most its own bytes
+    u64 total = 0;                                                  // global offset of the next chunk's first block
+    // queue: the source and the descriptors up, the packed call with room for every block, offsets and values down
+    auto queue = [&](size_t ci) -> cudaError_t {
+        int const k = (int)(ci % PackedPipe::NS);
+        const HostChunk& c = chunks[ci];
+        size_t const cb = c.b1 - c.b0;
+        u64 const bytes = c.a1 - c.a0;
+        cudaStream_t const s = P.st[k];
+        u64* const h = P.hD[k];
+        u64* const d = P.dD[k];
+        for (size_t b = 0, a = 0; b < cb; b++) { h[b] = reinterpret_cast<u64>(P.dA[k] + a); h[cb + b] = hSrcSizes[c.b0 + b]; a += unit * hSrcSizes[c.b0 + b]; }
+        cudaError_t r;
+        if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        if ((r = cudaMemcpyAsync(d, h, 2 * cb * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        u64* const offs = d + 2 * cb;
+        u64* const vals = d + 3 * cb + 1;
+        if (fse) r = launch_fse_compress_packed(P.dB[k], bytes, offs, vals, (const u8* const*)d, d + cb, (u32)cb, P.dW[k], P.capW, wide,
+                                                maxSymbolValue, tableLog, s);
+        else {
+            PackedDescs g;
+            g.out = P.dB[k]; g.outCap = bytes; g.offset = offs; g.result = vals;
+            g.src = (const u8* const*)d; g.srcSize = d + cb; g.nBlocks = (u32)cb;
+            r = launch_huf_encode_packed(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
+        }
+        if (r != cudaSuccess) return r;
+        return cudaMemcpyAsync(h + 2 * cb, offs, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, s);
+    };
+    // finish: global offsets, the capacity rule of one call over the whole batch, and the stored bytes -- a prefix of the chunk's
+    // packed bytes, since the blocks that fit come first -- copied down
+    auto finish = [&](size_t ci) -> cudaError_t {
+        int const k = (int)(ci % PackedPipe::NS);
+        const HostChunk& c = chunks[ci];
+        size_t const cb = c.b1 - c.b0;
+        cudaError_t r = cudaStreamSynchronize(P.st[k]);
+        if (r != cudaSuccess) return r;
+        const u64* const lo = P.hD[k] + 2 * cb;
+        const u64* const vals = lo + cb + 1;
+        u64 end = 0;
+        for (size_t b = 0; b < cb; b++) {
+            u64 const off = total + lo[b], len = lo[b + 1] - lo[b];
+            u64 v = vals[b];
+            if (!is_err(v) && off + len > outCapacity) v = err(E_DST_TOO_SMALL);
+            else if (!is_err(v) && len) end = lo[b + 1];
+            hOffsets[c.b0 + b] = (size_t)off; hCSizes[c.b0 + b] = (size_t)v;
+        }
+        if (end && (r = cudaMemcpyAsync((u8*)hOut + total, P.dB[k], end, cudaMemcpyDeviceToHost, P.st[k])) != cudaSuccess) return r;
+        total += lo[cb];
+        return cudaSuccess;
+    };
+    size_t const nc = chunks.size(), lag = PackedPipe::NS - 1;
+    for (size_t ci = 0; ci < nc + lag && e == cudaSuccess; ci++) {
+        if (ci >= lag) e = finish(ci - lag);
+        if (e == cudaSuccess && ci < nc) e = queue(ci);
+    }
+    cudaError_t const d = P.drain();
+    if (e != cudaSuccess || d != cudaSuccess) return (size_t)err(E_GENERIC);
+    hOffsets[nBlocks] = (size_t)total;
+    return 0;
+}
+
+FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size_t* hDstSizes, size_t* hResults,
+                                               const void* hIn, const size_t* hOffsets, size_t nBlocks)
+{
+    if (codec < 0 || codec > 3 || nBlocks > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    if (nBlocks == 0) return 0;
+    if (!hDst || !hDstSizes || !hResults || !hIn || !hOffsets) return (size_t)err(E_SRC_WRONG);
+    for (size_t b = 0; b < nBlocks; b++) if (hOffsets[b + 1] < hOffsets[b]) return (size_t)err(E_SRC_WRONG);
+    bool const fse = codec == 0 || codec == 2, wide = codec == 2;
+    u64 const unit = wide ? 2 : 1;
+    std::vector<HostChunk> const chunks = cut_chunks(hDstSizes, nBlocks, unit, [&](size_t b) { return (u64)(hOffsets[b + 1] - hOffsets[b]); });
+    size_t maxA = 0, maxB = 0, maxD = 0;
+    for (const HostChunk& c : chunks) {
+        size_t const cb = c.b1 - c.b0, a = (size_t)(c.a1 - c.a0), in = hOffsets[c.b1] - hOffsets[c.b0];
+        maxA = a > maxA ? a : maxA;
+        maxB = in > maxB ? in : maxB;
+        maxD = 4 * cb + 1 > maxD ? 4 * cb + 1 : maxD;
+    }
+    PackedPipe& P = ppipe();
+    std::lock_guard<std::mutex> lock(P.mu);
+    cudaError_t e = P.ensure(maxA, maxB, 0, maxD);
+    // collect: the results of the chunk that last used slot k, once its stream is done
+    auto collect = [&](size_t ci) -> cudaError_t {
+        int const k = (int)(ci % PackedPipe::NS);
+        size_t const cb = chunks[ci].b1 - chunks[ci].b0;
+        cudaError_t const r = cudaStreamSynchronize(P.st[k]);
+        if (r == cudaSuccess) std::memcpy(hResults + chunks[ci].b0, P.hD[k] + 3 * cb + 1, cb * sizeof(u64));
+        return r;
+    };
+    // queue: the chunk's packed bytes and descriptors up (offsets rebased to the chunk), the packed decompress, the blocks and
+    // their results down
+    auto queue = [&](size_t ci) -> cudaError_t {
+        int const k = (int)(ci % PackedPipe::NS);
+        const HostChunk& c = chunks[ci];
+        size_t const cb = c.b1 - c.b0;
+        u64 const in0 = hOffsets[c.b0], in = hOffsets[c.b1] - in0, bytes = c.a1 - c.a0;
+        cudaStream_t const s = P.st[k];
+        u64* const h = P.hD[k];
+        u64* const d = P.dD[k];
+        for (size_t b = 0, a = 0; b < cb; b++) { h[b] = reinterpret_cast<u64>(P.dA[k] + a); h[cb + b] = hDstSizes[c.b0 + b]; a += unit * hDstSizes[c.b0 + b]; }
+        for (size_t b = 0; b <= cb; b++) h[2 * cb + b] = hOffsets[c.b0 + b] - in0;
+        cudaError_t r;
+        if (in && (r = cudaMemcpyAsync(P.dB[k], (const u8*)hIn + in0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        if ((r = cudaMemcpyAsync(d, h, (3 * cb + 1) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        u8* const* const dsts = (u8* const*)d;
+        u64* const vals = d + 3 * cb + 1;
+        r = fse ? launch_fse_decompress_packed(dsts, d + cb, vals, P.dB[k], d + 2 * cb, (u32)cb, wide, s)
+                : launch_huf_decompress_packed(dsts, d + cb, vals, P.dB[k], d + 2 * cb, (u32)cb, codec == 1 ? 4 : 1, s);
+        if (r != cudaSuccess) return r;
+        if (bytes && (r = cudaMemcpyAsync((u8*)hDst + c.a0, P.dA[k], bytes, cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
+        return cudaMemcpyAsync(h + 3 * cb + 1, vals, cb * sizeof(u64), cudaMemcpyDeviceToHost, s);
+    };
+    size_t const nc = chunks.size();
+    for (size_t ci = 0; ci < nc + PackedPipe::NS && e == cudaSuccess; ci++) {
+        if (ci >= (size_t)PackedPipe::NS) e = collect(ci - PackedPipe::NS);
+        if (e == cudaSuccess && ci < nc) e = queue(ci);
+    }
+    cudaError_t const d = P.drain();
+    return e == cudaSuccess && d == cudaSuccess ? 0 : (size_t)err(E_GENERIC);
 }

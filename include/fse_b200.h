@@ -138,6 +138,24 @@ size_t FSEB200_HUF_compress_packed(size_t nBlocks, void* dOut, size_t outCapacit
 size_t FSEB200_HUF_compress1X_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,
                                      const void* const* dSrcs, const size_t* dSrcSizes,
                                      unsigned maxSymbolValue, unsigned tableLog, void* stream);
+/* Packed decompress (Huff0, 4X and 1X): every block of a buffer the packed compress above wrote, located by its offsets -- the
+ * recipe above without building the descriptor arrays.  Per block b, with L = dOffsets[b+1] - dOffsets[b] and n = dDstSizes[b]
+ * (the regenerated size, not a capacity):
+ *   n == 0 and L == 0: the result is 0 and nothing is written (an empty block as the packed compress stores it);
+ *   otherwise exactly what FSEB200_HUF_decompress_blocks (1X: FSEB200_HUF_decompress1X_blocks) returns for dCSrcs[b] = dIn +
+ *   dOffsets[b], dCSrcSizes[b] = L and dDstSizes[b] = n: a raw copy at L == n, RLE at L == 1, the decoders' limit verdicts, and
+ *   the reference's weight-12 exception above.
+ * So every block the packed compress stored with a value that is not an error decodes back to its source, but for that exception.
+ * All arrays and buffers are in DEVICE memory; the calls are asynchronous on `stream`, the host never reads the arrays, and the
+ * only memory they take is stream-ordered scratch of 16 bytes per block.
+ * Contract: dIn must be readable up to the end of the 32-byte sector that holds each block's last byte; no destination may
+ * overlap another destination, dIn or the arrays, and dResults overlaps no other array.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing and writes nothing); srcSize_wrong if nBlocks > 0xFFFFFFFF
+ * or a pointer is NULL while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_HUF_decompress_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                     const void* dIn, const size_t* dOffsets, void* stream);
+size_t FSEB200_HUF_decompress1X_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                       const void* dIn, const size_t* dOffsets, void* stream);
 
 /* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
  * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
@@ -241,6 +259,33 @@ size_t FSEB200_compress_host(int codec, void* hCBuf, size_t slot, size_t* hCSize
                              size_t blockSize, unsigned maxSymbolValue, unsigned tableLog);
 size_t FSEB200_decompress_host(int codec, void* hDst, size_t dstTotal, size_t blockSize, const void* hCBuf, size_t slot,
                                const size_t* hCSizes, size_t* hResults, const void* hOrig);
+
+/* Tier 1b, packed -- blocks of any size on HOST buffers through the packed device calls above.  The slot form keeps nothing for
+ * a raw block and needs hOrig to regenerate raw and RLE blocks; these calls produce and read the packed device stream instead --
+ * one buffer plus nBlocks + 1 offsets, raw and RLE blocks stored in place -- which decodes without the original.
+ * codec: 0 = FSE, 1 = Huff0 4X, 2 = FSE-U16, 3 = Huff0 1X.  Synchronous.  All pointers are host pointers, pinned or pageable,
+ * with no alignment required.  Let u = 1 (U16: 2) and n_b = hSrcSizes[b] / hDstSizes[b] (U16: symbols).  Blocks lie back to back:
+ * block b of the source starts at hSrc + u * (n_0 + ... + n_{b-1}), and decompress writes block b at the same place in hDst.
+ *   compress:   hCSizes, hOffsets (nBlocks + 1 entries) and hOut[0, min(total, outCapacity)) are byte for byte what the matching
+ *               device packed call (FSEB200_FSE_compress_packed, FSEB200_HUF_compress_packed, FSEB200_FSEU16_compress_packed,
+ *               FSEB200_HUF_compress1X_packed) gives for the same blocks at the same outCapacity, with the blocks on the device
+ *               at an even address and, for FSE, a workspace of FSEB200_FSE_packed_workspace: workSpace_tooSmall never appears.
+ *               Nothing outside the stored blocks is written to hOut; outCapacity = u * sum(n) always holds them all.
+ *   decompress: hResults equals the device packed decompress's (FSEB200_{FSE,HUF,FSEU16}_decompress_packed,
+ *               FSEB200_HUF_decompress1X_packed) for the same stream; for a block whose result is not an error, [0, result)
+ *               holds the regenerated symbols, and the bytes of a block whose result is an error are unspecified.  Nothing
+ *               outside [hDst, hDst + u * sum(n)) is written.  Exactly [hIn + hOffsets[0], hIn + hOffsets[nBlocks]) is read --
+ *               no slack is needed.  Offsets that decrease anywhere give srcSize_wrong.
+ * The batch is cut into chunks of blocks by a byte budget (FSEB200_HOST_PACKED_CHUNK_BYTES, default 64 MiB; a block counts its
+ * bytes plus 512, and one above the budget is a chunk of its own) that overlap their copies and kernels on alternating streams;
+ * only stored bytes cross PCIe.  Calls from several host threads are serialised per device.
+ * Return value: 0 (also for nBlocks == 0, which writes nothing); srcSize_wrong for a bad codec, nBlocks > 0xFFFFFFFF or a NULL
+ * pointer while nBlocks > 0; generic if a CUDA call fails. */
+size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
+                                    const void* hSrc, const size_t* hSrcSizes, size_t nBlocks,
+                                    unsigned maxSymbolValue, unsigned tableLog);
+size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size_t* hDstSizes, size_t* hResults,
+                                      const void* hIn, const size_t* hOffsets, size_t nBlocks);
 
 /* Measurement inputs generated directly in device memory: byte i of the output equals byte
  * (streamOffset + i) of the reference generator's stream (programs/probaGenerator.c:95-126 with
