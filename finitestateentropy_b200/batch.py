@@ -386,3 +386,35 @@ def host_decompress_packed(packed, offsets, dst_sizes, codec, out=None, results=
                                              offsets.data_ptr(), n)
     _ret(r, "FSEB200_decompress_host_packed")
     return out, results
+
+
+# .fse frames (FSEB200_frame_{compress,decompress}_host): codec name -> C codec number
+FRAME_CODECS = {"fse": 0, "huf": 1}
+
+
+def frame_compress(src, codec="fse", block_size_id=5):
+    """src (a CPU uint8 tensor, pinned or pageable) as one .fse frame, byte for byte what the reference's `fse -e` ("fse") or
+    `fse -h` ("huf") with -B<block_size_id> writes (blocks of 1 KB << block_size_id).  Synchronous.  Returns the frame as a CPU
+    uint8 tensor."""
+    from . import lib
+    cid = FRAME_CODECS[codec]
+    _host_check(src, torch.uint8)
+    bound = lib().FSEB200_frame_compressBound(src.numel(), block_size_id)
+    _ret(bound, "FSEB200_frame_compressBound")
+    out = torch.empty(bound, dtype=torch.uint8)
+    r = lib().FSEB200_frame_compress_host(cid, block_size_id, out.data_ptr(), out.numel(), _host_ptr(src), src.numel())
+    _ret(r, "FSEB200_frame_compress_host")
+    return out[:r]
+
+
+def frame_decompress(frame):
+    """the data of an .fse frame (a CPU uint8 tensor), exactly what the reference's `fse -d` writes for it; a frame it rejects
+    raises.  Synchronous.  Returns a CPU uint8 tensor."""
+    from . import lib
+    _host_check(frame, torch.uint8)
+    bound = lib().FSEB200_frame_decompress_bound(_host_ptr(frame), frame.numel())
+    _ret(bound, "FSEB200_frame_decompress_bound")
+    out = torch.empty(bound, dtype=torch.uint8)
+    r = lib().FSEB200_frame_decompress_host(_host_ptr(out), out.numel(), _host_ptr(frame), frame.numel())
+    _ret(r, "FSEB200_frame_decompress_host")
+    return out[:r]

@@ -14,10 +14,12 @@
 #include "micro.h"
 #include "fse_b200.h"
 #include "launch_util.cuh"
+#include "xxh32.h"
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <thread>
 #include <vector>
 
 namespace fseb {
@@ -36,6 +38,8 @@ cudaError_t launch_fse_decode_blocks(const BlockDescs&, bool, cudaStream_t);
 cudaError_t launch_fse_compress_packed(u8*, u64, u64*, u64*, const u8* const*, const u64*, u32, u8*, u64, bool, unsigned, unsigned, cudaStream_t);
 cudaError_t launch_fse_decompress_packed(u8* const*, const u64*, u64*, const u8*, const u64*, u32, bool, cudaStream_t);
 cudaError_t launch_huf_decompress_packed(u8* const*, const u64*, u64*, const u8*, const u64*, u32, int, cudaStream_t);
+cudaError_t launch_frame_body(u8*, const u8*, const u64*, const u64*, const u64*, u32, u64, cudaStream_t);
+cudaError_t launch_frame_stored(u8*, const u8*, const u64*, u64, cudaStream_t);
 cudaError_t launch_hist(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_hist16(const void*, u64, u32, u32*, u64*, cudaStream_t);
 cudaError_t launch_micro(int, const MicroArgs&, void*, u64*, cudaStream_t);
@@ -1182,6 +1186,33 @@ std::vector<HostChunk> cut_chunks(const size_t* sizes, size_t nBlocks, u64 unit,
     out.push_back(c);
     return out;
 }
+
+// Queues chunk c of a host batch through the device packed compress in slot k: the source and the descriptors up, the packed
+// call with room for every block.  On the device the slot's descriptor words are then: source pointers (cb), sizes (cb), offsets
+// (cb + 1), values (cb).  codec as the host packed calls.
+cudaError_t queue_packed_compress(PackedPipe& P, int k, const HostChunk& c, int codec, const void* hSrc, const size_t* hSrcSizes,
+                                  unsigned maxSymbolValue, unsigned tableLog)
+{
+    bool const fse = codec == 0 || codec == 2, wide = codec == 2;
+    u64 const unit = wide ? 2 : 1;
+    size_t const cb = c.b1 - c.b0;
+    u64 const bytes = c.a1 - c.a0;
+    cudaStream_t const s = P.st[k];
+    u64* const h = P.hD[k];
+    u64* const d = P.dD[k];
+    for (size_t b = 0, a = 0; b < cb; b++) { h[b] = reinterpret_cast<u64>(P.dA[k] + a); h[cb + b] = hSrcSizes[c.b0 + b]; a += unit * hSrcSizes[c.b0 + b]; }
+    cudaError_t r;
+    if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+    if ((r = cudaMemcpyAsync(d, h, 2 * cb * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+    u64* const offs = d + 2 * cb;
+    u64* const vals = d + 3 * cb + 1;
+    if (fse) return launch_fse_compress_packed(P.dB[k], bytes, offs, vals, (const u8* const*)d, d + cb, (u32)cb, P.dW[k], P.capW, wide,
+                                               maxSymbolValue, tableLog, s);
+    PackedDescs g;
+    g.out = P.dB[k]; g.outCap = bytes; g.offset = offs; g.result = vals;
+    g.src = (const u8* const*)d; g.srcSize = d + cb; g.nBlocks = (u32)cb;
+    return launch_huf_encode_packed(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
+}
 }
 
 FSEB_API size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
@@ -1208,28 +1239,10 @@ FSEB_API size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCa
     // queue: the source and the descriptors up, the packed call with room for every block, offsets and values down
     auto queue = [&](size_t ci) -> cudaError_t {
         int const k = (int)(ci % PackedPipe::NS);
-        const HostChunk& c = chunks[ci];
-        size_t const cb = c.b1 - c.b0;
-        u64 const bytes = c.a1 - c.a0;
-        cudaStream_t const s = P.st[k];
-        u64* const h = P.hD[k];
-        u64* const d = P.dD[k];
-        for (size_t b = 0, a = 0; b < cb; b++) { h[b] = reinterpret_cast<u64>(P.dA[k] + a); h[cb + b] = hSrcSizes[c.b0 + b]; a += unit * hSrcSizes[c.b0 + b]; }
-        cudaError_t r;
-        if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-        if ((r = cudaMemcpyAsync(d, h, 2 * cb * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-        u64* const offs = d + 2 * cb;
-        u64* const vals = d + 3 * cb + 1;
-        if (fse) r = launch_fse_compress_packed(P.dB[k], bytes, offs, vals, (const u8* const*)d, d + cb, (u32)cb, P.dW[k], P.capW, wide,
-                                                maxSymbolValue, tableLog, s);
-        else {
-            PackedDescs g;
-            g.out = P.dB[k]; g.outCap = bytes; g.offset = offs; g.result = vals;
-            g.src = (const u8* const*)d; g.srcSize = d + cb; g.nBlocks = (u32)cb;
-            r = launch_huf_encode_packed(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
-        }
+        size_t const cb = chunks[ci].b1 - chunks[ci].b0;
+        cudaError_t const r = queue_packed_compress(P, k, chunks[ci], codec, hSrc, hSrcSizes, maxSymbolValue, tableLog);
         if (r != cudaSuccess) return r;
-        return cudaMemcpyAsync(h + 2 * cb, offs, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, s);
+        return cudaMemcpyAsync(P.hD[k] + 2 * cb, P.dD[k] + 2 * cb, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, P.st[k]);
     };
     // finish: global offsets, the capacity rule of one call over the whole batch, and the stored bytes -- a prefix of the chunk's
     // packed bytes, since the blocks that fit come first -- copied down
@@ -1322,4 +1335,309 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
     }
     cudaError_t const d = P.drain();
     return e == cudaSuccess && d == cudaSuccess ? 0 : (size_t)err(E_GENERIC);
+}
+
+// ================================================================================================
+// tier 1b, frames: the .fse format of the reference's file tool (programs/fileio.c:266-626) on host buffers, through the packed
+// pipeline above.  Compress: each chunk runs the device packed compress, then frame.cu lays its frame body out on the device --
+// headers in front of the stored blocks -- so the body comes down in one copy to its place in the frame; a worker thread hashes
+// the whole input meanwhile.  Decompress: the host walks the block headers first (the frame is in host memory), each chunk copies
+// up exactly its own frame bytes, the compressed blocks go to the descriptor decoders and the raw and RLE blocks to frame.cu's
+// stored-block kernel.  An FSE block may decode short, so a chunk's output offset is known only once every earlier chunk's
+// results are in: a chunk is copied down, and hashed in frame order, in the lagged finish step.
+// ================================================================================================
+namespace {
+constexpr u32 MAGIC_FSE = 0x183E2309u, MAGIC_HUF = 0x183E3309u;
+constexpr u64 FRAME_HEADER = 5, FRAME_TRAILER = 3;
+enum { BT_COMPRESSED = 0, BT_RAW = 1, BT_RLE = 2, BT_END = 3 };
+
+u32 trailer_checksum(u32 h) { return (h >> 5) & ((1u << 22) - 1); }
+u64 be16(const u8* p) { return (u64)p[0] << 8 | p[1]; }
+
+struct FrameBlock { u64 head, payload, rSize, cSize; int type; };   // header and payload offsets in the frame
+
+struct FrameWalk {
+    size_t verdict = 0;             // 0, or the verdict where the walk stopped (the point FIO_decompressFilename stops at)
+    int codec = 0;                  // 0 FSE, 1 Huff0
+    std::vector<FrameBlock> blocks; // every block before that point
+    u32 checksum = 0;               // the trailer's 22 bits (verdict 0)
+};
+
+// the reference's header walk, with its exit codes as verdicts; blocks that would overrun its buffers are corruption_detected
+FrameWalk walk_frame(const u8* f, u64 size)
+{
+    FrameWalk w;
+    auto stop = [&w](unsigned code) { w.verdict = (size_t)err(code); };
+    if (size < FRAME_HEADER) { stop(E_SRC_WRONG); return w; }                                  // exit 30
+    u32 const magic = (u32)f[0] | (u32)f[1] << 8 | (u32)f[2] << 16 | (u32)f[3] << 24;
+    if (magic != MAGIC_FSE && magic != MAGIC_HUF) { stop(E_GENERIC); return w; }             // 31 (zlibh too)
+    if (f[4] > 6) { stop(E_GENERIC); return w; }                                              // 32
+    w.codec = magic == MAGIC_HUF;
+    u64 const bs = (u64)1024 << f[4];
+    u64 pos = FRAME_HEADER;
+    if (pos >= size) { stop(E_SRC_WRONG); return w; }                                         // 34
+    for (;;) {
+        FrameBlock k;
+        k.head = pos;
+        k.type = f[pos] >> 6;
+        if (k.type == BT_END) break;
+        bool const full = f[pos] & 0x20;
+        pos++;
+        k.rSize = bs;
+        if (!full) {
+            if (pos + 2 > size) { stop(E_SRC_WRONG); return w; }                              // 35
+            k.rSize = be16(f + pos); pos += 2;
+        }
+        if (k.type == BT_COMPRESSED) {
+            if (pos + 2 > size) { stop(E_SRC_WRONG); return w; }                              // 36
+            k.cSize = be16(f + pos); pos += 2;
+        } else k.cSize = k.type == BT_RAW ? k.rSize : 1;
+        if (k.cSize > bs + 4) { stop(E_CORRUPT); return w; }                                  // past its input buffer
+        if (pos + k.cSize + 1 > size) { stop(E_SRC_WRONG); return w; }                        // 38: payload + next header byte
+        if (k.type != BT_RAW && k.rSize > bs) { stop(E_CORRUPT); return w; }                  // past its output buffer
+        k.payload = pos; pos += k.cSize;
+        w.blocks.push_back(k);
+    }
+    if (pos + FRAME_TRAILER > size) { stop(E_SRC_WRONG); return w; }                          // 43
+    w.checksum = (u32)be16(f + pos + 1) | (u32)(f[pos] & 0x3F) << 16;
+    return w;
+}
+}
+
+FSEB_API unsigned FSEB200_XXH32(const void* src, size_t srcSize, unsigned seed)
+{
+    Xxh32 x(seed);
+    if (srcSize) x.update(src, srcSize);
+    return x.digest();
+}
+
+FSEB_API size_t FSEB200_frame_compressBound(size_t srcSize, unsigned blockSizeId)
+{
+    if (blockSizeId > 6) return (size_t)err(E_SRC_WRONG);
+    size_t const bs = (size_t)1024 << blockSizeId;
+    // the all-raw frame: a full block takes 1 + bs bytes, a partial one 3 + n; a compressed block is shorter than n - 1 bytes
+    // (lib/fse_compress.c, lib/huf_compress.c) behind at most 2 more header bytes, an RLE block 1 byte
+    return FRAME_HEADER + srcSize + srcSize / bs + (srcSize % bs ? 3 : 0) + FRAME_TRAILER;
+}
+
+FSEB_API size_t FSEB200_frame_compress_host(int codec, unsigned blockSizeId, void* hFrame, size_t frameCapacity,
+                                            const void* hSrc, size_t srcSize)
+{
+    if (codec < 0 || codec > 1 || blockSizeId > 6 || (!hSrc && srcSize) || (!hFrame && frameCapacity)) return (size_t)err(E_SRC_WRONG);
+    if (frameCapacity < FRAME_HEADER + FRAME_TRAILER) return (size_t)err(E_DST_TOO_SMALL);
+    u8* const out = (u8*)hFrame;
+    u32 const magic = codec ? MAGIC_HUF : MAGIC_FSE;
+    for (int i = 0; i < 4; i++) out[i] = (u8)(magic >> (8 * i));
+    out[4] = (u8)blockSizeId;
+    u32 hash = 0;
+    std::thread hasher([&hash, hSrc, srcSize] { hash = FSEB200_XXH32(hSrc, srcSize, 0); });
+    size_t const bs = (size_t)1024 << blockSizeId, nb = (srcSize + bs - 1) / bs;
+    size_t verdict = 0;
+    u64 body = 0;                                                   // frame body bytes written so far
+    if (nb) {
+        std::vector<size_t> sizes(nb, bs);
+        sizes[nb - 1] = srcSize - (nb - 1) * bs;
+        std::vector<HostChunk> const chunks = cut_chunks(sizes.data(), nb, 1, [](size_t) { return (u64)0; });
+        size_t maxA = 0, maxF = 0, maxW = 0, maxD = 0;
+        for (const HostChunk& c : chunks) {
+            size_t const cb = c.b1 - c.b0, a = (size_t)(c.a1 - c.a0);
+            maxA = a > maxA ? a : maxA;
+            maxF = a + 5 * cb > maxF ? a + 5 * cb : maxF;           // a body: the stored blocks plus at most 5 header bytes each
+            maxD = 4 * cb + 1 > maxD ? 4 * cb + 1 : maxD;
+            if (codec == 0) { size_t const w = FSEB200_FSE_packed_workspace(cb, a); maxW = w > maxW ? w : maxW; }
+        }
+        PackedPipe& P = ppipe();
+        std::lock_guard<std::mutex> lock(P.mu);
+        cudaError_t e = P.ensure(maxF, maxA, maxW, maxD);          // the body goes to the source's buffer once it is coded
+        // queue: the packed compress, the frame body, the offsets and values down
+        auto queue = [&](size_t ci) -> cudaError_t {
+            int const k = (int)(ci % PackedPipe::NS);
+            size_t const cb = chunks[ci].b1 - chunks[ci].b0;
+            u64* const d = P.dD[k];
+            cudaError_t r = queue_packed_compress(P, k, chunks[ci], codec, hSrc, sizes.data(), 255, 11);
+            if (r == cudaSuccess) r = launch_frame_body(P.dA[k], P.dB[k], d + 2 * cb, d + 3 * cb + 1, d + cb, (u32)cb, bs, P.st[k]);
+            if (r != cudaSuccess) return r;
+            return cudaMemcpyAsync(P.hD[k] + 2 * cb, d + 2 * cb, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, P.st[k]);
+        };
+        // finish: the first error value in block order stops the call (fileio.c:329); otherwise the body comes down if it fits
+        auto finish = [&](size_t ci) -> cudaError_t {
+            int const k = (int)(ci % PackedPipe::NS);
+            const HostChunk& c = chunks[ci];
+            size_t const cb = c.b1 - c.b0;
+            cudaError_t const r = cudaStreamSynchronize(P.st[k]);
+            if (r != cudaSuccess) return r;
+            const u64* const lo = P.hD[k] + 2 * cb;
+            const u64* const vals = lo + cb + 1;
+            u64 len = lo[cb];
+            for (size_t b = 0; b < cb && !verdict; b++) {
+                u64 const v = vals[b];
+                if (is_err(v)) verdict = (size_t)v;
+                len += 1 + (sizes[c.b0 + b] == bs ? 0 : 2) + (v >= 2 ? 2 : 0);
+            }
+            if (!verdict && FRAME_HEADER + body + len + FRAME_TRAILER > frameCapacity) verdict = (size_t)err(E_DST_TOO_SMALL);
+            if (verdict) return cudaSuccess;
+            u64 const at = body;
+            body += len;
+            return cudaMemcpyAsync(out + FRAME_HEADER + at, P.dA[k], len, cudaMemcpyDeviceToHost, P.st[k]);
+        };
+        size_t const nc = chunks.size(), lag = PackedPipe::NS - 1;
+        for (size_t ci = 0; ci < nc + lag && e == cudaSuccess && !verdict; ci++) {
+            if (ci >= lag) e = finish(ci - lag);
+            if (e == cudaSuccess && !verdict && ci < nc) e = queue(ci);
+        }
+        cudaError_t const d = P.drain();
+        if (!verdict && (e != cudaSuccess || d != cudaSuccess)) verdict = (size_t)err(E_GENERIC);
+    }
+    hasher.join();
+    if (verdict) return verdict;
+    u8* const t = out + FRAME_HEADER + body;
+    u32 const crc = trailer_checksum(hash);
+    t[0] = (u8)((crc >> 16) | (BT_END << 6)); t[1] = (u8)(crc >> 8); t[2] = (u8)crc;
+    return (size_t)(FRAME_HEADER + body + FRAME_TRAILER);
+}
+
+FSEB_API size_t FSEB200_frame_decompress_bound(const void* hFrame, size_t frameSize)
+{
+    if (!hFrame && frameSize) return (size_t)err(E_SRC_WRONG);
+    FrameWalk const w = walk_frame((const u8*)hFrame, frameSize);
+    if (w.verdict) return w.verdict;
+    u64 total = 0;
+    for (const FrameBlock& k : w.blocks) total += k.rSize;
+    return (size_t)total;
+}
+
+FSEB_API size_t FSEB200_frame_decompress_host(void* hDst, size_t dstCapacity, const void* hFrame, size_t frameSize)
+{
+    if ((!hFrame && frameSize) || (!hDst && dstCapacity)) return (size_t)err(E_SRC_WRONG);
+    const u8* const f = (const u8*)hFrame;
+    u8* const dst = (u8*)hDst;
+    FrameWalk const w = walk_frame(f, frameSize);
+    const std::vector<FrameBlock>& blk = w.blocks;
+    size_t const nb = blk.size();
+    u64 nominal = 0;
+    bool coded = false;
+    for (const FrameBlock& k : blk) { nominal += k.rSize; coded |= k.type == BT_COMPRESSED; }
+    if (!coded) {                                                   // every block's output size is known: settled here first
+        if (nominal > dstCapacity) return (size_t)err(E_DST_TOO_SMALL);
+        if (w.verdict) return w.verdict;
+    }
+    Xxh32 hash(0);
+    size_t verdict = 0;
+    u64 out = 0;                                                    // bytes regenerated so far
+    if (nb) {
+        std::vector<size_t> rs(nb);
+        for (size_t b = 0; b < nb; b++) rs[b] = (size_t)blk[b].rSize;
+        auto span = [&](size_t b) { return blk[b].payload + blk[b].cSize - blk[b].head; };
+        std::vector<HostChunk> const chunks = cut_chunks(rs.data(), nb, 1, [&](size_t b) { return span(b); });
+        std::vector<size_t> nCoded(chunks.size(), 0);
+        size_t maxA = 0, maxB = 0, maxD = 0;
+        for (size_t ci = 0; ci < chunks.size(); ci++) {
+            const HostChunk& c = chunks[ci];
+            size_t const cb = c.b1 - c.b0, a = (size_t)(c.a1 - c.a0);
+            size_t const in = (size_t)(blk[c.b1 - 1].payload + blk[c.b1 - 1].cSize - blk[c.b0].head);
+            for (size_t b = c.b0; b < c.b1; b++) nCoded[ci] += blk[b].type == BT_COMPRESSED;
+            maxA = a > maxA ? a : maxA;
+            maxB = in > maxB ? in : maxB;
+            maxD = 5 * cb > maxD ? 5 * cb : maxD;
+        }
+        PackedPipe& P = ppipe();
+        std::lock_guard<std::mutex> lock(P.mu);
+        cudaError_t e = P.ensure(maxA, maxB, 0, maxD);
+        // Descriptor words of a chunk with nc compressed and ns stored blocks: destinations, capacities, sources and sizes of
+        // the compressed ones (nc each), the stored-block index (3 ns), then the decoders' results (nc).
+        auto queue = [&](size_t ci) -> cudaError_t {
+            int const k = (int)(ci % PackedPipe::NS);
+            const HostChunk& c = chunks[ci];
+            size_t const cb = c.b1 - c.b0, nc = nCoded[ci], ns = cb - nc;
+            u64 const f0 = blk[c.b0].head, in = blk[c.b1 - 1].payload + blk[c.b1 - 1].cSize - f0;
+            cudaStream_t const s = P.st[k];
+            u64* const h = P.hD[k];
+            u64* const d = P.dD[k];
+            u64* const index = h + 4 * nc;
+            for (size_t b = c.b0, a = 0, j = 0, t = 0; b < c.b1; a += blk[b].rSize, b++) {
+                const FrameBlock& x = blk[b];
+                if (x.type == BT_COMPRESSED) {
+                    h[j] = reinterpret_cast<u64>(P.dA[k] + a); h[nc + j] = x.rSize;
+                    h[2 * nc + j] = reinterpret_cast<u64>(P.dB[k] + (x.payload - f0)); h[3 * nc + j] = x.cSize;
+                    j++;
+                } else {
+                    index[3 * t] = a; index[3 * t + 1] = x.payload - f0; index[3 * t + 2] = x.rSize | (u64)x.type << 32;
+                    t++;
+                }
+            }
+            cudaError_t r;
+            if ((r = cudaMemcpyAsync(P.dB[k], f + f0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+            if ((r = cudaMemcpyAsync(d, h, (4 * nc + 3 * ns) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+            u64* const res = d + 4 * nc + 3 * ns;
+            if (nc) {
+                BlockDescs g;
+                g.dst = (u8* const*)d; g.dstCap = d + nc; g.result = res;
+                g.src = (const u8* const*)(d + 2 * nc); g.srcSize = d + 3 * nc; g.nBlocks = (u32)nc;
+                r = w.codec ? launch_huf_decode_blocks(g, 4, s) : launch_fse_decode_blocks(g, false, s);
+                if (r != cudaSuccess) return r;
+                if ((r = cudaMemcpyAsync(h + 4 * nc + 3 * ns, res, nc * sizeof(u64), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
+            }
+            return ns ? launch_frame_stored(P.dA[k], P.dB[k], d + 4 * nc, ns, s) : cudaSuccess;
+        };
+        // the chunk whose output has been copied down but not hashed yet
+        struct { int k = 0; u64 a = 0, n = 0; } pend;
+        auto hash_pending = [&]() -> cudaError_t {
+            if (!pend.n) return cudaSuccess;
+            cudaError_t const r = cudaStreamSynchronize(P.st[pend.k]);
+            if (r == cudaSuccess) hash.update(dst + pend.a, pend.n);
+            pend.n = 0;
+            return r;
+        };
+        // finish: the first decoder error or overflow of dstCapacity in block order stops the call; otherwise the chunk's output
+        // comes down to its true offset -- in one copy, or block by block when an FSE block decoded short -- and the previous
+        // chunk's output, landed meanwhile, is hashed
+        auto finish = [&](size_t ci) -> cudaError_t {
+            int const k = (int)(ci % PackedPipe::NS);
+            const HostChunk& c = chunks[ci];
+            size_t const nc = nCoded[ci], ns = (c.b1 - c.b0) - nc;
+            cudaError_t r = cudaStreamSynchronize(P.st[k]);
+            if (r != cudaSuccess) return r;
+            const u64* const res = P.hD[k] + 4 * nc + 3 * ns;
+            u64 o = out;
+            bool shortBlock = false;
+            for (size_t b = c.b0, j = 0; b < c.b1 && !verdict; b++) {
+                u64 n = blk[b].rSize;
+                if (blk[b].type == BT_COMPRESSED) {
+                    u64 const v = res[j++];
+                    if (is_err(v)) { verdict = (size_t)v; break; }
+                    shortBlock |= v != n;
+                    n = v;
+                }
+                if (o + n > dstCapacity) verdict = (size_t)err(E_DST_TOO_SMALL);
+                o += n;
+            }
+            if (verdict) return cudaSuccess;
+            if (!shortBlock) {
+                if (o > out && (r = cudaMemcpyAsync(dst + out, P.dA[k], o - out, cudaMemcpyDeviceToHost, P.st[k])) != cudaSuccess) return r;
+            } else {
+                u64 at = out;
+                for (size_t b = c.b0, a = 0, j = 0; b < c.b1; a += blk[b].rSize, b++) {
+                    u64 const n = blk[b].type == BT_COMPRESSED ? res[j++] : blk[b].rSize;
+                    if (n && (r = cudaMemcpyAsync(dst + at, P.dA[k] + a, n, cudaMemcpyDeviceToHost, P.st[k])) != cudaSuccess) return r;
+                    at += n;
+                }
+            }
+            if ((r = hash_pending()) != cudaSuccess) return r;
+            pend.k = k; pend.a = out; pend.n = o - out;
+            out = o;
+            return cudaSuccess;
+        };
+        size_t const nChunks = chunks.size(), lag = PackedPipe::NS - 1;
+        for (size_t ci = 0; ci < nChunks + lag && e == cudaSuccess && !verdict; ci++) {
+            if (ci >= lag) e = finish(ci - lag);
+            if (e == cudaSuccess && !verdict && ci < nChunks) e = queue(ci);
+        }
+        if (e == cudaSuccess && !verdict) e = hash_pending();
+        cudaError_t const d = P.drain();
+        if (!verdict && (e != cudaSuccess || d != cudaSuccess)) verdict = (size_t)err(E_GENERIC);
+    }
+    if (verdict) return verdict;
+    if (w.verdict) return w.verdict;
+    if (trailer_checksum(hash.digest()) != w.checksum) return (size_t)err(E_CORRUPT);   // exit 44
+    return (size_t)out;
 }

@@ -135,19 +135,6 @@ __global__ void __launch_bounds__(CLASSIFY_THREADS) fse_unpack_classify_kernel(F
     g.decSize[b] = stored_kind<WIDE>(g, b, L) == DECODE ? L : 0;
 }
 
-// n unit copies from s (1 byte; U16: 2 bytes, d even) to d by the CTA: 16-byte stores in the aligned interior
-template <bool WIDE>
-__device__ __forceinline__ void cta_fill(u8* const d, const u8* const s, u32 const nb)
-{
-    u32 const w = WIDE ? ((u32)s[0] | (u32)s[1] << 8) * 0x10001u : (u32)s[0] * 0x01010101u;
-    u32 const head = min((u32)(-reinterpret_cast<u64>(d) & 15), nb);   // even for U16: the pattern stays in phase
-    u32 const nChunks = (nb - head) / 16, tailBeg = head + 16 * nChunks;
-    for (u32 i = threadIdx.x; i < head; i += blockDim.x) d[i] = (u8)(w >> (8 * (i & 3)));
-    for (u32 i = tailBeg + threadIdx.x; i < nb; i += blockDim.x) d[i] = (u8)(w >> (8 * (i & 3)));
-    uint4* const dp = reinterpret_cast<uint4*>(d + head);
-    for (u32 k = threadIdx.x; k < nChunks; k += blockDim.x) dp[k] = make_uint4(w, w, w, w);
-}
-
 // after the decoder, one CTA per block (blocks b0 + blockIdx.x): raw and RLE blocks and their results
 template <bool WIDE>
 __global__ void __launch_bounds__(pack::COPY_THREADS)
@@ -160,7 +147,7 @@ fse_unpack_stored_kernel(FseUnpack g, u64 b0)
     u64 const n = g.dstSize[b];
     u32 const nb = (u32)(WIDE ? 2 * n : n);                         // at most 2^30
     if (kind == RAW) pack::cta_copy<pack::COPY_THREADS, pack::COPY_UNROLL>(g.dst[b], g.in + off, nb);
-    else cta_fill<WIDE>(g.dst[b], g.in + off, nb);
+    else pack::cta_fill<WIDE>(g.dst[b], g.in + off, nb);
     if (threadIdx.x == 0) g.result[b] = n;
 }
 

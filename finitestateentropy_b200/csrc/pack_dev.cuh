@@ -1,5 +1,5 @@
 // pack_dev.cuh -- placing variable-length blocks back to back in one device buffer, shared by the packed calls of both codecs
-// (huf_encode.cu: Huff0 compress; fse_packed.cu: FSE / FSE-U16 compress and decompress).
+// (huf_encode.cu: Huff0 compress; fse_packed.cu: FSE / FSE-U16 compress and decompress) and the .fse frame calls (frame.cu).
 //
 // Offsets: a device-wide exclusive scan of per-block lengths, reduce-then-scan over tiles of PACK_TILE blocks -- the tiles'
 // sums (pack_sums_kernel), their exclusive scan in one CTA starting from a carried-in total (pack_scan_tiles_kernel), then the
@@ -9,7 +9,7 @@
 //   P::value(g, b)                         the per-block word the length derives from (read once per block by the place step)
 //   P::len(g, b, v)                        the bytes block b takes
 //   P::place(g, aux, b, v, off, len)       what the place step does for block b at offset off
-// Copies: cta_copy, one CTA moving one block with 16-byte aligned destination stores.
+// Copies: cta_copy, one CTA moving one block with 16-byte aligned destination stores; cta_fill, one CTA writing a run of one unit.
 #pragma once
 #include "common.cuh"
 
@@ -150,6 +150,19 @@ __device__ __forceinline__ void cta_copy(u8* const d, const u8* const s, u32 con
                                __funnelshift_r(y[2], y[3], r), __funnelshift_r(y[3], y[4], r));
         }
     }
+}
+
+// nb bytes of copies of the unit at s (1 byte; WIDE: 2 bytes, d even) to d by the CTA: 16-byte stores in the aligned interior
+template <bool WIDE>
+__device__ __forceinline__ void cta_fill(u8* const d, const u8* const s, u32 const nb)
+{
+    u32 const w = WIDE ? ((u32)s[0] | (u32)s[1] << 8) * 0x10001u : (u32)s[0] * 0x01010101u;
+    u32 const head = min((u32)(-reinterpret_cast<u64>(d) & 15), nb);   // even for U16: the pattern stays in phase
+    u32 const nChunks = (nb - head) / 16, tailBeg = head + 16 * nChunks;
+    for (u32 i = threadIdx.x; i < head; i += blockDim.x) d[i] = (u8)(w >> (8 * (i & 3)));
+    for (u32 i = tailBeg + threadIdx.x; i < nb; i += blockDim.x) d[i] = (u8)(w >> (8 * (i & 3)));
+    uint4* const dp = reinterpret_cast<uint4*>(d + head);
+    for (u32 k = threadIdx.x; k < nChunks; k += blockDim.x) dp[k] = make_uint4(w, w, w, w);
 }
 
 }  // namespace pack

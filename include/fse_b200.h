@@ -287,6 +287,50 @@ size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCapacity, s
 size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size_t* hDstSizes, size_t* hResults,
                                       const void* hIn, const size_t* hOffsets, size_t nBlocks);
 
+/* Tier 1b, frames -- the self-describing .fse format of the reference's file tool (programs/fileio.c:266-626) on HOST buffers:
+ *   frame   = LE32 magic (0x183E2309 FSE, 0x183E3309 Huff0), 1 byte block-size id (block = 1 KB << id, id <= 6),
+ *             { block header, payload }*, 3-byte trailer
+ *   header  = 1 byte { type:2 (0 compressed, 1 raw, 2 RLE, 3 trailer), full:1, 0:5 }, then the regenerated size rSize (2 bytes,
+ *             big endian) unless the block is full (rSize = block size), then the compressed size cSize (2 bytes, big endian)
+ *             if it is compressed; the payload is cSize compressed bytes, rSize raw bytes, or the 1 byte of an RLE block
+ *   trailer = type 3 in the top 2 bits, then the 22 bits (XXH32(data, seed 0) >> 5), big endian.
+ * Synchronous; host pointers, pinned or pageable, at any alignment.  They run through the packed host pipeline above (its chunks
+ * and FSEB200_HOST_PACKED_CHUNK_BYTES budget) and are serialised per device with the packed host calls.
+ *   compress:   codec 0 = FSE, 1 = Huff0.  Returns the frame size; the frame is byte for byte what the reference's writer,
+ *               FIO_compressFilename, writes at that block-size id (its `fse -e` / `fse -h` command line writes id 5; its -B
+ *               option sets the benchmark's block size): ceil(srcSize / block) blocks and no empty one, each
+ *               coded as FSE_compress / HUF_compress code it, i.e. at (maxSymbolValue 255, tableLog 11); a value of 0 makes a raw
+ *               block, 1 an RLE block.  An empty input gives the 8-byte frame of header and trailer.  The trailer's checksum is
+ *               computed on a host thread while the chunks run on the device.  frameCapacity >= FSEB200_frame_compressBound
+ *               always suffices; a frame that does not fit gives dstSize_tooSmall, and nothing past frameCapacity is written.
+ *               srcSize_wrong for a bad codec, blockSizeId > 6, or a NULL pointer with srcSize > 0 (hSrc) or frameCapacity > 0
+ *               (hFrame); the error value of a block, should one occur, stops the call as it stops the reference's tool.
+ *   compressBound: the size of the frame with every block raw, which no frame of srcSize bytes exceeds; srcSize_wrong for
+ *               blockSizeId > 6.  Host-side only.
+ *   decompress: returns what `fse -d` writes, in bytes, and hDst holds exactly those bytes.  A block is dispatched by the type in
+ *               its header: a compressed block goes to FSE_decompress / HUF_decompress (as FSEB200_FSE_decompress_blocks /
+ *               FSEB200_HUF_decompress_blocks) with capacity rSize and contributes what they return -- FSE may return less than
+ *               rSize --, a raw block contributes its payload, an RLE block rSize copies of its byte.  Bytes after the trailer
+ *               are never read.  A failure returns the verdict at the first point, in frame order, where the reference's tool
+ *               stops; hDst's contents are then unspecified:
+ *                 too few bytes for a header, a size field, a payload plus the next header byte, or the trailer: srcSize_wrong;
+ *                 an unknown magic number (zlibh frames included) or a block-size id above 6: GENERIC;
+ *                 a compressed block the decoder rejects: its error code;
+ *                 a checksum mismatch: corruption_detected;
+ *                 a block that would overrun the reference's buffers -- rSize above the block size for a compressed or RLE
+ *                 block, a payload above block size + 4 bytes: corruption_detected;
+ *                 output beyond dstCapacity: dstSize_tooSmall, with nothing written past dstCapacity.
+ *               srcSize_wrong also for a NULL hFrame with frameSize > 0 or a NULL hDst with dstCapacity > 0.
+ *   decompress_bound: the sum of the headers' rSize -- an upper bound on decompress's result, equal to it unless an FSE block
+ *               decodes short -- or the verdict of the header walk (the structural verdicts above).  Host-side only.
+ * FSEB200_XXH32 is the library's XXH32 (the public xxHash specification), the hash behind the trailer. */
+size_t   FSEB200_frame_compressBound(size_t srcSize, unsigned blockSizeId);
+size_t   FSEB200_frame_compress_host(int codec, unsigned blockSizeId, void* hFrame, size_t frameCapacity,
+                                     const void* hSrc, size_t srcSize);
+size_t   FSEB200_frame_decompress_bound(const void* hFrame, size_t frameSize);
+size_t   FSEB200_frame_decompress_host(void* hDst, size_t dstCapacity, const void* hFrame, size_t frameSize);
+unsigned FSEB200_XXH32(const void* src, size_t srcSize, unsigned seed);
+
 /* Measurement inputs generated directly in device memory: byte i of the output equals byte
  * (streamOffset + i) of the reference generator's stream (programs/probaGenerator.c:95-126 with
  * probability p, seed 1; programs/fuzzerU16.c:107-134 with the given start / p / seed). */

@@ -1,68 +1,25 @@
 /*
  * fse_b200_file.c -- the `.fse` frame format on top of libfse_b200 (SURVEY.md section 8f-2).
  *
- * Reads and writes exactly the container of the reference's file tool:
- *   frame   = LE32 magic (0x183E2309 FSE | 0x183E3309 Huff0) , 1 byte block-size id (block = 1 KB << id, id <= 6)
- *             { block header , payload }* , 3-byte trailer                       programs/fileio.c:121-128,266-285
- *   block   = 1 byte { type:2 (0 compressed, 1 raw, 2 rle, 3 end) , full:1 , 0:5 }
- *             [ 2 bytes regenerated size, big endian, unless `full` ]
- *             [ 2 bytes compressed size, big endian, if type == compressed ]       fileio.c:331-407,520-560
- *   trailer = type 3 in the top 2 bits + 22 bits of (XXH32(original, seed 0) >> 5), big endian   fileio.c:412-420,600-606
- * and codes every block with the library's one-liners' parameters, (maxSymbolValue 255, tableLog 11), as
- * FIO_compressFilename does through FSE_compress / HUF_compress (fileio.c:308,312).  A file written here is byte-identical
- * to the one `fse -e` / `fse -h` of the reference writes, and either tool decodes the other's output
- * (tests/test_frame_gpu.py checks both against the reference CLI compiled from the unmodified sources).
- *
- * What differs is the shape of the work: the reference codes one block per fread(); this tool hands ALL blocks of the file
- * to the GPU in one batched call (FSEB200_compress_host / FSEB200_decompress_host, include/fse_b200.h) and only then
- * walks the per-block results to lay the frame out.  Host code is plain C over the C-ABI; the checksum is the frame's own
- * integrity trailer (host side in the reference too), not part of the codec path.
+ * Reads and writes exactly the container of the reference's file tool (programs/fileio.c:121-128,266-626): a file written here
+ * is byte-identical to the one `fse -e` / `fse -h` of the reference writes, and either tool decodes the other's output
+ * (tests/test_frame_gpu.py checks both against the reference CLI compiled from the unmodified sources).  The layout, the coding
+ * parameters and the checksum are the library's: FSEB200_frame_compress_host / FSEB200_frame_decompress_host
+ * (include/fse_b200.h) code the whole file in one call each, so this program is file I/O around them.
  *
  * usage: fse_b200_file [-e | -h] [-B<id>] <input> <output>      compress (default -e = FSE)
  *        fse_b200_file -d <input> <output>                      decompress (codec from the magic number)
  */
-#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include "fse_b200.h"
 
-#define MAGIC_FSE 0x183E2309u
-#define MAGIC_HUF 0x183E3309u
-enum { BT_COMPRESSED = 0, BT_RAW = 1, BT_RLE = 2, BT_END = 3 };
-#define FULL_BIT 0x20
-
 static void die(const char* what)
 {
     fprintf(stderr, "fse_b200_file: %s\n", what);
     exit(1);
-}
-
-/* ---- XXH32 (public xxHash specification), one shot ---- */
-static uint32_t rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-static uint32_t rd32le(const unsigned char* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
-static uint32_t xxh32(const unsigned char* p, size_t len, uint32_t seed)
-{
-    const uint32_t P1 = 2654435761u, P2 = 2246822519u, P3 = 3266489917u, P4 = 668265263u, P5 = 374761393u;
-    const unsigned char* const end = p + len;
-    uint32_t h;
-    if (len >= 16) {
-        const unsigned char* const limit = end - 16;
-        uint32_t v1 = seed + P1 + P2, v2 = seed + P2, v3 = seed, v4 = seed - P1;
-        do {
-            v1 = rotl32(v1 + rd32le(p) * P2, 13) * P1; p += 4;
-            v2 = rotl32(v2 + rd32le(p) * P2, 13) * P1; p += 4;
-            v3 = rotl32(v3 + rd32le(p) * P2, 13) * P1; p += 4;
-            v4 = rotl32(v4 + rd32le(p) * P2, 13) * P1; p += 4;
-        } while (p <= limit);
-        h = rotl32(v1, 1) + rotl32(v2, 7) + rotl32(v3, 12) + rotl32(v4, 18);
-    } else h = seed + P5;
-    h += (uint32_t)len;
-    while (p + 4 <= end) { h = rotl32(h + rd32le(p) * P3, 17) * P4; p += 4; }
-    while (p < end) { h = rotl32(h + (*p) * P5, 11) * P1; p++; }
-    h ^= h >> 15; h *= P2; h ^= h >> 13; h *= P3; h ^= h >> 16;
-    return h;
 }
 
 static unsigned char* read_file(const char* name, size_t* size)
@@ -72,170 +29,54 @@ static unsigned char* read_file(const char* name, size_t* size)
     long n;
     if (!f) die("cannot open input");
     if (fseek(f, 0, SEEK_END) != 0 || (n = ftell(f)) < 0 || fseek(f, 0, SEEK_SET) != 0) die("cannot size input");
-    buf = (unsigned char*)malloc((size_t)n + 64);
+    buf = (unsigned char*)malloc((size_t)n + 1);
     if (!buf) die("out of memory");
     if (n && fread(buf, 1, (size_t)n, f) != (size_t)n) die("read error");
-    memset(buf + n, 0, 64);
     fclose(f);
     *size = (size_t)n;
     return buf;
 }
 
-static void put(FILE* f, const void* p, size_t n)
+static void write_file(const char* name, const void* p, size_t n)
 {
+    FILE* f = fopen(name, "wb");
+    if (!f) die("cannot open output");
     if (n && fwrite(p, 1, n, f) != n) die("write error");
+    if (fclose(f) != 0) die("write error");
 }
 
-/* ------------------------------------------------------------------------------------------------ */
 static int compress_file(const char* in, const char* out, int codec, unsigned blockId)
 {
-    size_t n, nb, b;
+    size_t n, cap, r;
     unsigned char* const src = read_file(in, &n);
-    size_t const blockSize = (size_t)1024 << blockId;
-    size_t const slot = FSE_compressBound(blockSize);                 /* fileio.c:294 */
-    unsigned char* cbuf;
-    size_t* cs;
-    FILE* f;
-    unsigned char hdr[5];
-    unsigned long long written = 5;
-
-    nb = (n + blockSize - 1) / blockSize;                             /* fread() returning 0 ends the reference's loop: no empty block */
-    cbuf = (unsigned char*)malloc(nb * slot + 64);
-    cs = (size_t*)malloc((nb + 1) * sizeof(size_t));
-    if (!cbuf || !cs) die("out of memory");
-    if (nb) {
-        size_t const r = FSEB200_compress_host(codec, cbuf, slot, cs, src, n, blockSize, 255, 11);   /* FSE_compress / HUF_compress defaults */
-        if (FSE_isError(r)) die(FSE_getErrorName(r));
-    }
-    f = fopen(out, "wb");
-    if (!f) die("cannot open output");
-    hdr[0] = (unsigned char)(codec ? MAGIC_HUF : MAGIC_FSE); hdr[1] = (unsigned char)((codec ? MAGIC_HUF : MAGIC_FSE) >> 8);
-    hdr[2] = (unsigned char)((codec ? MAGIC_HUF : MAGIC_FSE) >> 16); hdr[3] = (unsigned char)((codec ? MAGIC_HUF : MAGIC_FSE) >> 24);
-    hdr[4] = (unsigned char)blockId;
-    put(f, hdr, 5);
-    for (b = 0; b < nb; b++) {
-        size_t const off = b * blockSize;
-        size_t const inSize = (off + blockSize <= n) ? blockSize : n - off;
-        size_t const c = cs[b];
-        int const full = (inSize == blockSize);
-        unsigned type;
-        unsigned char h[5]; size_t hn = 0;
-        if (FSE_isError(c)) die(FSE_getErrorName(c));                 /* fileio.c:329 */
-        type = (c == 0) ? BT_RAW : (c == 1) ? BT_RLE : BT_COMPRESSED;
-        h[hn++] = (unsigned char)((type << 6) | (full ? FULL_BIT : 0));
-        if (!full) { h[hn++] = (unsigned char)(inSize >> 8); h[hn++] = (unsigned char)inSize; }
-        if (type == BT_COMPRESSED) { h[hn++] = (unsigned char)(c >> 8); h[hn++] = (unsigned char)c; }
-        put(f, h, hn);
-        if (type == BT_RAW) put(f, src + off, inSize);
-        else if (type == BT_RLE) put(f, src + off, 1);
-        else put(f, cbuf + b * slot, c);
-        written += hn + (type == BT_RAW ? inSize : type == BT_RLE ? 1 : c);
-    }
-    {   uint32_t const crc = (xxh32(src, n, 0) >> 5) & ((1u << 22) - 1);
-        unsigned char t[3];
-        t[0] = (unsigned char)((crc >> 16) + (BT_END << 6)); t[1] = (unsigned char)(crc >> 8); t[2] = (unsigned char)crc;
-        put(f, t, 3); written += 3;
-    }
-    fclose(f);
-    fprintf(stderr, "Compressed %llu bytes into %llu bytes ==> %.2f%%\n", (unsigned long long)n, written, n ? 100.0 * (double)written / (double)n : 0.0);
-    free(cbuf); free(cs); free(src);
+    unsigned char* frame;
+    cap = FSEB200_frame_compressBound(n, blockId);
+    if (FSE_isError(cap)) die(FSE_getErrorName(cap));
+    frame = (unsigned char*)malloc(cap);
+    if (!frame) die("out of memory");
+    r = FSEB200_frame_compress_host(codec, blockId, frame, cap, src, n);
+    if (FSE_isError(r)) die(FSE_getErrorName(r));
+    write_file(out, frame, r);
+    fprintf(stderr, "Compressed %llu bytes into %llu bytes ==> %.2f%%\n", (unsigned long long)n, (unsigned long long)r,
+            n ? 100.0 * (double)r / (double)n : 0.0);
+    free(frame); free(src);
     return 0;
 }
 
-/* ------------------------------------------------------------------------------------------------ */
-typedef struct { unsigned type; size_t rSize, cSize; const unsigned char* payload; } blk_t;
-
 static int decompress_file(const char* in, const char* out)
 {
-    size_t n, pos, nb = 0, cap = 1024, b, total = 0;
-    unsigned char* const src = read_file(in, &n);
-    blk_t* blk = (blk_t*)malloc(cap * sizeof(blk_t));
-    uint32_t magic, crcSaved;
-    int codec, uniform = 1;
-    size_t blockSize;
+    size_t n, bound, r;
+    unsigned char* const frame = read_file(in, &n);
     unsigned char* dst;
-    FILE* f;
-
-    if (!blk) die("out of memory");
-    if (n < 5 + 3) die("Read error : cannot read header");
-    magic = rd32le(src);
-    if (magic == MAGIC_FSE) codec = 0; else if (magic == MAGIC_HUF) codec = 1; else die("Wrong file type : unknown header");
-    if (src[4] > 6) die("Wrong version : unknown header flags");
-    blockSize = (size_t)1024 << src[4];
-    /* pass 1: walk the block headers (fileio.c:520-560) */
-    pos = 5;
-    for (;;) {
-        unsigned type; int full; blk_t k;
-        if (pos >= n) die("Read error : cannot read header");
-        type = src[pos] >> 6; full = src[pos] & FULL_BIT;
-        if (type == BT_END) break;
-        pos++;
-        k.type = type; k.rSize = blockSize;
-        if (!full) { if (pos + 2 > n) die("Read error : cannot read header"); k.rSize = ((size_t)src[pos] << 8) + src[pos + 1]; pos += 2; }
-        if (type == BT_COMPRESSED) { if (pos + 2 > n) die("Read error : cannot read header"); k.cSize = ((size_t)src[pos] << 8) + src[pos + 1]; pos += 2; }
-        else k.cSize = (type == BT_RAW) ? k.rSize : 1;
-        if (pos + k.cSize + 1 > n) die("Read error");                                  /* the payload and the next header byte */
-        if (k.rSize > blockSize) die("Decoding error : block larger than the frame's block size");
-        k.payload = src + pos; pos += k.cSize;
-        if (nb == cap) { cap *= 2; blk = (blk_t*)realloc(blk, cap * sizeof(blk_t)); if (!blk) die("out of memory"); }
-        blk[nb++] = k; total += k.rSize;
-    }
-    if (pos + 3 > n) die("Read error");
-    crcSaved = (uint32_t)src[pos + 2] + ((uint32_t)src[pos + 1] << 8) + (((uint32_t)src[pos] & 0x3F) << 16);
-    for (b = 0; b + 1 < nb; b++) if (blk[b].rSize != blockSize) uniform = 0;
-    dst = (unsigned char*)malloc(total + 64);
+    bound = FSEB200_frame_decompress_bound(frame, n);
+    if (FSE_isError(bound)) die(FSE_getErrorName(bound));
+    dst = (unsigned char*)malloc(bound + 1);
     if (!dst) die("out of memory");
-
-    if (uniform && nb) {
-        /* every block but the last is full: the frame has the uniform geometry of the batched call -- one GPU call for all
-         * compressed blocks; stored / run-length blocks are marked 0 (skipped by the kernels) and filled here */
-        size_t const slot = FSE_compressBound(blockSize);
-        unsigned char* const cbuf = (unsigned char*)calloc(nb * slot + 64, 1);
-        size_t* const cs = (size_t*)malloc(nb * sizeof(size_t));
-        size_t* const res = (size_t*)malloc(nb * sizeof(size_t));
-        size_t r;
-        if (!cbuf || !cs || !res) die("out of memory");
-        for (b = 0; b < nb; b++) {
-            if (blk[b].type == BT_COMPRESSED) {
-                if (blk[b].cSize > slot) die("Decoding error : compressed block larger than its bound");
-                memcpy(cbuf + b * slot, blk[b].payload, blk[b].cSize); cs[b] = blk[b].cSize;
-                if (cs[b] < 2) die("Decoding error : corrupted block header");
-            } else cs[b] = 0;
-        }
-        r = FSEB200_decompress_host(codec, dst, total, blockSize, cbuf, slot, cs, res, NULL);
-        if (FSE_isError(r)) die(FSE_getErrorName(r));
-        for (b = 0; b < nb; b++) {
-            unsigned char* const o = dst + b * blockSize;
-            if (blk[b].type == BT_RAW) memcpy(o, blk[b].payload, blk[b].rSize);
-            else if (blk[b].type == BT_RLE) memset(o, blk[b].payload[0], blk[b].rSize);
-            else {
-                if (FSE_isError(res[b])) { fprintf(stderr, "fse_b200_file: Decoding error : %s\n", FSE_getErrorName(res[b])); exit(1); }   /* fileio.c:565-567 */
-                if (res[b] != blk[b].rSize && codec == 1) die("Decoding error : size mismatch");
-            }
-        }
-        free(cbuf); free(cs); free(res);
-    } else {
-        /* a frame with odd-sized interior blocks (the reference's writer never makes one): one call per block */
-        size_t off = 0;
-        for (b = 0; b < nb; b++) {
-            unsigned char* const o = dst + off;
-            if (blk[b].type == BT_RAW) memcpy(o, blk[b].payload, blk[b].rSize);
-            else if (blk[b].type == BT_RLE) memset(o, blk[b].payload[0], blk[b].rSize);
-            else {
-                size_t const r = codec ? HUF_decompress(o, blk[b].rSize, blk[b].payload, blk[b].cSize)
-                                       : FSE_decompress(o, blk[b].rSize, blk[b].payload, blk[b].cSize);
-                if (FSE_isError(r)) { fprintf(stderr, "fse_b200_file: Decoding error : %s\n", FSE_getErrorName(r)); exit(1); }
-            }
-            off += blk[b].rSize;
-        }
-    }
-    if (((xxh32(dst, total, 0) >> 5) & ((1u << 22) - 1)) != crcSaved) die("CRC error : wrong checksum, corrupted data");   /* fileio.c:603-606 */
-    f = fopen(out, "wb");
-    if (!f) die("cannot open output");
-    put(f, dst, total);
-    fclose(f);
-    fprintf(stderr, "Decoded %llu bytes\n", (unsigned long long)total);
-    free(dst); free(blk); free(src);
+    r = FSEB200_frame_decompress_host(dst, bound, frame, n);
+    if (FSE_isError(r)) { fprintf(stderr, "fse_b200_file: Decoding error : %s\n", FSE_getErrorName(r)); exit(1); }
+    write_file(out, dst, r);
+    fprintf(stderr, "Decoded %llu bytes\n", (unsigned long long)r);
+    free(dst); free(frame);
     return 0;
 }
 
