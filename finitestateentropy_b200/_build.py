@@ -10,14 +10,15 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfse_b200.so")
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
-              "-Xcompiler", "-fPIC,-fvisibility=hidden", "--shared", "-cudart", "static"]
+              "-Xcompiler", "-fPIC,-fvisibility=hidden", "--shared", "-cudart", "static",
+              "-Xlinker", "-z,defs"]   # an undefined symbol (a launcher declared unlike its definition) fails the link, not the load
 
 
 def lib_is_stale():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    srcs = glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")) + \
+    srcs = glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) + \
         glob.glob(os.path.join(ROOT, "include", "*.h"))
     return any(os.path.getmtime(s) > t for s in srcs)
 

@@ -12,6 +12,7 @@
 // Decompress, per chunk: the compressed blocks go to the descriptor decoders with pointers into the chunk's frame bytes (the host
 // builds the descriptors); raw and RLE blocks come from frame_stored_kernel, one CTA per block of a compact index.
 #include "common.cuh"
+#include "launchers.h"
 #include "launch_util.cuh"
 #include "pack_dev.cuh"
 

@@ -21,6 +21,7 @@
 //   fse_encode_kernel      warp per block; takes the ragged last block and unaligned geometries
 #include <cstdlib>
 #include "common.cuh"
+#include "launchers.h"
 #include "launch_util.cuh"
 #include "fse_dev.cuh"
 #include "bitsrc_dev.cuh"

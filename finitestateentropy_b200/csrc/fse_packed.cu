@@ -15,13 +15,11 @@
 // decoder settles at once without writing), the descriptor decoder runs on them, then a raw / RLE kernel writes those blocks and
 // their results.
 #include "common.cuh"
+#include "launchers.h"
 #include "launch_util.cuh"
 #include "pack_dev.cuh"
 
 namespace fseb {
-
-cudaError_t launch_fse_encode_blocks(const BlockDescs&, bool, unsigned, unsigned, cudaStream_t);
-cudaError_t launch_fse_decode_blocks(const BlockDescs&, bool, cudaStream_t);
 
 namespace fsep {
 

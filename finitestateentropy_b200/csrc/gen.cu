@@ -6,6 +6,7 @@
 // jumped ahead per thread by composing affine maps (square-and-multiply), so every thread can
 // start anywhere in the stream; the byte at stream position i is identical to the reference's.
 #include "common.cuh"
+#include "launchers.h"
 
 namespace fseb {
 

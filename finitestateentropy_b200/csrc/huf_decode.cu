@@ -37,6 +37,7 @@
 // NS = 1: one lane per block column, 64 lanes = 2 warps per CTA (still the even or the odd columns per warp), no jump table;
 // the table, ring, fast loop, head, tail, passes and the X2 verdict pass are those of the 4X form (DESIGN.md 4.1).
 #include "common.cuh"
+#include "launchers.h"
 #include "huf_dev.cuh"
 #include "launch_util.cuh"
 #include <cstdlib>
@@ -641,9 +642,6 @@ huf_decode_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, cons
 }
 
 }  // namespace hufd
-
-cudaError_t launch_huf_x2_fixup(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results, cudaStream_t stream);
-cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
 
 namespace {
 

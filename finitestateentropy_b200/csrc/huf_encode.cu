@@ -33,6 +33,7 @@
 #include <type_traits>
 #include <vector>
 #include "common.cuh"
+#include "launchers.h"
 #include "launch_util.cuh"
 #include "fse_dev.cuh"
 #include "sink_dev.cuh"

@@ -8,11 +8,10 @@
 //   3. a kernel gives an empty block (n == 0 and L == 0, what the packed compress stores for it) the result 0 -- the decoder
 //      answers dstSize 0 with dstSize_tooSmall.
 #include "common.cuh"
+#include "launchers.h"
 #include "launch_util.cuh"
 
 namespace fseb {
-
-cudaError_t launch_huf_decode_blocks(const BlockDescs&, int, cudaStream_t);
 
 namespace hufp {
 

@@ -12,6 +12,7 @@
 // the X2 decoder (huf_x2_dev.cuh), writing the bytes and the verdict the reference produces.  On well-formed batches it
 // finds nothing to do: one coalesced sweep over the results.
 #include "common.cuh"
+#include "launchers.h"
 #include "huf_x2_dev.cuh"
 #include "launch_util.cuh"
 

@@ -3,6 +3,7 @@
 // batched kernels use, on one table, so that HIST_count / FSE_normalizeCount / FSE_buildCTable /
 // FSE_buildDTable / HUF_buildCTable / HUF_readDTableX1 ... are honest drop-ins executing on the GPU.
 #include "common.cuh"
+#include "launchers.h"
 #include "fse_dev.cuh"
 #include "bitsrc_dev.cuh"
 #include "sink_dev.cuh"

@@ -392,6 +392,19 @@ def _child():
             blocks.append(coded("fse", part)); regen += bytes(part)
     frame = build_frame("fse", 1, blocks, data=regen)
     assert frame_decompress(frame)[1] == regen
+    # a verdict with chunks still in flight, past chunk 4 at each budget of test_chunk_budgets (a 1 KB block weighs 1.5-2 KB):
+    # the decoder's (block 1200 coded with tableLog 20, which FSE_readNCount rejects) and a frame capacity that runs out
+    big = probagen(1600 * 1024, 0.2)
+    blocks = [coded("fse", big[i: i + 1024], full=True) for i in range(0, len(big), 1024)]
+    t, r, c, payload = blocks[1200]
+    assert t == 0
+    blocks[1200] = (t, r, c, bytes([payload[0] | 0x0F]) + payload[1:])
+    assert compare_with_ref(build_frame("fse", 0, blocks, data=big), tmp, "tableLog 20 at block 1200") == 39
+    for codec in ("fse", "huf"):
+        r, frame, ok = frame_compress(big, codec, 0)
+        assert ok and not _is_err(r), codec
+        rr, _, ok = frame_compress(big, codec, 0, cap=r * 3 // 4)
+        assert rr == ERR["dstSize_tooSmall"] and ok, (codec, rr)
     print("child ok")
 
 
