@@ -503,21 +503,25 @@ def m2_blocks(rng, n, top, wide=False):
     FSE_optimalTableLog keeps the request."""
     out = []
     for tl in range(5, 13):
-        k = min(1 << (tl - 1), 287 if wide else 256)
-        for it in range(100):
-            k2 = k // 2 + int(rng.integers(0, k // 4 + 1))
-            k1 = k - k2
-            c = np.concatenate([np.ones(k1) * ((n - k2) // k1) + rng.integers(-3, 4, k1), np.ones(k2)]).astype(np.int64)
-            c[0] += n - int(c.sum())
-            syms = np.concatenate([np.arange(k - 1), [top]]) if k <= top + 1 else np.arange(k)
-            h = np.zeros(int(syms.max()) + 1, np.int64)
-            h[syms] = c
-            if normalize_method(h, n, int(syms.max()), tl)[1]:
-                out.append(from_counts(rng, c, syms).astype(np.uint16 if wide else np.uint8))
-                break
-        else:
-            raise AssertionError("no input found for the second method at tableLog %d" % tl)
+        c, syms = m2_counts(rng, n, tl, top, wide)
+        out.append(from_counts(rng, c, syms).astype(np.uint16 if wide else np.uint8))
     return out
+
+
+def m2_counts(rng, n, tl, top, wide=False):
+    """(counts, symbols) of one m2_blocks histogram of n symbols at tableLog tl"""
+    k = min(1 << (tl - 1), 287 if wide else 256)
+    for it in range(100):
+        k2 = k // 2 + int(rng.integers(0, k // 4 + 1))
+        k1 = k - k2
+        c = np.concatenate([np.ones(k1) * ((n - k2) // k1) + rng.integers(-3, 4, k1), np.ones(k2)]).astype(np.int64)
+        c[0] += n - int(c.sum())
+        syms = np.concatenate([np.arange(k - 1), [top]]) if k <= top + 1 else np.arange(k)
+        h = np.zeros(int(syms.max()) + 1, np.int64)
+        h[syms] = c
+        if normalize_method(h, n, int(syms.max()), tl)[1]:
+            return c, syms
+    raise AssertionError("no input found for the second method at tableLog %d" % tl)
 
 
 def raw_weight_blocks(rng, n):

@@ -28,7 +28,7 @@ pytestmark = pytest.mark.gpu
 
 CODECS = ["fse", "huf", "huf1x", "fseu16"]
 UNIT = {"fse": 1, "huf": 1, "huf1x": 1, "fseu16": 2}
-MAX_BLOCK = {"fse": 1 << 18, "huf": 1 << 17, "huf1x": 1 << 17, "fseu16": 1 << 17}   # symbols; FSE's true limit is 2^30
+MAX_BLOCK = {"fse": 1 << 18, "huf": 1 << 17, "huf1x": 1 << 17, "fseu16": 1 << 17}   # symbols; a 2^30-byte FSE block: test_gpu_fse_large.py
 UNIT_MSV = {"fse": 255, "huf": 255, "huf1x": 255, "fseu16": 0}                  # the Python calls' default maxSymbolValue
 BLOCK_OVERHEAD = 512                                                              # what a block adds to a chunk's weight
 
