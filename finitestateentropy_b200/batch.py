@@ -418,3 +418,54 @@ def frame_decompress(frame):
     r = lib().FSEB200_frame_decompress_host(_host_ptr(out), out.numel(), _host_ptr(frame), frame.numel())
     _ret(r, "FSEB200_frame_decompress_host")
     return out[:r]
+
+
+def frame_compress_batch(src, sizes, codec="fse", block_size_id=5):
+    """Many .fse frames in one synchronous call: frame f is sizes[f] bytes of `src` (a CPU uint8 tensor, pinned or pageable)
+    right after frame f - 1, each coded exactly as frame_compress codes it.  Returns (frames, offsets, results): frame f is
+    frames[offsets[f]:offsets[f + 1]] (offsets: int64, n + 1 entries) and results[f] its size or error code (int64)."""
+    from . import lib
+    cid = FRAME_CODECS[codec]
+    sizes = _host_sizes(sizes)
+    n = sizes.numel()
+    _host_check(src, torch.uint8)
+    assert bool((sizes >= 0).all()), "sizes must not be negative"
+    assert src.numel() >= int(sizes.sum()), (src.numel(), int(sizes.sum()))
+    assert 0 <= block_size_id <= 6, block_size_id
+    cap = sum(int(lib().FSEB200_frame_compressBound(int(x), block_size_id)) for x in sizes.tolist())
+    frames = torch.empty(cap, dtype=torch.uint8)
+    offsets = torch.zeros(n + 1, dtype=torch.int64)                 # nFrames == 0 writes nothing
+    results = torch.empty(n, dtype=torch.int64)
+    r = lib().FSEB200_frame_compress_host_batch(cid, block_size_id, n, _host_ptr(frames), cap, offsets.data_ptr(), _host_ptr(results),
+                                                _host_ptr(src), _host_ptr(sizes))
+    _ret(r, "FSEB200_frame_compress_host_batch")
+    return frames[:int(offsets[-1])], offsets, results
+
+
+def frame_decompress_batch(frames, offsets, capacities=None):
+    """Many .fse frames in one synchronous call: frame f is frames[offsets[f]:offsets[f + 1]] (a CPU uint8 tensor; offsets int64,
+    n + 1 entries, non-decreasing).  Frame f decodes into out[start_f : start_f + capacities[f]], start_f the sum of the earlier
+    capacities; capacities default to each frame's FSEB200_frame_decompress_bound (0 for a frame its header walk rejects).
+    Returns (out, results): results[f] (int64) is what frame_decompress's C call returns for frame f -- its size or error code;
+    a failing frame does not stop the others."""
+    from . import lib, is_error
+    _host_check(frames, torch.uint8)
+    offsets = _host_sizes(offsets)
+    n = offsets.numel() - 1
+    assert n >= 0, "offsets needs n + 1 entries"
+    o = offsets.tolist()
+    assert all(o[i] <= o[i + 1] for i in range(n)) and (n == 0 or (o[0] >= 0 and o[-1] <= frames.numel())), "offsets"
+    if capacities is None:
+        caps = []
+        for f in range(n):
+            b = lib().FSEB200_frame_decompress_bound(frames.data_ptr() + o[f] if o[f + 1] > o[f] else None, o[f + 1] - o[f])
+            caps.append(0 if is_error(b) else int(b))
+        capacities = caps
+    capacities = _host_sizes(capacities)
+    assert capacities.numel() == n and bool((capacities >= 0).all()), (capacities.numel(), n)
+    out = torch.empty(int(capacities.sum()), dtype=torch.uint8)
+    results = torch.empty(n, dtype=torch.int64)
+    r = lib().FSEB200_frame_decompress_host_batch(n, _host_ptr(out), _host_ptr(capacities), _host_ptr(results), _host_ptr(frames),
+                                                  offsets.data_ptr())
+    _ret(r, "FSEB200_frame_decompress_host_batch")
+    return out, results

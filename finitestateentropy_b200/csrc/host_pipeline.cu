@@ -7,7 +7,11 @@
 #include "launch_util.cuh"
 #include "xxh32.h"
 #include <algorithm>
+#include <atomic>
 #include <cstring>
+#include <condition_variable>
+#include <deque>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -198,9 +202,11 @@ struct HostChunk { size_t b0, b1; u64 a0, a1; };   // blocks [b0, b1); uncompres
 struct ChunkMax { size_t blocks = 0; u64 bytes = 0, packed = 0; };   // each the largest over the chunks
 
 // chunks of blocks whose weight (uncompressed bytes + the packed bytes `packed(b)` + BLOCK_OVERHEAD) stays within the budget;
-// `most` gets the largest block count, uncompressed bytes and packed bytes of a chunk
+// `most` gets the largest block count, uncompressed bytes and packed bytes of a chunk.  With `whole` (the frame calls),
+// whole[b] is the weight of the frame that starts at block b (0 inside a frame): a chunk also closes in front of a frame that
+// fits the budget whole but not the rest of the chunk, so only frames above the budget span chunks.
 template <typename F>
-std::vector<HostChunk> cut_chunks(const size_t* sizes, size_t nBlocks, u64 unit, F packed, ChunkMax& most)
+std::vector<HostChunk> cut_chunks(const size_t* sizes, size_t nBlocks, u64 unit, F packed, ChunkMax& most, const u64* whole = nullptr)
 {
     std::vector<HostChunk> out;
     size_t const budget = chunk_budget();
@@ -212,7 +218,8 @@ std::vector<HostChunk> cut_chunks(const size_t* sizes, size_t nBlocks, u64 unit,
     };
     for (size_t b = 0; b < nBlocks; b++) {
         u64 const bytes = unit * sizes[b], pb = packed(b), wb = bytes + pb + BLOCK_OVERHEAD;
-        if (c.b1 > c.b0 && w + wb > budget) { close(); c = { b, b, c.a1, c.a1 }; w = 0; p = 0; }
+        bool const frameBreak = whole && whole[b] && whole[b] <= budget && w + whole[b] > budget;
+        if (c.b1 > c.b0 && (w + wb > budget || frameBreak)) { close(); c = { b, b, c.a1, c.a1 }; w = 0; p = 0; }
         c.b1 = b + 1; c.a1 += bytes; w += wb; p += pb;
     }
     close();
@@ -347,21 +354,39 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
 }
 
 // ================================================================================================
-// frames: the .fse format of the reference's file tool (programs/fileio.c:266-626) on host buffers, through the packed
-// pair's ring and chunk budget.  Compress: each chunk runs the device packed compress, then frame.cu lays its frame body out on the device --
-// headers in front of the stored blocks -- so the body comes down in one copy to its place in the frame; a worker thread hashes
-// the whole input meanwhile.  Decompress: the host walks the block headers first (the frame is in host memory), each chunk copies
-// up exactly its own frame bytes, the compressed blocks go to the descriptor decoders and the raw and RLE blocks to frame.cu's
-// stored-block kernel.  An FSE block may decode short, so a chunk's output offset is known only once every earlier chunk's
-// results are in: a chunk is copied down, and hashed in frame order, in the lagged finish step.
+// frames: the .fse format of the reference's file tool (programs/fileio.c:266-626) on host buffers, many frames per call,
+// through the packed pair's ring and chunk budget.  A batch of frames is a batch of blocks: the chunk cutter keeps a frame that
+// fits the budget in one chunk, so only frames above the budget span chunks, and a chunk holds many small frames.
+// Compress: each chunk runs the device packed compress, xxh32_kernel hashes the chunk's small frames in the source buffer, then
+// frame.cu lays the chunk's frame bodies out over that buffer -- frame headers, block headers, payloads and, for the frames
+// hashed there, trailers -- so runs of stored frames come down in one copy each.  Frames above DEVICE_HASH_MAX, and any that
+// span chunks, are hashed by host threads meanwhile and get their trailers once the chunks are done.
+// Decompress: the host walks every frame's headers first (the frames are in host memory), each chunk copies up its frames' bytes,
+// the compressed blocks go to the descriptor decoders and the raw and RLE blocks to frame.cu's stored-block kernel, and
+// xxh32_kernel hashes the chunk's small frames in the decoded output.  An FSE block may decode short, so a frame's output
+// offset of a block is known only once every earlier result of that frame is in: a chunk is copied down in the lagged finish
+// step, and the host-hashed frames' pieces go to their hash threads once they have landed.
 // ================================================================================================
 namespace {
 constexpr u32 MAGIC_FSE = 0x183E2309u, MAGIC_HUF = 0x183E3309u;
 constexpr u64 FRAME_HEADER = 5, FRAME_TRAILER = 3;
 enum { BT_COMPRESSED = 0, BT_RAW = 1, BT_RLE = 2, BT_END = 3 };
+enum : u64 { ROLE_FIRST = 1, ROLE_LAST = 2, ROLE_HASHED = 4 };   // frame.cu's Body::role
+
+// Frames of at most this many bytes that lie in one chunk are hashed on the device, the rest on host threads.  One frame is a
+// serial chain on either side, slower on the device than on a host core, so the device wins while a chunk holds many frames to
+// hash side by side.  Set at the measured crossover (DESIGN 5b: batches of 64 KiB to 16 MiB frames, each placement alone):
+// the device is faster up to 1 MiB, the host from 4 MiB, and at 2 MiB each wins one direction.
+constexpr u64 DEVICE_HASH_MAX = 1ull << 20;
 
 u32 trailer_checksum(u32 h) { return (h >> 5) & ((1u << 22) - 1); }
 u64 be16(const u8* p) { return (u64)p[0] << 8 | p[1]; }
+void put_trailer(u8* t, u32 hash)
+{
+    u32 const crc = trailer_checksum(hash);
+    t[0] = (u8)((crc >> 16) | (BT_END << 6)); t[1] = (u8)(crc >> 8); t[2] = (u8)crc;
+}
+u64 block_header_len(u64 v, u64 n, u64 bs) { return 1 + (n == bs ? 0 : 2) + (v >= 2 ? 2 : 0); }
 
 struct FrameBlock { u64 head, payload, rSize, cSize; int type; };   // header and payload offsets in the frame
 
@@ -411,7 +436,417 @@ FrameWalk walk_frame(const u8* f, u64 size)
     w.checksum = (u32)be16(f + pos + 1) | (u32)(f[pos] & 0x3F) << 16;
     return w;
 }
+
+// Device-to-host copies of one chunk, merged while both sides stay contiguous
+struct CopyRun {
+    cudaStream_t s;
+    const u8* dev = nullptr; u8* host = nullptr; u64 n = 0;
+    cudaError_t add(const u8* d, u8* h, u64 len)
+    {
+        if (!len) return cudaSuccess;
+        if (n && dev + n == d && host + n == h) { n += len; return cudaSuccess; }
+        cudaError_t const r = flush();
+        dev = d; host = h; n = len;
+        return r;
+    }
+    cudaError_t flush()
+    {
+        cudaError_t const r = n ? cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+        n = 0;
+        return r;
+    }
+};
+
+// Arguments checked by the callers.  Returns 0 or generic; hResults and hOffsets as FSEB200_frame_compress_host_batch.  With
+// hOffsets NULL (the one-frame call, which reports no offsets and promises only that nothing past the capacity is written) a
+// frame that spans chunks is written straight to its place while it fits, and the call stops once the last frame has failed.
+size_t frame_compress_batch(int codec, unsigned blockSizeId, size_t nFrames, u8* out, size_t outCapacity, size_t* hOffsets,
+                            size_t* hResults, const u8* src, const size_t* hSrcSizes)
+{
+    u64 const bs = (u64)1024 << blockSizeId;
+    std::vector<size_t> fb(nFrames + 1, 0);                         // frame f's blocks: [fb[f], fb[f + 1])
+    std::vector<u64> fsrc(nFrames + 1, 0);                          // frame f's source offset
+    for (size_t f = 0; f < nFrames; f++) { fb[f + 1] = fb[f] + (hSrcSizes[f] + bs - 1) / bs; fsrc[f + 1] = fsrc[f] + hSrcSizes[f]; }
+    size_t const nb = fb[nFrames];
+    std::vector<size_t> sizes(nb);
+    std::vector<u32> frameOf(nb);
+    std::vector<u64> whole(nb, 0);
+    for (size_t f = 0; f < nFrames; f++) {
+        for (size_t b = fb[f]; b < fb[f + 1]; b++) { sizes[b] = (size_t)std::min(bs, hSrcSizes[f] - (b - fb[f]) * bs); frameOf[b] = (u32)f; }
+        if (fb[f + 1] > fb[f]) whole[fb[f]] = hSrcSizes[f] + (fb[f + 1] - fb[f]) * BLOCK_OVERHEAD;
+    }
+    ChunkMax most;
+    std::vector<HostChunk> const chunks = cut_chunks(sizes.data(), nb, 1, [](size_t) { return (u64)0; }, most, whole.data());
+    // a frame is hashed on the device if it is short and lies in one chunk; otherwise on a host thread
+    std::vector<char> onDevice(nFrames, 0);
+    std::vector<size_t> hostFrames;
+    for (size_t ci = 0; ci < chunks.size() && nb; ci++)
+        for (size_t b = chunks[ci].b0; b < chunks[ci].b1; b++) {
+            size_t const f = frameOf[b];
+            if (b == fb[f]) onDevice[f] = hSrcSizes[f] <= DEVICE_HASH_MAX && fb[f + 1] <= chunks[ci].b1;
+            if (b == fb[f] && !onDevice[f]) hostFrames.push_back(f);
+        }
+    std::vector<u32> hostHash(nFrames, 0);
+    std::atomic<size_t> nextHost{0};
+    std::vector<std::thread> hashers;
+    size_t const cores = std::max(1u, std::thread::hardware_concurrency());
+    for (size_t i = 0; i < std::min(hostFrames.size(), cores); i++)
+        hashers.emplace_back([&] {
+            for (size_t j; (j = nextHost++) < hostFrames.size();) hostHash[hostFrames[j]] = FSEB200_XXH32(src + fsrc[hostFrames[j]], hSrcSizes[hostFrames[j]], 0);
+        });
+    u32 const magic = codec ? MAGIC_HUF : MAGIC_FSE;
+    u8 emptyFrame[FRAME_HEADER + FRAME_TRAILER];
+    for (int i = 0; i < 4; i++) emptyFrame[i] = (u8)(magic >> (8 * i));
+    emptyFrame[4] = (u8)blockSizeId;
+    put_trailer(emptyFrame + FRAME_HEADER, FSEB200_XXH32(nullptr, 0, 0));
+
+    u64 total = 0;                                                  // offset of the next frame
+    size_t closed = 0;                                              // frames [0, closed) have their offsets and results
+    std::vector<char> stored(nFrames, 0);
+    std::vector<u64> at(nFrames, 0);                                // frame f's offset
+    // frame f at `total` with `len` bytes or a verdict: the capacity rule and the packed calls' offsets
+    auto close = [&](size_t f, u64 len, size_t verdict) {
+        at[f] = total;
+        if (verdict) { hResults[f] = verdict; }
+        else if (total + len > outCapacity) { hResults[f] = (size_t)err(E_DST_TOO_SMALL); total += len; }
+        else { hResults[f] = (size_t)len; stored[f] = 1; total += len; }
+        closed = f + 1;
+    };
+    auto close_empty_until = [&](size_t f) {                        // the frames without blocks in front of frame f
+        for (size_t g = closed; g < f; g++) {
+            u64 const at = total;
+            close(g, FRAME_HEADER + FRAME_TRAILER, 0);
+            if (stored[g]) std::memcpy(out + at, emptyFrame, sizeof(emptyFrame));
+        }
+    };
+    // The frame being built across chunks (one at a time spans chunks): bytes so far, verdict, and where its pieces go -- its
+    // place, or, in a batch, a host stage when its bound does not fit from its offset (copied in once it closes and fits)
+    struct { u64 len = 0; size_t verdict = 0; u8* to = nullptr; std::unique_ptr<u8[]> stage; } cur;
+    size_t const lastFrame = nb ? frameOf[nb - 1] : 0;             // the last frame with blocks
+    size_t stop = 0;                                                // the one-frame call: the last frame has failed
+    cudaError_t e = cudaSuccess;
+    if (nb) {
+        auto& P = packed_ring();
+        std::lock_guard<std::mutex> lock(P.mu);
+        // The bodies go to the source's buffer once it is coded and hashed: the stored blocks plus at most 5 block-header bytes
+        // and 8 frame-header and trailer bytes per block.  Descriptor words of a chunk of cb blocks with nh device-hashed frames:
+        // queue_packed_compress's 4 cb + 1, the roles (cb), the hash ranges (2 nh) and the hashes (nh); nh <= cb.
+        size_t maxW = 0;
+        if (codec == 0) for (const HostChunk& c : chunks) maxW = std::max(maxW, FSEB200_FSE_packed_workspace(c.b1 - c.b0, c.a1 - c.a0));
+        e = P.ensure(most.bytes + 13 * most.blocks, most.bytes, maxW, 8 * most.blocks + 1, 8 * most.blocks + 1);
+        // queue: the packed compress, the hashes, the frame bodies, the offsets and values down
+        auto queue = [&](size_t ci, int k) -> cudaError_t {
+            const HostChunk& c = chunks[ci];
+            size_t const cb = c.b1 - c.b0;
+            u64* const h = P.hD[k];
+            u64* const d = P.dD[k];
+            cudaError_t r = queue_packed_compress(P, k, c, codec, src, sizes.data(), 255, 11);
+            if (r != cudaSuccess) return r;
+            u64* const role = h + 4 * cb + 1;
+            u64* const range = role + cb;
+            u32 nh = 0;
+            for (size_t b = c.b0; b < c.b1; b++) {
+                size_t const f = frameOf[b];
+                u64 x = (b == fb[f] ? ROLE_FIRST : 0) | (b + 1 == fb[f + 1] ? ROLE_LAST : 0);
+                if (b + 1 == fb[f + 1] && onDevice[f]) {
+                    x |= ROLE_HASHED | (u64)nh << 32;
+                    range[2 * nh] = fsrc[f] - c.a0; range[2 * nh + 1] = hSrcSizes[f];
+                    nh++;
+                }
+                role[b - c.b0] = x;
+            }
+            cudaStream_t const s = P.st[k];
+            if ((r = cudaMemcpyAsync(d + 4 * cb + 1, role, (cb + 2 * nh) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+            u64* const hashes = d + 5 * cb + 1 + 2 * nh;
+            if ((r = launch_xxh32_ranges(P.dA[k], d + 5 * cb + 1, nh, hashes, s)) != cudaSuccess) return r;
+            r = launch_frame_body(P.dA[k], P.dB[k], d + 2 * cb, d + 3 * cb + 1, d + cb, d + 4 * cb + 1, hashes, (u32)cb, bs, magic, blockSizeId, s);
+            if (r != cudaSuccess) return r;
+            return cudaMemcpyAsync(h + 2 * cb, d + 2 * cb, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, s);
+        };
+        // finish: each frame's length and verdict from its blocks' values (an error value makes it an error frame of length 0),
+        // the capacity rule, and the stored frames' bytes down from the chunk's body -- a run of whole frames in one copy, the
+        // piece of a spanning frame straight to its place, or to a host stage when the frame might not fit
+        auto finish = [&](size_t ci, int k) -> cudaError_t {
+            const HostChunk& c = chunks[ci];
+            size_t const cb = c.b1 - c.b0;
+            cudaError_t r = cudaStreamSynchronize(P.st[k]);
+            if (r != cudaSuccess) return r;
+            const u64* const lo = P.hD[k] + 2 * cb;
+            const u64* const vals = lo + cb + 1;
+            CopyRun run; run.s = P.st[k];
+            u64 dpos = 0;                                           // the body offset of the next block
+            for (size_t b = c.b0; b < c.b1 && r == cudaSuccess;) {
+                size_t const f = frameOf[b], e1 = std::min(c.b1, fb[f + 1]);
+                bool const first = b == fb[f], last = e1 == fb[f + 1], spans = !(first && last);
+                if (first) {
+                    close_empty_until(f);
+                    cur.len = 0; cur.verdict = 0; cur.to = nullptr; cur.stage.reset();
+                    size_t const bound = FSEB200_frame_compressBound(hSrcSizes[f], blockSizeId);
+                    if (spans && (!hOffsets || total + bound <= outCapacity)) cur.to = out + total;
+                    else if (spans) { cur.stage.reset(new u8[bound]); cur.to = cur.stage.get(); }
+                }
+                u64 const d0 = dpos, pieceAt = cur.len;
+                for (; b < e1; b++) {
+                    u64 const v = vals[b - c.b0], L = lo[b - c.b0 + 1] - lo[b - c.b0];
+                    u64 const n = (b == fb[f] ? FRAME_HEADER : 0) + (b + 1 == fb[f + 1] ? FRAME_TRAILER : 0) + (is_err(v) ? 0 : block_header_len(v, sizes[b], bs) + L);
+                    dpos += n;
+                    if (cur.verdict) continue;
+                    if (is_err(v)) cur.verdict = (size_t)v;
+                    else cur.len += n;
+                }
+                bool const over = !hOffsets && total + cur.len > outCapacity;
+                if (f == lastFrame && (cur.verdict || over)) { stop = 1; break; }
+                if (spans && !cur.verdict) r = run.add(P.dA[k] + d0, cur.to + pieceAt, dpos - d0);
+                if (!last) continue;
+                u64 const frameAt = total;
+                close(f, cur.len, cur.verdict);
+                if (stored[f] && !spans) r = run.add(P.dA[k] + d0, out + frameAt, cur.len);
+                if (cur.stage) {                                    // its pieces land before the stage is copied or freed
+                    if (r == cudaSuccess) r = run.flush();
+                    if (r == cudaSuccess) r = cudaStreamSynchronize(P.st[k]);
+                    if (r != cudaSuccess) return r;
+                    if (stored[f]) std::memcpy(out + frameAt, cur.stage.get(), cur.len);
+                    cur.stage.reset();
+                }
+            }
+            if (r == cudaSuccess) r = run.flush();
+            return r;
+        };
+        if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish, &stop);
+    }
+    for (std::thread& t : hashers) t.join();
+    if (e != cudaSuccess) return (size_t)err(E_GENERIC);
+    if (stop) close(lastFrame, cur.len, cur.verdict ? cur.verdict : (size_t)err(E_DST_TOO_SMALL));
+    close_empty_until(nFrames);
+    if (hOffsets) {
+        for (size_t f = 0; f < nFrames; f++) hOffsets[f] = (size_t)at[f];
+        hOffsets[nFrames] = (size_t)total;
+    }
+    for (size_t f : hostFrames) if (stored[f]) put_trailer(out + at[f] + hResults[f] - FRAME_TRAILER, hostHash[f]);
+    return 0;
 }
+
+// Arguments checked by the callers; offsets non-decreasing.  Returns 0 or generic; hResults as FSEB200_frame_decompress_host_batch.
+size_t frame_decompress_batch(size_t nFrames, u8* dst, const size_t* caps, size_t* hResults, const u8* in, const size_t* hOffsets)
+{
+    std::vector<FrameWalk> walks(nFrames);
+    std::vector<u64> region(nFrames + 1, 0);                        // frame f's output region starts at dst + region[f]
+    std::vector<size_t> fb(nFrames + 1, 0);                         // frame f's scheduled blocks: [fb[f], fb[f + 1])
+    std::vector<u64> nominal(nFrames, 0);
+    std::vector<size_t> verdict(nFrames, 0);                        // a decoder error or overflow, in block order
+    for (size_t f = 0; f < nFrames; f++) {
+        FrameWalk& w = walks[f];
+        w = walk_frame(in + hOffsets[f], hOffsets[f + 1] - hOffsets[f]);
+        region[f + 1] = region[f] + caps[f];
+        bool coded = false;
+        for (const FrameBlock& k : w.blocks) { nominal[f] += k.rSize; coded |= k.type == BT_COMPRESSED; }
+        // every block's output size is known: settled here first, as the single call does, without running its blocks
+        bool const settled = !coded && (nominal[f] > caps[f] || w.verdict);
+        if (!coded && nominal[f] > caps[f]) verdict[f] = (size_t)err(E_DST_TOO_SMALL);
+        fb[f + 1] = fb[f] + (settled ? 0 : w.blocks.size());
+    }
+    size_t const nb = fb[nFrames];
+    std::vector<u32> frameOf(nb);
+    std::vector<size_t> rs(nb);
+    std::vector<u64> whole(nb, 0);
+    auto blk = [&](size_t b) -> const FrameBlock& { return walks[frameOf[b]].blocks[b - fb[frameOf[b]]]; };
+    auto frame_bytes = [&](const FrameBlock& k) { return k.payload + k.cSize - k.head; };
+    for (size_t f = 0; f < nFrames; f++)
+        for (size_t b = fb[f]; b < fb[f + 1]; b++) {
+            frameOf[b] = (u32)f;
+            const FrameBlock& k = walks[f].blocks[b - fb[f]];
+            rs[b] = (size_t)k.rSize;
+            whole[fb[f]] += k.rSize + frame_bytes(k) + BLOCK_OVERHEAD;
+        }
+    ChunkMax most;
+    std::vector<HostChunk> const chunks = cut_chunks(rs.data(), nb, 1, [&](size_t b) { return frame_bytes(blk(b)); }, most, whole.data());
+    // Each chunk copies up runs of its frames' bytes: a block joins the run unless 4 KiB or more of other bytes (frames whose
+    // blocks do not run, or a long tail after a trailer) lie between.  src[b]: block b's header in the chunk's device copy.
+    struct Run { u64 from, n, to; };
+    std::vector<std::vector<Run>> runs(chunks.size());
+    std::vector<u64> srcOff(nb);
+    u64 mostIn = 0;
+    std::vector<char> onDevice(nFrames, 0);
+    std::vector<size_t> nCoded(chunks.size(), 0), nFse(chunks.size(), 0);     // compressed blocks, and those of FSE frames
+    for (size_t ci = 0; ci < chunks.size(); ci++) {
+        std::vector<Run>& R = runs[ci];
+        u64 to = 0;
+        for (size_t b = chunks[ci].b0; b < chunks[ci].b1; b++) {
+            size_t const f = frameOf[b];
+            const FrameBlock& k = blk(b);
+            u64 const a = hOffsets[f] + k.head, z = hOffsets[f] + k.payload + k.cSize;
+            if (R.empty() || a >= R.back().from + R.back().n + 4096) { R.push_back({ a, 0, to }); }
+            Run& r = R.back();
+            to = r.to + (z - r.from);
+            r.n = z - r.from;
+            srcOff[b] = r.to + (a - r.from);
+            nCoded[ci] += k.type == BT_COMPRESSED;
+            nFse[ci] += k.type == BT_COMPRESSED && walks[f].codec == 0;
+            if (b == fb[f]) onDevice[f] = !walks[f].verdict && nominal[f] <= DEVICE_HASH_MAX && fb[f + 1] <= chunks[ci].b1;
+        }
+        mostIn = std::max(mostIn, to);
+    }
+    std::vector<u64> done(nFrames, 0);                              // bytes regenerated so far
+    std::vector<char> shortFrame(nFrames, 0);
+    std::vector<u32> devHash(nFrames, 0);
+    std::vector<Xxh32> hostHash(nFrames);
+    cudaError_t e = cudaSuccess;
+    if (nb) {
+        auto& P = packed_ring();
+        std::lock_guard<std::mutex> lock(P.mu);
+        e = P.ensure(most.bytes, mostIn, 0, 8 * most.blocks, 8 * most.blocks);
+        // Descriptor words of a chunk with nc compressed and ns stored blocks and nh device-hashed frames: destinations,
+        // capacities, sources and sizes of the compressed ones (nc each; the FSE frames' blocks first, then the Huff0 frames'),
+        // the stored-block index (3 ns), the hash ranges (2 nh), then the decoders' results (nc) and the hashes (nh).
+        std::vector<u32> nHashed(chunks.size(), 0);
+        auto queue = [&](size_t ci, int k) -> cudaError_t {
+            const HostChunk& c = chunks[ci];
+            size_t const cb = c.b1 - c.b0, nc = nCoded[ci], ns = cb - nc;
+            cudaStream_t const s = P.st[k];
+            u64* const h = P.hD[k];
+            u64* const d = P.dD[k];
+            u64* const index = h + 4 * nc;
+            u64* const range = index + 3 * ns;
+            u32 nh = 0;
+            for (size_t b = c.b0, a = 0, jf = 0, jh = nFse[ci], t = 0; b < c.b1; a += rs[b], b++) {
+                const FrameBlock& x = blk(b);
+                size_t const f = frameOf[b];
+                u64 const pay = srcOff[b] + (x.payload - x.head);
+                if (b == fb[f] && onDevice[f]) { range[2 * nh] = a; range[2 * nh + 1] = nominal[f]; nh++; }
+                if (x.type == BT_COMPRESSED) {
+                    size_t const j = walks[f].codec ? jh++ : jf++;
+                    h[j] = reinterpret_cast<u64>(P.dA[k] + a); h[nc + j] = x.rSize;
+                    h[2 * nc + j] = reinterpret_cast<u64>(P.dB[k] + pay); h[3 * nc + j] = x.cSize;
+                } else {
+                    index[3 * t] = a; index[3 * t + 1] = pay; index[3 * t + 2] = x.rSize | (u64)x.type << 32;
+                    t++;
+                }
+            }
+            nHashed[ci] = nh;
+            cudaError_t r;
+            for (const Run& x : runs[ci])
+                if ((r = cudaMemcpyAsync(P.dB[k] + x.to, in + x.from, x.n, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+            if ((r = cudaMemcpyAsync(d, h, (4 * nc + 3 * ns + 2 * nh) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+            u64* const res = d + 4 * nc + 3 * ns + 2 * nh;
+            for (int huf = 0; huf < 2; huf++) {
+                size_t const j0 = huf ? nFse[ci] : 0, n = huf ? nc - nFse[ci] : nFse[ci];
+                if (!n) continue;
+                BlockDescs g;
+                g.dst = (u8* const*)d + j0; g.dstCap = d + nc + j0; g.result = res + j0;
+                g.src = (const u8* const*)(d + 2 * nc) + j0; g.srcSize = d + 3 * nc + j0; g.nBlocks = (u32)n;
+                if ((r = huf ? launch_huf_decode_blocks(g, 4, s) : launch_fse_decode_blocks(g, false, s)) != cudaSuccess) return r;
+            }
+            if (ns && (r = launch_frame_stored(P.dA[k], P.dB[k], d + 4 * nc, ns, s)) != cudaSuccess) return r;
+            if ((r = launch_xxh32_ranges(P.dA[k], d + 4 * nc + 3 * ns, nh, res + nc, s)) != cudaSuccess) return r;
+            return nc + nh ? cudaMemcpyAsync(h + 4 * nc + 3 * ns + 2 * nh, res, (nc + nh) * sizeof(u64), cudaMemcpyDeviceToHost, s) : cudaSuccess;
+        };
+        // Frames hashed on the host from the start get worker threads, one per frame up to the core count, taking frames in
+        // frame order: each hashes its frame's pieces as they land, in order, and moves on once the frame's last block is in.
+        struct Piece { size_t f; const u8* p; u64 n; };
+        struct HashQueue { std::deque<Piece> q; bool closed = false; };
+        std::vector<size_t> hostFrames, slot(nFrames, SIZE_MAX);
+        for (size_t f = 0; f < nFrames; f++)
+            if (fb[f + 1] > fb[f] && !walks[f].verdict && !onDevice[f]) { slot[f] = hostFrames.size(); hostFrames.push_back(f); }
+        std::vector<HashQueue> queues(hostFrames.size());
+        std::mutex hm;
+        std::condition_variable hcv;
+        std::atomic<size_t> nextHost{0};
+        std::vector<std::thread> hashers;
+        size_t const cores = std::max(1u, std::thread::hardware_concurrency());
+        for (size_t i = 0; i < std::min(hostFrames.size(), cores); i++)
+            hashers.emplace_back([&] {
+                for (size_t j; (j = nextHost++) < hostFrames.size();) {
+                    for (;;) {
+                        Piece x;
+                        {
+                            std::unique_lock<std::mutex> lk(hm);
+                            hcv.wait(lk, [&] { return !queues[j].q.empty() || queues[j].closed; });
+                            if (queues[j].q.empty()) break;
+                            x = queues[j].q.front(); queues[j].q.pop_front();
+                        }
+                        hostHash[x.f].update(x.p, x.n);
+                    }
+                }
+            });
+        // the chunk whose output has been copied down but whose pieces are not handed to the hashers yet, and the host-hashed
+        // frames that end in it
+        struct { int k = 0; std::vector<Piece> pieces; std::vector<size_t> ends; } pend;
+        auto hash_pending = [&]() -> cudaError_t {
+            if (pend.pieces.empty() && pend.ends.empty()) return cudaSuccess;
+            cudaError_t const r = cudaStreamSynchronize(P.st[pend.k]);
+            if (r == cudaSuccess) {
+                std::lock_guard<std::mutex> lk(hm);
+                for (const Piece& x : pend.pieces) if (slot[x.f] != SIZE_MAX) queues[slot[x.f]].q.push_back(x);
+                for (size_t j : pend.ends) queues[j].closed = true;
+            }
+            hcv.notify_all();
+            if (r == cudaSuccess) for (const Piece& x : pend.pieces) if (slot[x.f] == SIZE_MAX) hostHash[x.f].update(x.p, x.n);
+            pend.pieces.clear(); pend.ends.clear();
+            return r;
+        };
+        size_t const lastFrame = frameOf[nb - 1];
+        size_t stop = 0;                                            // the last frame has failed: nothing left to decide
+        // finish: per frame, the first decoder error or overflow of its capacity in block order ends it; its output comes down
+        // to its place -- runs of blocks and frames contiguous on both sides in one copy --, and the previous chunk's host-hashed
+        // pieces, landed meanwhile, are hashed
+        auto finish = [&](size_t ci, int k) -> cudaError_t {
+            const HostChunk& c = chunks[ci];
+            size_t const nc = nCoded[ci], ns = (c.b1 - c.b0) - nc;
+            cudaError_t r = cudaStreamSynchronize(P.st[k]);
+            if (r != cudaSuccess) return r;
+            const u64* const res = P.hD[k] + 4 * nc + 3 * ns + 2 * nHashed[ci];
+            const u64* const hashes = res + nc;
+            CopyRun run; run.s = P.st[k];
+            std::vector<Piece> landed;
+            std::vector<size_t> ends;
+            for (size_t b = c.b0, a = 0, jf = 0, jh = nFse[ci], t = 0; b < c.b1 && r == cudaSuccess; a += rs[b], b++) {
+                size_t const f = frameOf[b];
+                const FrameBlock& x = blk(b);
+                if (b + 1 == fb[f + 1] && slot[f] != SIZE_MAX) ends.push_back(slot[f]);
+                if (b == fb[f] && onDevice[f]) devHash[f] = (u32)hashes[t++];
+                u64 n = x.rSize;
+                if (x.type == BT_COMPRESSED) {
+                    u64 const v = res[walks[f].codec ? jh++ : jf++];
+                    if (verdict[f]) continue;
+                    if (is_err(v)) { verdict[f] = (size_t)v; continue; }
+                    shortFrame[f] |= v != n;
+                    n = v;
+                } else if (verdict[f]) continue;
+                if (done[f] + n > caps[f]) { verdict[f] = (size_t)err(E_DST_TOO_SMALL); continue; }
+                u8* const to = dst + region[f] + done[f];
+                r = run.add(P.dA[k] + a, to, n);
+                done[f] += n;
+                // host-hashed frames piece by piece; a device-hashed frame that decoded short (its hash covered the nominal
+                // layout, gaps included) whole, once its last block is in -- it lies in this chunk
+                if (walks[f].verdict) continue;
+                if (!onDevice[f]) landed.push_back({ f, to, n });
+                else if (b + 1 == fb[f + 1] && shortFrame[f]) landed.push_back({ f, dst + region[f], done[f] });
+            }
+            if (r == cudaSuccess) r = run.flush();
+            if (r == cudaSuccess) r = hash_pending();
+            pend.k = k; pend.pieces.swap(landed); pend.ends.swap(ends);
+            stop = verdict[lastFrame] != 0;
+            return r;
+        };
+        if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish, &stop);
+        if (e == cudaSuccess) e = hash_pending();                  // the last chunk's pieces, landed by the drain
+        {
+            std::lock_guard<std::mutex> lk(hm);
+            for (HashQueue& q : queues) q.closed = true;            // also after a failure or an early stop
+        }
+        hcv.notify_all();
+        for (std::thread& t : hashers) t.join();
+    }
+    if (e != cudaSuccess) return (size_t)err(E_GENERIC);
+    for (size_t f = 0; f < nFrames; f++) {
+        if (verdict[f]) { hResults[f] = verdict[f]; continue; }
+        if (walks[f].verdict) { hResults[f] = walks[f].verdict; continue; }
+        u32 const hash = onDevice[f] && !shortFrame[f] ? devHash[f] : hostHash[f].digest();
+        hResults[f] = trailer_checksum(hash) != walks[f].checksum ? (size_t)err(E_CORRUPT) : (size_t)done[f];   // exit 44
+    }
+    return 0;
+}
+}  // namespace
 
 FSEB_API unsigned FSEB200_XXH32(const void* src, size_t srcSize, unsigned seed)
 {
@@ -429,70 +864,24 @@ FSEB_API size_t FSEB200_frame_compressBound(size_t srcSize, unsigned blockSizeId
     return FRAME_HEADER + srcSize + srcSize / bs + (srcSize % bs ? 3 : 0) + FRAME_TRAILER;
 }
 
+FSEB_API size_t FSEB200_frame_compress_host_batch(int codec, unsigned blockSizeId, size_t nFrames, void* hOut, size_t outCapacity,
+                                                  size_t* hOffsets, size_t* hResults, const void* hSrc, const size_t* hSrcSizes)
+{
+    if (codec < 0 || codec > 1 || blockSizeId > 6 || nFrames > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    if (nFrames == 0) return 0;
+    if (!hOut || !hOffsets || !hResults || !hSrcSizes) return (size_t)err(E_SRC_WRONG);
+    if (!hSrc) for (size_t f = 0; f < nFrames; f++) if (hSrcSizes[f]) return (size_t)err(E_SRC_WRONG);
+    return frame_compress_batch(codec, blockSizeId, nFrames, (u8*)hOut, outCapacity, hOffsets, hResults, (const u8*)hSrc, hSrcSizes);
+}
 
 FSEB_API size_t FSEB200_frame_compress_host(int codec, unsigned blockSizeId, void* hFrame, size_t frameCapacity,
                                             const void* hSrc, size_t srcSize)
 {
     if (codec < 0 || codec > 1 || blockSizeId > 6 || (!hSrc && srcSize) || (!hFrame && frameCapacity)) return (size_t)err(E_SRC_WRONG);
     if (frameCapacity < FRAME_HEADER + FRAME_TRAILER) return (size_t)err(E_DST_TOO_SMALL);
-    u8* const out = (u8*)hFrame;
-    u32 const magic = codec ? MAGIC_HUF : MAGIC_FSE;
-    for (int i = 0; i < 4; i++) out[i] = (u8)(magic >> (8 * i));
-    out[4] = (u8)blockSizeId;
-    u32 hash = 0;
-    std::thread hasher([&hash, hSrc, srcSize] { hash = FSEB200_XXH32(hSrc, srcSize, 0); });
-    size_t const bs = (size_t)1024 << blockSizeId, nb = (srcSize + bs - 1) / bs;
-    size_t verdict = 0;
-    u64 body = 0;                                                   // frame body bytes written so far
-    if (nb) {
-        std::vector<size_t> sizes(nb, bs);
-        sizes[nb - 1] = srcSize - (nb - 1) * bs;
-        ChunkMax most;
-        std::vector<HostChunk> const chunks = cut_chunks(sizes.data(), nb, 1, [](size_t) { return (u64)0; }, most);
-        auto& P = packed_ring();
-        std::lock_guard<std::mutex> lock(P.mu);
-        // The body goes to the source's buffer once it is coded: the stored blocks plus at most 5 header bytes each.  Every block
-        // but the last is full, so the chunk with the most blocks also has the most bytes.
-        cudaError_t e = P.ensure(most.bytes + 5 * most.blocks, most.bytes, codec == 0 ? FSEB200_FSE_packed_workspace(most.blocks, most.bytes) : 0,
-                                 4 * most.blocks + 1, 4 * most.blocks + 1);
-        // queue: the packed compress, the frame body, the offsets and values down
-        auto queue = [&](size_t ci, int k) -> cudaError_t {
-            size_t const cb = chunks[ci].b1 - chunks[ci].b0;
-            u64* const d = P.dD[k];
-            cudaError_t r = queue_packed_compress(P, k, chunks[ci], codec, hSrc, sizes.data(), 255, 11);
-            if (r == cudaSuccess) r = launch_frame_body(P.dA[k], P.dB[k], d + 2 * cb, d + 3 * cb + 1, d + cb, (u32)cb, bs, P.st[k]);
-            if (r != cudaSuccess) return r;
-            return cudaMemcpyAsync(P.hD[k] + 2 * cb, d + 2 * cb, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, P.st[k]);
-        };
-        // finish: the first error value in block order stops the call (fileio.c:329); otherwise the body comes down if it fits
-        auto finish = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
-            size_t const cb = c.b1 - c.b0;
-            cudaError_t const r = cudaStreamSynchronize(P.st[k]);
-            if (r != cudaSuccess) return r;
-            const u64* const lo = P.hD[k] + 2 * cb;
-            const u64* const vals = lo + cb + 1;
-            u64 len = lo[cb];
-            for (size_t b = 0; b < cb && !verdict; b++) {
-                u64 const v = vals[b];
-                if (is_err(v)) verdict = (size_t)v;
-                len += 1 + (sizes[c.b0 + b] == bs ? 0 : 2) + (v >= 2 ? 2 : 0);
-            }
-            if (!verdict && FRAME_HEADER + body + len + FRAME_TRAILER > frameCapacity) verdict = (size_t)err(E_DST_TOO_SMALL);
-            if (verdict) return cudaSuccess;
-            u64 const at = body;
-            body += len;
-            return cudaMemcpyAsync(out + FRAME_HEADER + at, P.dA[k], len, cudaMemcpyDeviceToHost, P.st[k]);
-        };
-        if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish, &verdict);
-        if (!verdict && e != cudaSuccess) verdict = (size_t)err(E_GENERIC);
-    }
-    hasher.join();
-    if (verdict) return verdict;
-    u8* const t = out + FRAME_HEADER + body;
-    u32 const crc = trailer_checksum(hash);
-    t[0] = (u8)((crc >> 16) | (BT_END << 6)); t[1] = (u8)(crc >> 8); t[2] = (u8)crc;
-    return (size_t)(FRAME_HEADER + body + FRAME_TRAILER);
+    size_t result = 0;
+    size_t const r = frame_compress_batch(codec, blockSizeId, 1, (u8*)hFrame, frameCapacity, nullptr, &result, (const u8*)hSrc, &srcSize);
+    return r ? r : result;
 }
 
 FSEB_API size_t FSEB200_frame_decompress_bound(const void* hFrame, size_t frameSize)
@@ -505,124 +894,21 @@ FSEB_API size_t FSEB200_frame_decompress_bound(const void* hFrame, size_t frameS
     return (size_t)total;
 }
 
+FSEB_API size_t FSEB200_frame_decompress_host_batch(size_t nFrames, void* hDst, const size_t* hDstCapacities, size_t* hResults,
+                                                    const void* hIn, const size_t* hOffsets)
+{
+    if (nFrames > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    if (nFrames == 0) return 0;
+    if (!hDst || !hDstCapacities || !hResults || !hIn || !hOffsets) return (size_t)err(E_SRC_WRONG);
+    for (size_t f = 0; f < nFrames; f++) if (hOffsets[f + 1] < hOffsets[f]) return (size_t)err(E_SRC_WRONG);
+    return frame_decompress_batch(nFrames, (u8*)hDst, hDstCapacities, hResults, (const u8*)hIn, hOffsets);
+}
+
 FSEB_API size_t FSEB200_frame_decompress_host(void* hDst, size_t dstCapacity, const void* hFrame, size_t frameSize)
 {
     if ((!hFrame && frameSize) || (!hDst && dstCapacity)) return (size_t)err(E_SRC_WRONG);
-    const u8* const f = (const u8*)hFrame;
-    u8* const dst = (u8*)hDst;
-    FrameWalk const w = walk_frame(f, frameSize);
-    const std::vector<FrameBlock>& blk = w.blocks;
-    size_t const nb = blk.size();
-    u64 nominal = 0;
-    bool coded = false;
-    for (const FrameBlock& k : blk) { nominal += k.rSize; coded |= k.type == BT_COMPRESSED; }
-    if (!coded) {                                                   // every block's output size is known: settled here first
-        if (nominal > dstCapacity) return (size_t)err(E_DST_TOO_SMALL);
-        if (w.verdict) return w.verdict;
-    }
-    Xxh32 hash(0);
-    size_t verdict = 0;
-    u64 out = 0;                                                    // bytes regenerated so far
-    if (nb) {
-        std::vector<size_t> rs(nb);
-        for (size_t b = 0; b < nb; b++) rs[b] = (size_t)blk[b].rSize;
-        // a chunk's packed bytes are its frame bytes, headers included
-        ChunkMax most;
-        std::vector<HostChunk> const chunks = cut_chunks(rs.data(), nb, 1, [&](size_t b) { return blk[b].payload + blk[b].cSize - blk[b].head; }, most);
-        std::vector<size_t> nCoded(chunks.size(), 0);
-        for (size_t ci = 0; ci < chunks.size(); ci++)
-            for (size_t b = chunks[ci].b0; b < chunks[ci].b1; b++) nCoded[ci] += blk[b].type == BT_COMPRESSED;
-        auto& P = packed_ring();
-        std::lock_guard<std::mutex> lock(P.mu);
-        cudaError_t e = P.ensure(most.bytes, most.packed, 0, 5 * most.blocks, 5 * most.blocks);
-        // Descriptor words of a chunk with nc compressed and ns stored blocks: destinations, capacities, sources and sizes of
-        // the compressed ones (nc each), the stored-block index (3 ns), then the decoders' results (nc).
-        auto queue = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
-            size_t const cb = c.b1 - c.b0, nc = nCoded[ci], ns = cb - nc;
-            u64 const f0 = blk[c.b0].head, in = blk[c.b1 - 1].payload + blk[c.b1 - 1].cSize - f0;
-            cudaStream_t const s = P.st[k];
-            u64* const h = P.hD[k];
-            u64* const d = P.dD[k];
-            u64* const index = h + 4 * nc;
-            for (size_t b = c.b0, a = 0, j = 0, t = 0; b < c.b1; a += blk[b].rSize, b++) {
-                const FrameBlock& x = blk[b];
-                if (x.type == BT_COMPRESSED) {
-                    h[j] = reinterpret_cast<u64>(P.dA[k] + a); h[nc + j] = x.rSize;
-                    h[2 * nc + j] = reinterpret_cast<u64>(P.dB[k] + (x.payload - f0)); h[3 * nc + j] = x.cSize;
-                    j++;
-                } else {
-                    index[3 * t] = a; index[3 * t + 1] = x.payload - f0; index[3 * t + 2] = x.rSize | (u64)x.type << 32;
-                    t++;
-                }
-            }
-            cudaError_t r;
-            if ((r = cudaMemcpyAsync(P.dB[k], f + f0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-            if ((r = cudaMemcpyAsync(d, h, (4 * nc + 3 * ns) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-            u64* const res = d + 4 * nc + 3 * ns;
-            if (nc) {
-                BlockDescs g;
-                g.dst = (u8* const*)d; g.dstCap = d + nc; g.result = res;
-                g.src = (const u8* const*)(d + 2 * nc); g.srcSize = d + 3 * nc; g.nBlocks = (u32)nc;
-                r = w.codec ? launch_huf_decode_blocks(g, 4, s) : launch_fse_decode_blocks(g, false, s);
-                if (r != cudaSuccess) return r;
-                if ((r = cudaMemcpyAsync(h + 4 * nc + 3 * ns, res, nc * sizeof(u64), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
-            }
-            return ns ? launch_frame_stored(P.dA[k], P.dB[k], d + 4 * nc, ns, s) : cudaSuccess;
-        };
-        // the chunk whose output has been copied down but not hashed yet
-        struct { int k = 0; u64 a = 0, n = 0; } pend;
-        auto hash_pending = [&]() -> cudaError_t {
-            if (!pend.n) return cudaSuccess;
-            cudaError_t const r = cudaStreamSynchronize(P.st[pend.k]);
-            if (r == cudaSuccess) hash.update(dst + pend.a, pend.n);
-            pend.n = 0;
-            return r;
-        };
-        // finish: the first decoder error or overflow of dstCapacity in block order stops the call; otherwise the chunk's output
-        // comes down to its true offset -- in one copy, or block by block when an FSE block decoded short -- and the previous
-        // chunk's output, landed meanwhile, is hashed
-        auto finish = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
-            size_t const nc = nCoded[ci], ns = (c.b1 - c.b0) - nc;
-            cudaError_t r = cudaStreamSynchronize(P.st[k]);
-            if (r != cudaSuccess) return r;
-            const u64* const res = P.hD[k] + 4 * nc + 3 * ns;
-            u64 o = out;
-            bool shortBlock = false;
-            for (size_t b = c.b0, j = 0; b < c.b1 && !verdict; b++) {
-                u64 n = blk[b].rSize;
-                if (blk[b].type == BT_COMPRESSED) {
-                    u64 const v = res[j++];
-                    if (is_err(v)) { verdict = (size_t)v; break; }
-                    shortBlock |= v != n;
-                    n = v;
-                }
-                if (o + n > dstCapacity) verdict = (size_t)err(E_DST_TOO_SMALL);
-                o += n;
-            }
-            if (verdict) return cudaSuccess;
-            if (!shortBlock) {
-                if (o > out && (r = cudaMemcpyAsync(dst + out, P.dA[k], o - out, cudaMemcpyDeviceToHost, P.st[k])) != cudaSuccess) return r;
-            } else {
-                u64 at = out;
-                for (size_t b = c.b0, a = 0, j = 0; b < c.b1; a += blk[b].rSize, b++) {
-                    u64 const n = blk[b].type == BT_COMPRESSED ? res[j++] : blk[b].rSize;
-                    if (n && (r = cudaMemcpyAsync(dst + at, P.dA[k] + a, n, cudaMemcpyDeviceToHost, P.st[k])) != cudaSuccess) return r;
-                    at += n;
-                }
-            }
-            if ((r = hash_pending()) != cudaSuccess) return r;
-            pend.k = k; pend.a = out; pend.n = o - out;
-            out = o;
-            return cudaSuccess;
-        };
-        if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish, &verdict);
-        if (e == cudaSuccess && !verdict) e = hash_pending();      // the last chunk's output, landed by the drain
-        if (!verdict && e != cudaSuccess) verdict = (size_t)err(E_GENERIC);
-    }
-    if (verdict) return verdict;
-    if (w.verdict) return w.verdict;
-    if (trailer_checksum(hash.digest()) != w.checksum) return (size_t)err(E_CORRUPT);   // exit 44
-    return (size_t)out;
+    size_t const offsets[2] = { 0, frameSize };
+    size_t result = 0;
+    size_t const r = frame_decompress_batch(1, (u8*)hDst, &dstCapacity, &result, (const u8*)hFrame, offsets);
+    return r ? r : result;
 }

@@ -31,9 +31,10 @@ cudaError_t launch_fse_decompress_packed(u8* const* dst, const u64* dstSize, u64
                                          u32 nBlocks, bool wide, cudaStream_t stream);
 cudaError_t launch_huf_decompress_packed(u8* const* dst, const u64* dstSize, u64* result, const u8* in, const u64* offset,
                                          u32 nBlocks, int nStreams, cudaStream_t stream);
-cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, const u64* value, const u64* srcSize, u32 nBlocks,
-                              u64 blockSize, cudaStream_t stream);
+cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, const u64* value, const u64* srcSize, const u64* role,
+                              const u64* hash, u32 nBlocks, u64 blockSize, u32 magic, u32 blockSizeId, cudaStream_t stream);
 cudaError_t launch_frame_stored(u8* out, const u8* in, const u64* index, u64 nStored, cudaStream_t stream);
+cudaError_t launch_xxh32_ranges(const u8* base, const u64* desc, u32 n, u64* hash, cudaStream_t stream);
 
 // single-CTA table kernels (micro.cu) and generators (gen.cu)
 cudaError_t launch_hist(const void* src, u64 n, u32 declared, u32* out, u64* ret, cudaStream_t s);

@@ -301,7 +301,8 @@ size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size_t* hDstS
  *               option sets the benchmark's block size): ceil(srcSize / block) blocks and no empty one, each
  *               coded as FSE_compress / HUF_compress code it, i.e. at (maxSymbolValue 255, tableLog 11); a value of 0 makes a raw
  *               block, 1 an RLE block.  An empty input gives the 8-byte frame of header and trailer.  The trailer's checksum is
- *               computed on a host thread while the chunks run on the device.  frameCapacity >= FSEB200_frame_compressBound
+ *               computed on the device for a short input, on a host thread while the chunks run on the device for a longer one
+ *               (the batches' threshold below).  frameCapacity >= FSEB200_frame_compressBound
  *               always suffices; a frame that does not fit gives dstSize_tooSmall, and nothing past frameCapacity is written.
  *               srcSize_wrong for a bad codec, blockSizeId > 6, or a NULL pointer with srcSize > 0 (hSrc) or frameCapacity > 0
  *               (hFrame); the error value of a block, should one occur, stops the call as it stops the reference's tool.
@@ -323,12 +324,38 @@ size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size_t* hDstS
  *               srcSize_wrong also for a NULL hFrame with frameSize > 0 or a NULL hDst with dstCapacity > 0.
  *   decompress_bound: the sum of the headers' rSize -- an upper bound on decompress's result, equal to it unless an FSE block
  *               decodes short -- or the verdict of the header walk (the structural verdicts above).  Host-side only.
+ *   batches:    many frames in one call, each exactly what the one-frame call gives for it, through one chunk pipeline: a
+ *               chunk holds many small frames (a frame that fits the chunk budget is never split), and the checksums of frames
+ *               of up to DEVICE_HASH_MAX bytes (csrc/host_pipeline.cu) are computed on the device in one kernel per chunk --
+ *               longer frames are hashed on host threads, one per frame up to the core count.  Host pointers, pinned or pageable, at any alignment; synchronous; serialised
+ *               per device with the packed host calls.  Return value: 0 (also for nFrames == 0, which writes nothing);
+ *               srcSize_wrong for a bad codec, blockSizeId > 6, nFrames > 0xFFFFFFFF, or a NULL pointer while nFrames > 0 (hSrc
+ *               may be NULL when every size is 0); generic if a CUDA call fails.
+ *   compress_host_batch: frame f's source is hSrcSizes[f] bytes at hSrc + hSrcSizes[0] + ... + hSrcSizes[f - 1].
+ *               hResults[f] is what FSEB200_frame_compress_host(codec, blockSizeId, buf, FSEB200_frame_compressBound(n_f,
+ *               blockSizeId), src_f, n_f) returns -- the frame size or that call's error -- except that a frame is stored, at
+ *               hOut + hOffsets[f], only if it ends at or before outCapacity; otherwise its result is dstSize_tooSmall.  hOffsets
+ *               (nFrames + 1 entries) is the prefix sum of the frame sizes, an error frame counting 0, written in full even when
+ *               frames do not fit, so hOffsets[nFrames] is the capacity the batch needs.  Nothing outside the stored frames is
+ *               written; the sum of FSEB200_frame_compressBound over the frames always suffices.  (One exception: a frame above
+ *               the chunk budget that ends in an error value -- which the coders do not return here, coding every block with
+ *               room for it -- may leave its first pieces written where it would have been stored.)
+ *   decompress_host_batch: frame f is hIn[hOffsets[f], hOffsets[f + 1]); its output region starts at hDst plus the sum of the
+ *               earlier capacities and holds hDstCapacities[f] bytes.  hResults[f] is what FSEB200_frame_decompress_host(region,
+ *               capacity, frame, size) returns for it: every verdict above, frame by frame.  A failing frame does not stop the
+ *               others, and the bytes of its region are then unspecified.  Nothing outside the regions is written, and only the
+ *               frames' bytes are read.  Offsets that decrease give srcSize_wrong for the whole call.
  * FSEB200_XXH32 is the library's XXH32 (the public xxHash specification), the hash behind the trailer. */
 size_t   FSEB200_frame_compressBound(size_t srcSize, unsigned blockSizeId);
 size_t   FSEB200_frame_compress_host(int codec, unsigned blockSizeId, void* hFrame, size_t frameCapacity,
                                      const void* hSrc, size_t srcSize);
 size_t   FSEB200_frame_decompress_bound(const void* hFrame, size_t frameSize);
 size_t   FSEB200_frame_decompress_host(void* hDst, size_t dstCapacity, const void* hFrame, size_t frameSize);
+size_t   FSEB200_frame_compress_host_batch(int codec, unsigned blockSizeId, size_t nFrames,
+                                           void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hResults,
+                                           const void* hSrc, const size_t* hSrcSizes);
+size_t   FSEB200_frame_decompress_host_batch(size_t nFrames, void* hDst, const size_t* hDstCapacities, size_t* hResults,
+                                             const void* hIn, const size_t* hOffsets);
 unsigned FSEB200_XXH32(const void* src, size_t srcSize, unsigned seed);
 
 /* Measurement inputs generated directly in device memory: byte i of the output equals byte
