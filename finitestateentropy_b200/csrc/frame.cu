@@ -100,8 +100,6 @@ __global__ void __launch_bounds__(pack::COPY_THREADS) frame_stored_kernel(u8* ou
     else pack::cta_fill<false>(out + e[0], in + e[1], n);
 }
 
-constexpr u64 GRID_MAX = 1ull << 30;                                // CTAs per launch of the one-CTA-per-block kernels
-
 // XXH32 (seed 0) of ranges [desc[2 f], desc[2 f] + desc[2 f + 1]) of `base`, f < n, into hash[f].  Four lanes of a warp take one
 // range, one lane per accumulator; a warp takes GROUPS ranges and a CTA WARPS warps.  Each round the warp stages TILE bytes of
 // each of its ranges in shared memory with 16-byte cp.async copies, double-buffered so the next round's copies overlap this
@@ -199,7 +197,7 @@ cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, cons
 {
     if (nBlocks == 0) return cudaSuccess;
     size_t const n = nBlocks;
-    unsigned const tiles = (unsigned)((n + pack::PACK_TILE - 1) / pack::PACK_TILE);
+    unsigned const tiles = pack::tiles_of(n);
     cudaError_t e;
     u64* const s = (u64*)stream_scratch(8, stream, sizeof(u64) * (n + tiles + 1), &e);
     if (e != cudaSuccess) return e;
@@ -208,18 +206,14 @@ cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, cons
     g.role = role; g.hash = hash; g.magic = magic; g.blockSizeId = blockSizeId;
     g.out = out; g.bodyOff = s; g.blockSize = blockSize; g.nBlocks = nBlocks;
     u64* const tileSum = s + n;                                     // tiles + 1 words: the body's length goes to the last
-    pack::pack_sums_kernel<frame::Headers><<<tiles, pack::PACK_THREADS, 0, stream>>>(g, tileSum);
-    pack::pack_scan_tiles_kernel<<<1, pack::PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, nullptr, tileSum + tiles);
-    pack::pack_place_kernel<frame::Headers><<<tiles, pack::PACK_THREADS, 0, stream>>>(g, tileSum, nullptr);
-    for (u64 b0 = 0; b0 < n; b0 += frame::GRID_MAX)
-        frame::frame_payload_kernel<<<(unsigned)(n - b0 < frame::GRID_MAX ? n - b0 : frame::GRID_MAX), pack::COPY_THREADS, 0, stream>>>(g, b0);
+    pack::launch_pack<frame::Headers>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+    pack::launch_per_block(frame::frame_payload_kernel, n, stream, g);
     return cudaGetLastError();
 }
 
 cudaError_t launch_frame_stored(u8* out, const u8* in, const u64* index, u64 nStored, cudaStream_t stream)
 {
-    for (u64 j0 = 0; j0 < nStored; j0 += frame::GRID_MAX)
-        frame::frame_stored_kernel<<<(unsigned)(nStored - j0 < frame::GRID_MAX ? nStored - j0 : frame::GRID_MAX), pack::COPY_THREADS, 0, stream>>>(out, in, index, j0);
+    pack::launch_per_block(frame::frame_stored_kernel, nStored, stream, out, in, index);
     return cudaGetLastError();
 }
 

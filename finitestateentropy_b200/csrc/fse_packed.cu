@@ -149,34 +149,27 @@ fse_unpack_stored_kernel(FseUnpack g, u64 b0)
     if (threadIdx.x == 0) g.result[b] = n;
 }
 
-constexpr u64 GRID_MAX = 1ull << 30;                                // CTAs per launch of the one-CTA-per-block kernels
-
 template <bool WIDE>
 cudaError_t compress_packed(FsePack g, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
     size_t const n = g.nBlocks;
-    unsigned const tiles = (unsigned)((n + pack::PACK_TILE - 1) / pack::PACK_TILE);
+    unsigned const tiles = pack::tiles_of(n);
     cudaError_t e;
     u8* const s = (u8*)stream_scratch(5, stream, 3 * sizeof(u64) * n + sizeof(u64) * (tiles + 1), &e);
     if (e != cudaSuccess) return e;
     g.stageDst = (u8**)s; g.stageCap = (u64*)(s + 8 * n); g.stageSize = (u64*)(s + 16 * n);
     u64* const tileSum = (u64*)(s + 24 * n);                        // tiles + 1 words: the slots' total goes to the last
     // 1. staging slots
-    pack::pack_sums_kernel<StageSlots<WIDE>><<<tiles, pack::PACK_THREADS, 0, stream>>>(g, tileSum);
-    pack::pack_scan_tiles_kernel<<<1, pack::PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, nullptr, tileSum + tiles);
-    pack::pack_place_kernel<StageSlots<WIDE>><<<tiles, pack::PACK_THREADS, 0, stream>>>(g, tileSum, nullptr);
+    pack::launch_pack<StageSlots<WIDE>>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // 2. the descriptor encode into the slots
     BlockDescs st;
     st.dst = g.stageDst; st.dstCap = g.stageCap; st.result = g.result; st.src = g.src; st.srcSize = g.stageSize; st.nBlocks = g.nBlocks;
     if ((e = launch_fse_encode_blocks(st, WIDE, msv, tlog, stream)) != cudaSuccess) return e;
     // 3. offsets and verdicts
-    pack::pack_sums_kernel<PackedBlocks<WIDE>><<<tiles, pack::PACK_THREADS, 0, stream>>>(g, tileSum);
-    pack::pack_scan_tiles_kernel<<<1, pack::PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, nullptr, g.offset + n);
-    pack::pack_place_kernel<PackedBlocks<WIDE>><<<tiles, pack::PACK_THREADS, 0, stream>>>(g, tileSum, nullptr);
+    pack::launch_pack<PackedBlocks<WIDE>>(g, tileSum, nullptr, g.offset + n, nullptr, stream);
     // 4. the bytes
-    for (u64 b0 = 0; b0 < n; b0 += GRID_MAX)
-        fse_pack_copy_kernel<WIDE><<<(unsigned)(n - b0 < GRID_MAX ? n - b0 : GRID_MAX), pack::COPY_THREADS, 0, stream>>>(g, b0);
+    pack::launch_per_block(fse_pack_copy_kernel<WIDE>, n, stream, g);
     return cudaGetLastError();
 }
 
@@ -193,8 +186,7 @@ cudaError_t decompress_packed(FseUnpack g, cudaStream_t stream)
     BlockDescs d;
     d.dst = g.dst; d.dstCap = g.dstSize; d.result = g.result; d.src = g.decSrc; d.srcSize = g.decSize; d.nBlocks = g.nBlocks;
     if ((e = launch_fse_decode_blocks(d, WIDE, stream)) != cudaSuccess) return e;
-    for (u64 b0 = 0; b0 < n; b0 += GRID_MAX)
-        fse_unpack_stored_kernel<WIDE><<<(unsigned)(n - b0 < GRID_MAX ? n - b0 : GRID_MAX), pack::COPY_THREADS, 0, stream>>>(g, b0);
+    pack::launch_per_block(fse_unpack_stored_kernel<WIDE>, n, stream, g);
     return cudaGetLastError();
 }
 

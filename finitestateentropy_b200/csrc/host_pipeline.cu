@@ -7,10 +7,10 @@
 #include "launch_util.cuh"
 #include "xxh32.h"
 #include <algorithm>
+#include <cassert>
 #include <atomic>
 #include <cstring>
 #include <condition_variable>
-#include <deque>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -201,6 +201,25 @@ constexpr u64 BLOCK_OVERHEAD = 512;
 struct HostChunk { size_t b0, b1; u64 a0, a1; };   // blocks [b0, b1); uncompressed bytes [a0, a1) of the batch
 struct ChunkMax { size_t blocks = 0; u64 bytes = 0, packed = 0; };   // each the largest over the chunks
 
+// A chunk's per-block words, one layout per pipelined call: the same segment offsets in the pinned image and the device words,
+// and `end`, which sizes Ring::ensure.  The packed pair, for cb blocks: block pointers, sizes, offsets (cb + 1), values.
+struct PackedWords {
+    size_t ptr = 0, size, offset, value, end;
+    explicit PackedWords(size_t cb) : size(cb), offset(2 * cb), value(3 * cb + 1), end(4 * cb + 1) {}
+};
+// The frame compress, for cb blocks and nh device-hashed frames: queue_packed_compress's words, roles, hash ranges, hashes.
+struct FrameCompressWords {
+    PackedWords packed; size_t role, range, hash, end;
+    FrameCompressWords(size_t cb, size_t nh) : packed(cb), role(packed.end), range(role + cb), hash(range + 2 * nh), end(hash + nh) {}
+};
+// The frame decompress, for nc compressed and ns stored blocks and nh device-hashed frames: the compressed blocks' destinations,
+// capacities, sources and sizes (the FSE frames' first), the stored-block index, hash ranges, then the results and hashes.
+struct FrameDecompressWords {
+    size_t dst = 0, cap, src, srcSize, index, range, result, hash, end;
+    FrameDecompressWords(size_t nc, size_t ns, size_t nh) : cap(nc), src(2 * nc), srcSize(3 * nc), index(4 * nc), range(index + 3 * ns),
+        result(range + 2 * nh), hash(result + nc), end(hash + nh) {}
+};
+
 // chunks of blocks whose weight (uncompressed bytes + the packed bytes `packed(b)` + BLOCK_OVERHEAD) stays within the budget;
 // `most` gets the largest block count, uncompressed bytes and packed bytes of a chunk.  With `whole` (the frame calls),
 // whole[b] is the weight of the frame that starts at block b (0 inside a frame): a chunk also closes in front of a frame that
@@ -227,29 +246,28 @@ std::vector<HostChunk> cut_chunks(const size_t* sizes, size_t nBlocks, u64 unit,
 }
 
 // Queues chunk c of a host batch through the device packed compress in slot k: the source and the descriptors up, the packed
-// call with room for every block.  On the device the slot's descriptor words are then: source pointers (cb), sizes (cb), offsets
-// (cb + 1), values (cb).  codec as the host packed calls.
+// call with room for every block, its device words laid out as PackedWords.  codec as the host packed calls.
 cudaError_t queue_packed_compress(Ring<3>& P, int k, const HostChunk& c, int codec, const void* hSrc, const size_t* hSrcSizes,
                                   unsigned maxSymbolValue, unsigned tableLog)
 {
     bool const fse = codec == 0 || codec == 2, wide = codec == 2;
     u64 const unit = wide ? 2 : 1;
     size_t const cb = c.b1 - c.b0;
+    PackedWords const L(cb);
     u64 const bytes = c.a1 - c.a0;
     cudaStream_t const s = P.st[k];
     u64* const h = P.hD[k];
     u64* const d = P.dD[k];
-    for (size_t b = 0, a = 0; b < cb; b++) { h[b] = reinterpret_cast<u64>(P.dA[k] + a); h[cb + b] = hSrcSizes[c.b0 + b]; a += unit * hSrcSizes[c.b0 + b]; }
+    for (size_t b = 0, a = 0; b < cb; b++) { h[L.ptr + b] = reinterpret_cast<u64>(P.dA[k] + a); h[L.size + b] = hSrcSizes[c.b0 + b]; a += unit * hSrcSizes[c.b0 + b]; }
     cudaError_t r;
     if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-    if ((r = cudaMemcpyAsync(d, h, 2 * cb * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-    u64* const offs = d + 2 * cb;
-    u64* const vals = d + 3 * cb + 1;
-    if (fse) return launch_fse_compress_packed(P.dB[k], bytes, offs, vals, (const u8* const*)d, d + cb, (u32)cb, P.dW[k], P.capW, wide,
+    if ((r = cudaMemcpyAsync(d, h, L.offset * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+    const u8* const* const src = (const u8* const*)(d + L.ptr);
+    if (fse) return launch_fse_compress_packed(P.dB[k], bytes, d + L.offset, d + L.value, src, d + L.size, (u32)cb, P.dW[k], P.capW, wide,
                                                maxSymbolValue, tableLog, s);
     PackedDescs g;
-    g.out = P.dB[k]; g.outCap = bytes; g.offset = offs; g.result = vals;
-    g.src = (const u8* const*)d; g.srcSize = d + cb; g.nBlocks = (u32)cb;
+    g.out = P.dB[k]; g.outCap = bytes; g.offset = d + L.offset; g.result = d + L.value;
+    g.src = src; g.srcSize = d + L.size; g.nBlocks = (u32)cb;
     return launch_huf_encode_packed(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
 }
 }
@@ -269,24 +287,26 @@ FSEB_API size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCa
     auto& P = packed_ring();
     std::lock_guard<std::mutex> lock(P.mu);
     // a block stores at most its own bytes
-    cudaError_t e = P.ensure(most.bytes, most.bytes, maxW, 4 * most.blocks + 1, 4 * most.blocks + 1);
+    size_t const words = PackedWords(most.blocks).end;
+    cudaError_t e = P.ensure(most.bytes, most.bytes, maxW, words, words);
     u64 total = 0;                                                  // global offset of the next chunk's first block
     // queue: the source and the descriptors up, the packed call with room for every block, offsets and values down
     auto queue = [&](size_t ci, int k) -> cudaError_t {
-        size_t const cb = chunks[ci].b1 - chunks[ci].b0;
+        PackedWords const L(chunks[ci].b1 - chunks[ci].b0);
         cudaError_t const r = queue_packed_compress(P, k, chunks[ci], codec, hSrc, hSrcSizes, maxSymbolValue, tableLog);
         if (r != cudaSuccess) return r;
-        return cudaMemcpyAsync(P.hD[k] + 2 * cb, P.dD[k] + 2 * cb, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, P.st[k]);
+        return cudaMemcpyAsync(P.hD[k] + L.offset, P.dD[k] + L.offset, (L.end - L.offset) * sizeof(u64), cudaMemcpyDeviceToHost, P.st[k]);
     };
     // finish: global offsets, the capacity rule of one call over the whole batch, and the stored bytes -- a prefix of the chunk's
     // packed bytes, since the blocks that fit come first -- copied down
     auto finish = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
         size_t const cb = c.b1 - c.b0;
+        PackedWords const L(cb);
         cudaError_t r = cudaStreamSynchronize(P.st[k]);
         if (r != cudaSuccess) return r;
-        const u64* const lo = P.hD[k] + 2 * cb;
-        const u64* const vals = lo + cb + 1;
+        const u64* const lo = P.hD[k] + L.offset;
+        const u64* const vals = P.hD[k] + L.value;
         u64 end = 0;
         for (size_t b = 0; b < cb; b++) {
             u64 const off = total + lo[b], len = lo[b + 1] - lo[b];
@@ -318,35 +338,37 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
     std::vector<HostChunk> const chunks = cut_chunks(hDstSizes, nBlocks, unit, [&](size_t b) { return (u64)(hOffsets[b + 1] - hOffsets[b]); }, most);
     auto& P = packed_ring();
     std::lock_guard<std::mutex> lock(P.mu);
-    cudaError_t e = P.ensure(most.bytes, most.packed, 0, 4 * most.blocks + 1, 4 * most.blocks + 1);
+    size_t const words = PackedWords(most.blocks).end;
+    cudaError_t e = P.ensure(most.bytes, most.packed, 0, words, words);
     // queue: the chunk's packed bytes and descriptors up (offsets rebased to the chunk), the packed decompress, the blocks and
     // their results down
     auto queue = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
         size_t const cb = c.b1 - c.b0;
+        PackedWords const L(cb);
         u64 const in0 = hOffsets[c.b0], in = hOffsets[c.b1] - in0, bytes = c.a1 - c.a0;
         cudaStream_t const s = P.st[k];
         u64* const h = P.hD[k];
         u64* const d = P.dD[k];
-        for (size_t b = 0, a = 0; b < cb; b++) { h[b] = reinterpret_cast<u64>(P.dA[k] + a); h[cb + b] = hDstSizes[c.b0 + b]; a += unit * hDstSizes[c.b0 + b]; }
-        for (size_t b = 0; b <= cb; b++) h[2 * cb + b] = hOffsets[c.b0 + b] - in0;
+        for (size_t b = 0, a = 0; b < cb; b++) { h[L.ptr + b] = reinterpret_cast<u64>(P.dA[k] + a); h[L.size + b] = hDstSizes[c.b0 + b]; a += unit * hDstSizes[c.b0 + b]; }
+        for (size_t b = 0; b <= cb; b++) h[L.offset + b] = hOffsets[c.b0 + b] - in0;
         cudaError_t r;
         if (in && (r = cudaMemcpyAsync(P.dB[k], (const u8*)hIn + in0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-        if ((r = cudaMemcpyAsync(d, h, (3 * cb + 1) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-        u8* const* const dsts = (u8* const*)d;
-        u64* const vals = d + 3 * cb + 1;
-        r = fse ? launch_fse_decompress_packed(dsts, d + cb, vals, P.dB[k], d + 2 * cb, (u32)cb, wide, s)
-                : launch_huf_decompress_packed(dsts, d + cb, vals, P.dB[k], d + 2 * cb, (u32)cb, codec == 1 ? 4 : 1, s);
+        if ((r = cudaMemcpyAsync(d, h, L.value * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        u8* const* const dsts = (u8* const*)(d + L.ptr);
+        u64* const vals = d + L.value;
+        r = fse ? launch_fse_decompress_packed(dsts, d + L.size, vals, P.dB[k], d + L.offset, (u32)cb, wide, s)
+                : launch_huf_decompress_packed(dsts, d + L.size, vals, P.dB[k], d + L.offset, (u32)cb, codec == 1 ? 4 : 1, s);
         if (r != cudaSuccess) return r;
         if (bytes && (r = cudaMemcpyAsync((u8*)hDst + c.a0, P.dA[k], bytes, cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
-        return cudaMemcpyAsync(h + 3 * cb + 1, vals, cb * sizeof(u64), cudaMemcpyDeviceToHost, s);
+        return cudaMemcpyAsync(h + L.value, vals, (L.end - L.value) * sizeof(u64), cudaMemcpyDeviceToHost, s);
     };
     // finish: the results of the chunk, once its stream is done; it runs before the chunk's stream and pinned image take the
     // next chunk
     auto finish = [&](size_t ci, int k) -> cudaError_t {
-        size_t const cb = chunks[ci].b1 - chunks[ci].b0;
+        PackedWords const L(chunks[ci].b1 - chunks[ci].b0);
         cudaError_t const r = cudaStreamSynchronize(P.st[k]);
-        if (r == cudaSuccess) std::memcpy(hResults + chunks[ci].b0, P.hD[k] + 3 * cb + 1, cb * sizeof(u64));
+        if (r == cudaSuccess) std::memcpy(hResults + chunks[ci].b0, P.hD[k] + L.value, (L.end - L.value) * sizeof(u64));
         return r;
     };
     if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS, queue, finish);
@@ -354,18 +376,8 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
 }
 
 // ================================================================================================
-// frames: the .fse format of the reference's file tool (programs/fileio.c:266-626) on host buffers, many frames per call,
-// through the packed pair's ring and chunk budget.  A batch of frames is a batch of blocks: the chunk cutter keeps a frame that
-// fits the budget in one chunk, so only frames above the budget span chunks, and a chunk holds many small frames.
-// Compress: each chunk runs the device packed compress, xxh32_kernel hashes the chunk's small frames in the source buffer, then
-// frame.cu lays the chunk's frame bodies out over that buffer -- frame headers, block headers, payloads and, for the frames
-// hashed there, trailers -- so runs of stored frames come down in one copy each.  Frames above DEVICE_HASH_MAX, and any that
-// span chunks, are hashed by host threads meanwhile and get their trailers once the chunks are done.
-// Decompress: the host walks every frame's headers first (the frames are in host memory), each chunk copies up its frames' bytes,
-// the compressed blocks go to the descriptor decoders and the raw and RLE blocks to frame.cu's stored-block kernel, and
-// xxh32_kernel hashes the chunk's small frames in the decoded output.  An FSE block may decode short, so a frame's output
-// offset of a block is known only once every earlier result of that frame is in: a chunk is copied down in the lagged finish
-// step, and the host-hashed frames' pieces go to their hash threads once they have landed.
+// frames: the .fse format of the reference's file tool (programs/fileio.c:266-626) on host buffers, many frames per call (the
+// one-frame calls are batches of one), through the packed pair's ring and chunk budget; DESIGN 5b describes the pipeline.
 // ================================================================================================
 namespace {
 constexpr u32 MAGIC_FSE = 0x183E2309u, MAGIC_HUF = 0x183E3309u;
@@ -439,191 +451,273 @@ FrameWalk walk_frame(const u8* f, u64 size)
 
 // Device-to-host copies of one chunk, merged while both sides stay contiguous
 struct CopyRun {
-    cudaStream_t s;
-    const u8* dev = nullptr; u8* host = nullptr; u64 n = 0;
+    cudaStream_t s; const u8* dev = nullptr; u8* host = nullptr; u64 n = 0;
     cudaError_t add(const u8* d, u8* h, u64 len)
     {
-        if (!len) return cudaSuccess;
-        if (n && dev + n == d && host + n == h) { n += len; return cudaSuccess; }
+        if (!len || (n && dev + n == d && host + n == h)) { n += len; return cudaSuccess; }
         cudaError_t const r = flush();
         dev = d; host = h; n = len;
         return r;
     }
-    cudaError_t flush()
+    cudaError_t flush() { cudaError_t const r = n ? cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, s) : cudaSuccess; n = 0; return r; }
+};
+
+// A batch of frames as a batch of blocks, as both frame directions run it: frame f's blocks are [fb[f], fb[f + 1]), block b has
+// bytes[b] uncompressed bytes, and onDevice[f] says frame f's checksum comes from xxh32_kernel, nHashed[ci] of them in chunk ci.
+struct FramePlan {
+    std::vector<size_t> fb, bytes, hostFrames;                      // hostFrames: those hashed on host threads, in frame order
+    std::vector<u32> frameOf, nHashed;
+    std::vector<char> onDevice;
+    std::vector<HostChunk> chunks; ChunkMax most;
+};
+struct FrameShape { size_t nBlocks; u64 hashLen; bool hashable; }; struct BlockShape { u64 bytes, stored; };
+
+// frame(f): frame f's block count, the bytes its checksum covers, whether it has one; block(f, i): bytes and stored bytes.  A frame
+// weighs its blocks' weights; it is hashed on the device if it covers at most DEVICE_HASH_MAX bytes and lies in one chunk.
+template <class Frame, class Block>
+FramePlan plan_frames(size_t nFrames, Frame frame, Block block)
+{
+    FramePlan p; p.fb.assign(nFrames + 1, 0);
+    std::vector<FrameShape> shape(nFrames);
+    for (size_t f = 0; f < nFrames; f++) { shape[f] = frame(f); p.fb[f + 1] = p.fb[f] + shape[f].nBlocks; }
+    size_t const nb = p.fb[nFrames];
+    p.frameOf.resize(nb); p.bytes.resize(nb);
+    std::vector<u64> stored(nb), whole(nb, 0);                      // whole[b]: the weight of the frame that starts at block b
+    for (size_t f = 0; f < nFrames; f++)
+        for (size_t b = p.fb[f]; b < p.fb[f + 1]; b++) {
+            BlockShape const k = block(f, b - p.fb[f]);
+            p.frameOf[b] = (u32)f; p.bytes[b] = (size_t)k.bytes; stored[b] = k.stored;
+            whole[p.fb[f]] += k.bytes + k.stored + BLOCK_OVERHEAD;
+        }
+    p.chunks = cut_chunks(p.bytes.data(), nb, 1, [&](size_t b) { return stored[b]; }, p.most, whole.data());
+    p.onDevice.assign(nFrames, 0); p.nHashed.assign(p.chunks.size(), 0);
+    for (size_t ci = 0; ci < p.chunks.size(); ci++)
+        for (size_t b = p.chunks[ci].b0; b < p.chunks[ci].b1; b++) {
+            size_t const f = p.frameOf[b];
+            if (b != p.fb[f] || !shape[f].hashable) continue;
+            p.onDevice[f] = shape[f].hashLen <= DEVICE_HASH_MAX && p.fb[f + 1] <= p.chunks[ci].b1;
+            if (p.onDevice[f]) p.nHashed[ci]++;
+            else p.hostFrames.push_back(f);
+        }
+    return p;
+}
+
+// XXH32 of `frames` on min(frames, cores) host threads, each taking frames in frame order and hashing a frame's pieces as fed,
+// up to the one marked last.  join(), also the destructor's after a failure or an early stop, closes every frame and waits for
+// the threads; digest(f) is read after it (a frame not among `frames`: the empty input's).
+class HostHasher {
+    struct Queue { std::vector<std::pair<const u8*, u64>> pieces; bool closed = false; std::condition_variable cv; };
+    static constexpr size_t NONE = SIZE_MAX;
+    std::vector<size_t> frames_, slot_;                             // slot_[f]: frame f's index in frames_, or NONE
+    std::vector<Xxh32> state_;                                      // by slot
+    std::vector<Queue> q_;
+    std::mutex mu_;
+    std::atomic<size_t> next_{0};
+    std::vector<std::thread> threads_;
+public:
+    struct Piece { size_t f; const u8* p; u64 n; bool last; };
+    HostHasher(size_t nFrames, const std::vector<size_t>& frames) : frames_(frames), slot_(nFrames, NONE), state_(frames.size()), q_(frames.size())
     {
-        cudaError_t const r = n ? cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, s) : cudaSuccess;
-        n = 0;
-        return r;
+        for (size_t j = 0; j < frames.size(); j++) slot_[frames[j]] = j;
+        for (size_t i = 0; i < std::min(frames.size(), (size_t)std::max(1u, std::thread::hardware_concurrency())); i++)
+            threads_.emplace_back([this] {
+                for (size_t j; (j = next_++) < q_.size();)
+                    for (std::vector<std::pair<const u8*, u64>> got;; got.clear()) {
+                        {
+                            std::unique_lock<std::mutex> lk(mu_);
+                            q_[j].cv.wait(lk, [&] { return !q_[j].pieces.empty() || q_[j].closed; });
+                            if (q_[j].pieces.empty()) break;
+                            got.swap(q_[j].pieces);
+                        }
+                        for (const auto& x : got) state_[j].update(x.first, x.second);
+                    }
+            });
+    }
+    ~HostHasher() { join(); }
+    void feed(const Piece& x)
+    {
+        assert(slot_[x.f] != NONE);                                 // only `frames` are fed
+        Queue& q = q_[slot_[x.f]];
+        { std::lock_guard<std::mutex> lk(mu_); if (x.n) q.pieces.push_back({ x.p, x.n }); q.closed |= x.last; }
+        q.cv.notify_one();
+    }
+    void join() { for (size_t f : frames_) feed({ f, nullptr, 0, true }); for (std::thread& t : threads_) t.join(); threads_.clear(); }
+    u32 digest(size_t f) const { return slot_[f] == NONE ? Xxh32().digest() : state_[slot_[f]].digest(); }
+};
+
+// A compress call's frames as they close in frame order: offsets, results under the capacity rule, empty-source frames written
+struct FrameOutput {
+    u8* out; size_t capacity; size_t* results;
+    u8 empty[FRAME_HEADER + FRAME_TRAILER];                         // the frame of an empty source
+    u64 total = 0;                                                  // offset of the next frame
+    size_t closed = 0;                                              // frames [0, closed) have their offsets and results
+    std::vector<char> stored;
+    std::vector<u64> at;                                            // frame f's offset; at[nFrames]: the total
+    FrameOutput(u8* o, size_t cap, size_t* res, size_t nFrames, u32 magic, unsigned blockSizeId)
+        : out(o), capacity(cap), results(res), empty{ (u8)magic, (u8)(magic >> 8), (u8)(magic >> 16), (u8)(magic >> 24), (u8)blockSizeId },
+          stored(nFrames, 0), at(nFrames + 1, 0) { put_trailer(empty + FRAME_HEADER, FSEB200_XXH32(nullptr, 0, 0)); }
+    // frame f at `total` with `len` bytes or a verdict
+    void close(size_t f, u64 len, size_t verdict)
+    {
+        at[f] = total; closed = f + 1;
+        if (verdict) { results[f] = verdict; return; }
+        stored[f] = total + len <= capacity;
+        results[f] = stored[f] ? (size_t)len : (size_t)err(E_DST_TOO_SMALL);
+        total += len;
+    }
+    void close_empty_until(size_t f)                                // the frames without blocks in front of frame f
+    {
+        for (size_t g = closed; g < f; g++) {
+            u64 const pos = total;
+            close(g, FRAME_HEADER + FRAME_TRAILER, 0);
+            if (stored[g]) std::memcpy(out + pos, empty, sizeof(empty));
+        }
     }
 };
 
-// Arguments checked by the callers.  Returns 0 or generic; hResults and hOffsets as FSEB200_frame_compress_host_batch.  With
-// hOffsets NULL (the one-frame call, which reports no offsets and promises only that nothing past the capacity is written) a
-// frame that spans chunks is written straight to its place while it fits, and the call stops once the last frame has failed.
-size_t frame_compress_batch(int codec, unsigned blockSizeId, size_t nFrames, u8* out, size_t outCapacity, size_t* hOffsets,
-                            size_t* hResults, const u8* src, const size_t* hSrcSizes)
+// How a frame that spans chunks is written.  ONE_FRAME (the one-frame call, which promises only that nothing past the capacity
+// is written): straight to its place while it fits, and the call stops once the frame fails.  BATCH: to its place if its
+// compressBound fits from its offset, else to a host stage copied in once it closes and fits; the other frames go on.
+enum class Spanning { ONE_FRAME, BATCH };
+
+// Arguments checked by the callers.  Returns 0 or generic; hResults, hOffsets (NULL for ONE_FRAME) as the batch call's.
+size_t frame_compress_batch(Spanning spanning, int codec, unsigned blockSizeId, size_t nFrames, u8* out, size_t outCapacity,
+                            size_t* hOffsets, size_t* hResults, const u8* src, const size_t* hSrcSizes)
 {
     u64 const bs = (u64)1024 << blockSizeId;
-    std::vector<size_t> fb(nFrames + 1, 0);                         // frame f's blocks: [fb[f], fb[f + 1])
+    FramePlan const p = plan_frames(nFrames, [&](size_t f) { return FrameShape{ (size_t)((hSrcSizes[f] + bs - 1) / bs), hSrcSizes[f], true }; },
+                                    [&](size_t f, size_t i) { return BlockShape{ std::min(bs, hSrcSizes[f] - i * bs), 0 }; });
     std::vector<u64> fsrc(nFrames + 1, 0);                          // frame f's source offset
-    for (size_t f = 0; f < nFrames; f++) { fb[f + 1] = fb[f] + (hSrcSizes[f] + bs - 1) / bs; fsrc[f + 1] = fsrc[f] + hSrcSizes[f]; }
-    size_t const nb = fb[nFrames];
-    std::vector<size_t> sizes(nb);
-    std::vector<u32> frameOf(nb);
-    std::vector<u64> whole(nb, 0);
-    for (size_t f = 0; f < nFrames; f++) {
-        for (size_t b = fb[f]; b < fb[f + 1]; b++) { sizes[b] = (size_t)std::min(bs, hSrcSizes[f] - (b - fb[f]) * bs); frameOf[b] = (u32)f; }
-        if (fb[f + 1] > fb[f]) whole[fb[f]] = hSrcSizes[f] + (fb[f + 1] - fb[f]) * BLOCK_OVERHEAD;
-    }
-    ChunkMax most;
-    std::vector<HostChunk> const chunks = cut_chunks(sizes.data(), nb, 1, [](size_t) { return (u64)0; }, most, whole.data());
-    // a frame is hashed on the device if it is short and lies in one chunk; otherwise on a host thread
-    std::vector<char> onDevice(nFrames, 0);
-    std::vector<size_t> hostFrames;
-    for (size_t ci = 0; ci < chunks.size() && nb; ci++)
-        for (size_t b = chunks[ci].b0; b < chunks[ci].b1; b++) {
-            size_t const f = frameOf[b];
-            if (b == fb[f]) onDevice[f] = hSrcSizes[f] <= DEVICE_HASH_MAX && fb[f + 1] <= chunks[ci].b1;
-            if (b == fb[f] && !onDevice[f]) hostFrames.push_back(f);
-        }
-    std::vector<u32> hostHash(nFrames, 0);
-    std::atomic<size_t> nextHost{0};
-    std::vector<std::thread> hashers;
-    size_t const cores = std::max(1u, std::thread::hardware_concurrency());
-    for (size_t i = 0; i < std::min(hostFrames.size(), cores); i++)
-        hashers.emplace_back([&] {
-            for (size_t j; (j = nextHost++) < hostFrames.size();) hostHash[hostFrames[j]] = FSEB200_XXH32(src + fsrc[hostFrames[j]], hSrcSizes[hostFrames[j]], 0);
-        });
+    for (size_t f = 0; f < nFrames; f++) fsrc[f + 1] = fsrc[f] + hSrcSizes[f];
+    HostHasher hasher(nFrames, p.hostFrames);
+    for (size_t f : p.hostFrames) hasher.feed({ f, src + fsrc[f], hSrcSizes[f], true });
     u32 const magic = codec ? MAGIC_HUF : MAGIC_FSE;
-    u8 emptyFrame[FRAME_HEADER + FRAME_TRAILER];
-    for (int i = 0; i < 4; i++) emptyFrame[i] = (u8)(magic >> (8 * i));
-    emptyFrame[4] = (u8)blockSizeId;
-    put_trailer(emptyFrame + FRAME_HEADER, FSEB200_XXH32(nullptr, 0, 0));
-
-    u64 total = 0;                                                  // offset of the next frame
-    size_t closed = 0;                                              // frames [0, closed) have their offsets and results
-    std::vector<char> stored(nFrames, 0);
-    std::vector<u64> at(nFrames, 0);                                // frame f's offset
-    // frame f at `total` with `len` bytes or a verdict: the capacity rule and the packed calls' offsets
-    auto close = [&](size_t f, u64 len, size_t verdict) {
-        at[f] = total;
-        if (verdict) { hResults[f] = verdict; }
-        else if (total + len > outCapacity) { hResults[f] = (size_t)err(E_DST_TOO_SMALL); total += len; }
-        else { hResults[f] = (size_t)len; stored[f] = 1; total += len; }
-        closed = f + 1;
-    };
-    auto close_empty_until = [&](size_t f) {                        // the frames without blocks in front of frame f
-        for (size_t g = closed; g < f; g++) {
-            u64 const at = total;
-            close(g, FRAME_HEADER + FRAME_TRAILER, 0);
-            if (stored[g]) std::memcpy(out + at, emptyFrame, sizeof(emptyFrame));
-        }
-    };
+    FrameOutput o(out, outCapacity, hResults, nFrames, magic, blockSizeId);
     // The frame being built across chunks (one at a time spans chunks): bytes so far, verdict, and where its pieces go -- its
-    // place, or, in a batch, a host stage when its bound does not fit from its offset (copied in once it closes and fits)
+    // place, or a host stage (Spanning)
     struct { u64 len = 0; size_t verdict = 0; u8* to = nullptr; std::unique_ptr<u8[]> stage; } cur;
-    size_t const lastFrame = nb ? frameOf[nb - 1] : 0;             // the last frame with blocks
-    size_t stop = 0;                                                // the one-frame call: the last frame has failed
+    size_t const nb = p.bytes.size(), lastFrame = nb ? p.frameOf[nb - 1] : 0;     // the last frame with blocks
+    size_t stop = 0;                                                // the last frame has failed: nothing left to decide
     cudaError_t e = cudaSuccess;
     if (nb) {
         auto& P = packed_ring();
         std::lock_guard<std::mutex> lock(P.mu);
         // The bodies go to the source's buffer once it is coded and hashed: the stored blocks plus at most 5 block-header bytes
-        // and 8 frame-header and trailer bytes per block.  Descriptor words of a chunk of cb blocks with nh device-hashed frames:
-        // queue_packed_compress's 4 cb + 1, the roles (cb), the hash ranges (2 nh) and the hashes (nh); nh <= cb.
-        size_t maxW = 0;
-        if (codec == 0) for (const HostChunk& c : chunks) maxW = std::max(maxW, FSEB200_FSE_packed_workspace(c.b1 - c.b0, c.a1 - c.a0));
-        e = P.ensure(most.bytes + 13 * most.blocks, most.bytes, maxW, 8 * most.blocks + 1, 8 * most.blocks + 1);
+        // and 8 frame-header and trailer bytes per block.
+        size_t maxW = 0, words = 0;
+        for (size_t ci = 0; ci < p.chunks.size(); ci++) {
+            const HostChunk& c = p.chunks[ci];
+            if (codec == 0) maxW = std::max(maxW, FSEB200_FSE_packed_workspace(c.b1 - c.b0, c.a1 - c.a0));
+            words = std::max(words, FrameCompressWords(c.b1 - c.b0, p.nHashed[ci]).end);
+        }
+        e = P.ensure(p.most.bytes + 13 * p.most.blocks, p.most.bytes, maxW, words, words);
         // queue: the packed compress, the hashes, the frame bodies, the offsets and values down
         auto queue = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
+            const HostChunk& c = p.chunks[ci];
             size_t const cb = c.b1 - c.b0;
-            u64* const h = P.hD[k];
-            u64* const d = P.dD[k];
-            cudaError_t r = queue_packed_compress(P, k, c, codec, src, sizes.data(), 255, 11);
+            FrameCompressWords const L(cb, p.nHashed[ci]);
+            u64* const h = P.hD[k], * const d = P.dD[k];
+            cudaError_t r = queue_packed_compress(P, k, c, codec, src, p.bytes.data(), 255, 11);
             if (r != cudaSuccess) return r;
-            u64* const role = h + 4 * cb + 1;
-            u64* const range = role + cb;
-            u32 nh = 0;
-            for (size_t b = c.b0; b < c.b1; b++) {
-                size_t const f = frameOf[b];
-                u64 x = (b == fb[f] ? ROLE_FIRST : 0) | (b + 1 == fb[f + 1] ? ROLE_LAST : 0);
-                if (b + 1 == fb[f + 1] && onDevice[f]) {
-                    x |= ROLE_HASHED | (u64)nh << 32;
-                    range[2 * nh] = fsrc[f] - c.a0; range[2 * nh + 1] = hSrcSizes[f];
-                    nh++;
-                }
-                role[b - c.b0] = x;
+            for (size_t b = c.b0, j = 0; b < c.b1; b++) {
+                size_t const f = p.frameOf[b];
+                bool const last = b + 1 == p.fb[f + 1], hashed = last && p.onDevice[f];
+                h[L.role + b - c.b0] = (b == p.fb[f] ? ROLE_FIRST : 0) | (last ? ROLE_LAST : 0) | (hashed ? ROLE_HASHED | (u64)j << 32 : 0);
+                if (hashed) { h[L.range + 2 * j] = fsrc[f] - c.a0; h[L.range + 2 * j + 1] = hSrcSizes[f]; j++; }
             }
             cudaStream_t const s = P.st[k];
-            if ((r = cudaMemcpyAsync(d + 4 * cb + 1, role, (cb + 2 * nh) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-            u64* const hashes = d + 5 * cb + 1 + 2 * nh;
-            if ((r = launch_xxh32_ranges(P.dA[k], d + 5 * cb + 1, nh, hashes, s)) != cudaSuccess) return r;
-            r = launch_frame_body(P.dA[k], P.dB[k], d + 2 * cb, d + 3 * cb + 1, d + cb, d + 4 * cb + 1, hashes, (u32)cb, bs, magic, blockSizeId, s);
+            if ((r = cudaMemcpyAsync(d + L.role, h + L.role, (L.hash - L.role) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+            if ((r = launch_xxh32_ranges(P.dA[k], d + L.range, p.nHashed[ci], d + L.hash, s)) != cudaSuccess) return r;
+            r = launch_frame_body(P.dA[k], P.dB[k], d + L.packed.offset, d + L.packed.value, d + L.packed.size, d + L.role, d + L.hash,
+                                  (u32)cb, bs, magic, blockSizeId, s);
             if (r != cudaSuccess) return r;
-            return cudaMemcpyAsync(h + 2 * cb, d + 2 * cb, (2 * cb + 1) * sizeof(u64), cudaMemcpyDeviceToHost, s);
+            return cudaMemcpyAsync(h + L.packed.offset, d + L.packed.offset, (L.packed.end - L.packed.offset) * sizeof(u64), cudaMemcpyDeviceToHost, s);
         };
         // finish: each frame's length and verdict from its blocks' values (an error value makes it an error frame of length 0),
         // the capacity rule, and the stored frames' bytes down from the chunk's body -- a run of whole frames in one copy, the
-        // piece of a spanning frame straight to its place, or to a host stage when the frame might not fit
+        // piece of a spanning frame to where `cur` says
         auto finish = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
-            size_t const cb = c.b1 - c.b0;
-            cudaError_t r = cudaStreamSynchronize(P.st[k]);
-            if (r != cudaSuccess) return r;
-            const u64* const lo = P.hD[k] + 2 * cb;
-            const u64* const vals = lo + cb + 1;
+            const HostChunk& c = p.chunks[ci];
+            FrameCompressWords const L(c.b1 - c.b0, p.nHashed[ci]);
+            cudaError_t r = cudaStreamSynchronize(P.st[k]); if (r != cudaSuccess) return r;
+            const u64* const lo = P.hD[k] + L.packed.offset, * const vals = P.hD[k] + L.packed.value;
             CopyRun run; run.s = P.st[k];
             u64 dpos = 0;                                           // the body offset of the next block
             for (size_t b = c.b0; b < c.b1 && r == cudaSuccess;) {
-                size_t const f = frameOf[b], e1 = std::min(c.b1, fb[f + 1]);
-                bool const first = b == fb[f], last = e1 == fb[f + 1], spans = !(first && last);
+                size_t const f = p.frameOf[b], e1 = std::min(c.b1, p.fb[f + 1]);
+                bool const first = b == p.fb[f], last = e1 == p.fb[f + 1], spans = !(first && last);
                 if (first) {
-                    close_empty_until(f);
+                    o.close_empty_until(f);
                     cur.len = 0; cur.verdict = 0; cur.to = nullptr; cur.stage.reset();
                     size_t const bound = FSEB200_frame_compressBound(hSrcSizes[f], blockSizeId);
-                    if (spans && (!hOffsets || total + bound <= outCapacity)) cur.to = out + total;
+                    if (spans && (spanning == Spanning::ONE_FRAME || o.total + bound <= outCapacity)) cur.to = out + o.total;
                     else if (spans) { cur.stage.reset(new u8[bound]); cur.to = cur.stage.get(); }
                 }
                 u64 const d0 = dpos, pieceAt = cur.len;
                 for (; b < e1; b++) {
-                    u64 const v = vals[b - c.b0], L = lo[b - c.b0 + 1] - lo[b - c.b0];
-                    u64 const n = (b == fb[f] ? FRAME_HEADER : 0) + (b + 1 == fb[f + 1] ? FRAME_TRAILER : 0) + (is_err(v) ? 0 : block_header_len(v, sizes[b], bs) + L);
+                    u64 const v = vals[b - c.b0], len = lo[b - c.b0 + 1] - lo[b - c.b0];
+                    u64 const n = (b == p.fb[f] ? FRAME_HEADER : 0) + (b + 1 == p.fb[f + 1] ? FRAME_TRAILER : 0) +
+                                  (is_err(v) ? 0 : block_header_len(v, p.bytes[b], bs) + len);
                     dpos += n;
                     if (cur.verdict) continue;
                     if (is_err(v)) cur.verdict = (size_t)v;
                     else cur.len += n;
                 }
-                bool const over = !hOffsets && total + cur.len > outCapacity;
+                bool const over = spanning == Spanning::ONE_FRAME && o.total + cur.len > outCapacity;
                 if (f == lastFrame && (cur.verdict || over)) { stop = 1; break; }
                 if (spans && !cur.verdict) r = run.add(P.dA[k] + d0, cur.to + pieceAt, dpos - d0);
                 if (!last) continue;
-                u64 const frameAt = total;
-                close(f, cur.len, cur.verdict);
-                if (stored[f] && !spans) r = run.add(P.dA[k] + d0, out + frameAt, cur.len);
+                u64 const frameAt = o.total;
+                o.close(f, cur.len, cur.verdict);
+                if (o.stored[f] && !spans) r = run.add(P.dA[k] + d0, out + frameAt, cur.len);
                 if (cur.stage) {                                    // its pieces land before the stage is copied or freed
                     if (r == cudaSuccess) r = run.flush();
                     if (r == cudaSuccess) r = cudaStreamSynchronize(P.st[k]);
                     if (r != cudaSuccess) return r;
-                    if (stored[f]) std::memcpy(out + frameAt, cur.stage.get(), cur.len);
+                    if (o.stored[f]) std::memcpy(out + frameAt, cur.stage.get(), cur.len);
                     cur.stage.reset();
                 }
             }
             if (r == cudaSuccess) r = run.flush();
             return r;
         };
-        if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish, &stop);
+        if (e == cudaSuccess) e = run_chunks(P, p.chunks.size(), P.NS - 1, queue, finish, &stop);
     }
-    for (std::thread& t : hashers) t.join();
+    hasher.join();
     if (e != cudaSuccess) return (size_t)err(E_GENERIC);
-    if (stop) close(lastFrame, cur.len, cur.verdict ? cur.verdict : (size_t)err(E_DST_TOO_SMALL));
-    close_empty_until(nFrames);
-    if (hOffsets) {
-        for (size_t f = 0; f < nFrames; f++) hOffsets[f] = (size_t)at[f];
-        hOffsets[nFrames] = (size_t)total;
-    }
-    for (size_t f : hostFrames) if (stored[f]) put_trailer(out + at[f] + hResults[f] - FRAME_TRAILER, hostHash[f]);
+    if (stop) o.close(lastFrame, cur.len, cur.verdict ? cur.verdict : (size_t)err(E_DST_TOO_SMALL));
+    o.close_empty_until(nFrames);
+    o.at[nFrames] = o.total;
+    if (hOffsets) std::copy(o.at.begin(), o.at.end(), hOffsets);
+    for (size_t f : p.hostFrames) if (o.stored[f]) put_trailer(out + o.at[f] + hResults[f] - FRAME_TRAILER, hasher.digest(f));
     return 0;
+}
+
+// What each decompress chunk copies up: runs of its frames' bytes, unless 4 KiB or more of other bytes lie between (frames that do
+// not run, long tails); srcOff[b], block b's header there; the largest chunk's bytes; its compressed blocks, nFse of FSE frames.
+struct ChunkInputs {
+    struct Run { u64 from, n, to; };
+    std::vector<std::vector<Run>> runs; std::vector<u64> srcOff; u64 most = 0; std::vector<size_t> nCoded, nFse;
+};
+ChunkInputs chunk_inputs(const FramePlan& p, const std::vector<FrameWalk>& walks, const size_t* hOffsets)
+{
+    ChunkInputs c;
+    c.runs.resize(p.chunks.size()); c.srcOff.resize(p.bytes.size()); c.nCoded.assign(p.chunks.size(), 0); c.nFse.assign(p.chunks.size(), 0);
+    for (size_t ci = 0; ci < p.chunks.size(); ci++) {
+        std::vector<ChunkInputs::Run>& R = c.runs[ci];
+        for (size_t b = p.chunks[ci].b0; b < p.chunks[ci].b1; b++) {
+            size_t const f = p.frameOf[b];
+            const FrameBlock& k = walks[f].blocks[b - p.fb[f]];
+            u64 const a = hOffsets[f] + k.head, z = hOffsets[f] + k.payload + k.cSize;
+            if (R.empty() || a >= R.back().from + R.back().n + 4096) R.push_back({ a, 0, R.empty() ? 0 : R.back().to + R.back().n });
+            R.back().n = z - R.back().from;
+            c.srcOff[b] = R.back().to + (a - R.back().from);
+            c.nCoded[ci] += k.type == BT_COMPRESSED;
+            c.nFse[ci] += k.type == BT_COMPRESSED && walks[f].codec == 0;
+        }
+        if (!R.empty()) c.most = std::max(c.most, R.back().to + R.back().n);
+    }
+    return c;
 }
 
 // Arguments checked by the callers; offsets non-decreasing.  Returns 0 or generic; hResults as FSEB200_frame_decompress_host_batch.
@@ -631,217 +725,116 @@ size_t frame_decompress_batch(size_t nFrames, u8* dst, const size_t* caps, size_
 {
     std::vector<FrameWalk> walks(nFrames);
     std::vector<u64> region(nFrames + 1, 0);                        // frame f's output region starts at dst + region[f]
-    std::vector<size_t> fb(nFrames + 1, 0);                         // frame f's scheduled blocks: [fb[f], fb[f + 1])
     std::vector<u64> nominal(nFrames, 0);
     std::vector<size_t> verdict(nFrames, 0);                        // a decoder error or overflow, in block order
     for (size_t f = 0; f < nFrames; f++) {
-        FrameWalk& w = walks[f];
-        w = walk_frame(in + hOffsets[f], hOffsets[f + 1] - hOffsets[f]);
+        FrameWalk& w = walks[f] = walk_frame(in + hOffsets[f], hOffsets[f + 1] - hOffsets[f]);
         region[f + 1] = region[f] + caps[f];
         bool coded = false;
         for (const FrameBlock& k : w.blocks) { nominal[f] += k.rSize; coded |= k.type == BT_COMPRESSED; }
-        // every block's output size is known: settled here first, as the single call does, without running its blocks
-        bool const settled = !coded && (nominal[f] > caps[f] || w.verdict);
+        // every block's output size is known: settled here first, as the single call does, and none of its blocks runs
         if (!coded && nominal[f] > caps[f]) verdict[f] = (size_t)err(E_DST_TOO_SMALL);
-        fb[f + 1] = fb[f] + (settled ? 0 : w.blocks.size());
+        if (!coded && (nominal[f] > caps[f] || w.verdict)) w.blocks.clear();
     }
-    size_t const nb = fb[nFrames];
-    std::vector<u32> frameOf(nb);
-    std::vector<size_t> rs(nb);
-    std::vector<u64> whole(nb, 0);
-    auto blk = [&](size_t b) -> const FrameBlock& { return walks[frameOf[b]].blocks[b - fb[frameOf[b]]]; };
-    auto frame_bytes = [&](const FrameBlock& k) { return k.payload + k.cSize - k.head; };
-    for (size_t f = 0; f < nFrames; f++)
-        for (size_t b = fb[f]; b < fb[f + 1]; b++) {
-            frameOf[b] = (u32)f;
-            const FrameBlock& k = walks[f].blocks[b - fb[f]];
-            rs[b] = (size_t)k.rSize;
-            whole[fb[f]] += k.rSize + frame_bytes(k) + BLOCK_OVERHEAD;
-        }
-    ChunkMax most;
-    std::vector<HostChunk> const chunks = cut_chunks(rs.data(), nb, 1, [&](size_t b) { return frame_bytes(blk(b)); }, most, whole.data());
-    // Each chunk copies up runs of its frames' bytes: a block joins the run unless 4 KiB or more of other bytes (frames whose
-    // blocks do not run, or a long tail after a trailer) lie between.  src[b]: block b's header in the chunk's device copy.
-    struct Run { u64 from, n, to; };
-    std::vector<std::vector<Run>> runs(chunks.size());
-    std::vector<u64> srcOff(nb);
-    u64 mostIn = 0;
-    std::vector<char> onDevice(nFrames, 0);
-    std::vector<size_t> nCoded(chunks.size(), 0), nFse(chunks.size(), 0);     // compressed blocks, and those of FSE frames
-    for (size_t ci = 0; ci < chunks.size(); ci++) {
-        std::vector<Run>& R = runs[ci];
-        u64 to = 0;
-        for (size_t b = chunks[ci].b0; b < chunks[ci].b1; b++) {
-            size_t const f = frameOf[b];
-            const FrameBlock& k = blk(b);
-            u64 const a = hOffsets[f] + k.head, z = hOffsets[f] + k.payload + k.cSize;
-            if (R.empty() || a >= R.back().from + R.back().n + 4096) { R.push_back({ a, 0, to }); }
-            Run& r = R.back();
-            to = r.to + (z - r.from);
-            r.n = z - r.from;
-            srcOff[b] = r.to + (a - r.from);
-            nCoded[ci] += k.type == BT_COMPRESSED;
-            nFse[ci] += k.type == BT_COMPRESSED && walks[f].codec == 0;
-            if (b == fb[f]) onDevice[f] = !walks[f].verdict && nominal[f] <= DEVICE_HASH_MAX && fb[f + 1] <= chunks[ci].b1;
-        }
-        mostIn = std::max(mostIn, to);
-    }
+    FramePlan const p = plan_frames(nFrames, [&](size_t f) { return FrameShape{ walks[f].blocks.size(), nominal[f], !walks[f].verdict }; },
+                                    [&](size_t f, size_t i) { const FrameBlock& k = walks[f].blocks[i]; return BlockShape{ k.rSize, k.payload + k.cSize - k.head }; });
+    size_t const nb = p.bytes.size();
+    auto blk = [&](size_t b) -> const FrameBlock& { return walks[p.frameOf[b]].blocks[b - p.fb[p.frameOf[b]]]; };
+    ChunkInputs const up = chunk_inputs(p, walks, hOffsets);
+    auto layout = [&](size_t ci) { return FrameDecompressWords(up.nCoded[ci], p.chunks[ci].b1 - p.chunks[ci].b0 - up.nCoded[ci], p.nHashed[ci]); };
     std::vector<u64> done(nFrames, 0);                              // bytes regenerated so far
-    std::vector<char> shortFrame(nFrames, 0);
     std::vector<u32> devHash(nFrames, 0);
-    std::vector<Xxh32> hostHash(nFrames);
+    HostHasher hasher(nFrames, p.hostFrames);
+    std::vector<std::vector<HostHasher::Piece>> landed(p.chunks.size());    // each chunk's pieces of the host-hashed frames
+    size_t fed = 0;                                                 // chunks [0, fed) went to the hasher
     cudaError_t e = cudaSuccess;
     if (nb) {
         auto& P = packed_ring();
         std::lock_guard<std::mutex> lock(P.mu);
-        e = P.ensure(most.bytes, mostIn, 0, 8 * most.blocks, 8 * most.blocks);
-        // Descriptor words of a chunk with nc compressed and ns stored blocks and nh device-hashed frames: destinations,
-        // capacities, sources and sizes of the compressed ones (nc each; the FSE frames' blocks first, then the Huff0 frames'),
-        // the stored-block index (3 ns), the hash ranges (2 nh), then the decoders' results (nc) and the hashes (nh).
-        std::vector<u32> nHashed(chunks.size(), 0);
+        size_t words = 0;
+        for (size_t ci = 0; ci < p.chunks.size(); ci++) words = std::max(words, layout(ci).end);
+        e = P.ensure(p.most.bytes, up.most, 0, words, words);
+        // queue: the frames' bytes and the descriptors up, the decoders, the stored blocks and the hashes, the results down
         auto queue = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
-            size_t const cb = c.b1 - c.b0, nc = nCoded[ci], ns = cb - nc;
+            const HostChunk& c = p.chunks[ci];
+            FrameDecompressWords const L = layout(ci);
+            size_t const nc = up.nCoded[ci];
             cudaStream_t const s = P.st[k];
-            u64* const h = P.hD[k];
-            u64* const d = P.dD[k];
-            u64* const index = h + 4 * nc;
-            u64* const range = index + 3 * ns;
-            u32 nh = 0;
-            for (size_t b = c.b0, a = 0, jf = 0, jh = nFse[ci], t = 0; b < c.b1; a += rs[b], b++) {
+            u64* const h = P.hD[k], * const d = P.dD[k];
+            for (size_t b = c.b0, a = 0, jf = 0, jh = up.nFse[ci], t = 0, j = 0; b < c.b1; a += p.bytes[b], b++) {
                 const FrameBlock& x = blk(b);
-                size_t const f = frameOf[b];
-                u64 const pay = srcOff[b] + (x.payload - x.head);
-                if (b == fb[f] && onDevice[f]) { range[2 * nh] = a; range[2 * nh + 1] = nominal[f]; nh++; }
+                size_t const f = p.frameOf[b];
+                u64 const pay = up.srcOff[b] + (x.payload - x.head);
+                if (b == p.fb[f] && p.onDevice[f]) { h[L.range + 2 * j] = a; h[L.range + 2 * j + 1] = nominal[f]; j++; }
                 if (x.type == BT_COMPRESSED) {
-                    size_t const j = walks[f].codec ? jh++ : jf++;
-                    h[j] = reinterpret_cast<u64>(P.dA[k] + a); h[nc + j] = x.rSize;
-                    h[2 * nc + j] = reinterpret_cast<u64>(P.dB[k] + pay); h[3 * nc + j] = x.cSize;
+                    size_t const i = walks[f].codec ? jh++ : jf++;
+                    h[L.dst + i] = reinterpret_cast<u64>(P.dA[k] + a); h[L.cap + i] = x.rSize;
+                    h[L.src + i] = reinterpret_cast<u64>(P.dB[k] + pay); h[L.srcSize + i] = x.cSize;
                 } else {
-                    index[3 * t] = a; index[3 * t + 1] = pay; index[3 * t + 2] = x.rSize | (u64)x.type << 32;
-                    t++;
+                    u64* const index = h + L.index + 3 * t++;
+                    index[0] = a; index[1] = pay; index[2] = x.rSize | (u64)x.type << 32;
                 }
             }
-            nHashed[ci] = nh;
             cudaError_t r;
-            for (const Run& x : runs[ci])
+            for (const ChunkInputs::Run& x : up.runs[ci])
                 if ((r = cudaMemcpyAsync(P.dB[k] + x.to, in + x.from, x.n, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-            if ((r = cudaMemcpyAsync(d, h, (4 * nc + 3 * ns + 2 * nh) * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-            u64* const res = d + 4 * nc + 3 * ns + 2 * nh;
+            if ((r = cudaMemcpyAsync(d, h, L.result * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
             for (int huf = 0; huf < 2; huf++) {
-                size_t const j0 = huf ? nFse[ci] : 0, n = huf ? nc - nFse[ci] : nFse[ci];
+                size_t const j0 = huf ? up.nFse[ci] : 0, n = huf ? nc - up.nFse[ci] : up.nFse[ci];
                 if (!n) continue;
                 BlockDescs g;
-                g.dst = (u8* const*)d + j0; g.dstCap = d + nc + j0; g.result = res + j0;
-                g.src = (const u8* const*)(d + 2 * nc) + j0; g.srcSize = d + 3 * nc + j0; g.nBlocks = (u32)n;
+                g.dst = (u8* const*)(d + L.dst) + j0; g.dstCap = d + L.cap + j0; g.result = d + L.result + j0;
+                g.src = (const u8* const*)(d + L.src) + j0; g.srcSize = d + L.srcSize + j0; g.nBlocks = (u32)n;
                 if ((r = huf ? launch_huf_decode_blocks(g, 4, s) : launch_fse_decode_blocks(g, false, s)) != cudaSuccess) return r;
             }
-            if (ns && (r = launch_frame_stored(P.dA[k], P.dB[k], d + 4 * nc, ns, s)) != cudaSuccess) return r;
-            if ((r = launch_xxh32_ranges(P.dA[k], d + 4 * nc + 3 * ns, nh, res + nc, s)) != cudaSuccess) return r;
-            return nc + nh ? cudaMemcpyAsync(h + 4 * nc + 3 * ns + 2 * nh, res, (nc + nh) * sizeof(u64), cudaMemcpyDeviceToHost, s) : cudaSuccess;
+            size_t const ns = c.b1 - c.b0 - nc;
+            if (ns && (r = launch_frame_stored(P.dA[k], P.dB[k], d + L.index, ns, s)) != cudaSuccess) return r;
+            if ((r = launch_xxh32_ranges(P.dA[k], d + L.range, p.nHashed[ci], d + L.hash, s)) != cudaSuccess) return r;
+            return L.end > L.result ? cudaMemcpyAsync(h + L.result, d + L.result, (L.end - L.result) * sizeof(u64), cudaMemcpyDeviceToHost, s) : cudaSuccess;
         };
-        // Frames hashed on the host from the start get worker threads, one per frame up to the core count, taking frames in
-        // frame order: each hashes its frame's pieces as they land, in order, and moves on once the frame's last block is in.
-        struct Piece { size_t f; const u8* p; u64 n; };
-        struct HashQueue { std::deque<Piece> q; bool closed = false; };
-        std::vector<size_t> hostFrames, slot(nFrames, SIZE_MAX);
-        for (size_t f = 0; f < nFrames; f++)
-            if (fb[f + 1] > fb[f] && !walks[f].verdict && !onDevice[f]) { slot[f] = hostFrames.size(); hostFrames.push_back(f); }
-        std::vector<HashQueue> queues(hostFrames.size());
-        std::mutex hm;
-        std::condition_variable hcv;
-        std::atomic<size_t> nextHost{0};
-        std::vector<std::thread> hashers;
-        size_t const cores = std::max(1u, std::thread::hardware_concurrency());
-        for (size_t i = 0; i < std::min(hostFrames.size(), cores); i++)
-            hashers.emplace_back([&] {
-                for (size_t j; (j = nextHost++) < hostFrames.size();) {
-                    for (;;) {
-                        Piece x;
-                        {
-                            std::unique_lock<std::mutex> lk(hm);
-                            hcv.wait(lk, [&] { return !queues[j].q.empty() || queues[j].closed; });
-                            if (queues[j].q.empty()) break;
-                            x = queues[j].q.front(); queues[j].q.pop_front();
-                        }
-                        hostHash[x.f].update(x.p, x.n);
-                    }
-                }
-            });
-        // the chunk whose output has been copied down but whose pieces are not handed to the hashers yet, and the host-hashed
-        // frames that end in it
-        struct { int k = 0; std::vector<Piece> pieces; std::vector<size_t> ends; } pend;
-        auto hash_pending = [&]() -> cudaError_t {
-            if (pend.pieces.empty() && pend.ends.empty()) return cudaSuccess;
-            cudaError_t const r = cudaStreamSynchronize(P.st[pend.k]);
-            if (r == cudaSuccess) {
-                std::lock_guard<std::mutex> lk(hm);
-                for (const Piece& x : pend.pieces) if (slot[x.f] != SIZE_MAX) queues[slot[x.f]].q.push_back(x);
-                for (size_t j : pend.ends) queues[j].closed = true;
+        auto feed_until = [&](size_t end) -> cudaError_t {          // in chunk order, once each chunk's copies have landed
+            for (cudaError_t r; fed < end; fed++) {
+                if (!landed[fed].empty() && (r = cudaStreamSynchronize(P.st[fed % P.NS])) != cudaSuccess) return r;
+                for (const HostHasher::Piece& x : landed[fed]) hasher.feed(x);
             }
-            hcv.notify_all();
-            if (r == cudaSuccess) for (const Piece& x : pend.pieces) if (slot[x.f] == SIZE_MAX) hostHash[x.f].update(x.p, x.n);
-            pend.pieces.clear(); pend.ends.clear();
-            return r;
+            return cudaSuccess;
         };
-        size_t const lastFrame = frameOf[nb - 1];
+        size_t const lastFrame = p.frameOf[nb - 1];
         size_t stop = 0;                                            // the last frame has failed: nothing left to decide
         // finish: per frame, the first decoder error or overflow of its capacity in block order ends it; its output comes down
-        // to its place -- runs of blocks and frames contiguous on both sides in one copy --, and the previous chunk's host-hashed
-        // pieces, landed meanwhile, are hashed
+        // to its place -- runs of blocks and frames contiguous on both sides in one copy -- and then goes to the hasher
         auto finish = [&](size_t ci, int k) -> cudaError_t {
-            const HostChunk& c = chunks[ci];
-            size_t const nc = nCoded[ci], ns = (c.b1 - c.b0) - nc;
-            cudaError_t r = cudaStreamSynchronize(P.st[k]);
-            if (r != cudaSuccess) return r;
-            const u64* const res = P.hD[k] + 4 * nc + 3 * ns + 2 * nHashed[ci];
-            const u64* const hashes = res + nc;
+            const HostChunk& c = p.chunks[ci];
+            FrameDecompressWords const L = layout(ci);
+            cudaError_t r = cudaStreamSynchronize(P.st[k]); if (r != cudaSuccess) return r;
+            const u64* const res = P.hD[k] + L.result, * const hashes = P.hD[k] + L.hash;
             CopyRun run; run.s = P.st[k];
-            std::vector<Piece> landed;
-            std::vector<size_t> ends;
-            for (size_t b = c.b0, a = 0, jf = 0, jh = nFse[ci], t = 0; b < c.b1 && r == cudaSuccess; a += rs[b], b++) {
-                size_t const f = frameOf[b];
+            for (size_t b = c.b0, a = 0, jf = 0, jh = up.nFse[ci], t = 0; b < c.b1 && r == cudaSuccess; a += p.bytes[b], b++) {
+                size_t const f = p.frameOf[b];
                 const FrameBlock& x = blk(b);
-                if (b + 1 == fb[f + 1] && slot[f] != SIZE_MAX) ends.push_back(slot[f]);
-                if (b == fb[f] && onDevice[f]) devHash[f] = (u32)hashes[t++];
-                u64 n = x.rSize;
-                if (x.type == BT_COMPRESSED) {
-                    u64 const v = res[walks[f].codec ? jh++ : jf++];
-                    if (verdict[f]) continue;
-                    if (is_err(v)) { verdict[f] = (size_t)v; continue; }
-                    shortFrame[f] |= v != n;
-                    n = v;
-                } else if (verdict[f]) continue;
-                if (done[f] + n > caps[f]) { verdict[f] = (size_t)err(E_DST_TOO_SMALL); continue; }
+                bool const last = b + 1 == p.fb[f + 1], onHost = !walks[f].verdict && !p.onDevice[f];
+                if (b == p.fb[f] && p.onDevice[f]) devHash[f] = (u32)hashes[t++];
+                u64 const n = x.type == BT_COMPRESSED ? res[walks[f].codec ? jh++ : jf++] : x.rSize;   // the block's result
+                if (!verdict[f] && is_err(n)) verdict[f] = (size_t)n;
+                if (!verdict[f] && done[f] + n > caps[f]) verdict[f] = (size_t)err(E_DST_TOO_SMALL);
                 u8* const to = dst + region[f] + done[f];
-                r = run.add(P.dA[k] + a, to, n);
-                done[f] += n;
-                // host-hashed frames piece by piece; a device-hashed frame that decoded short (its hash covered the nominal
-                // layout, gaps included) whole, once its last block is in -- it lies in this chunk
-                if (walks[f].verdict) continue;
-                if (!onDevice[f]) landed.push_back({ f, to, n });
-                else if (b + 1 == fb[f + 1] && shortFrame[f]) landed.push_back({ f, dst + region[f], done[f] });
+                if (!verdict[f]) { r = run.add(P.dA[k] + a, to, n); done[f] += n; }
+                if (onHost && (last || !verdict[f])) landed[ci].push_back({ f, to, verdict[f] ? 0 : n, last });
             }
             if (r == cudaSuccess) r = run.flush();
-            if (r == cudaSuccess) r = hash_pending();
-            pend.k = k; pend.pieces.swap(landed); pend.ends.swap(ends);
+            if (r == cudaSuccess) r = feed_until(ci);               // the earlier chunks', landed meanwhile
             stop = verdict[lastFrame] != 0;
             return r;
         };
-        if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish, &stop);
-        if (e == cudaSuccess) e = hash_pending();                  // the last chunk's pieces, landed by the drain
-        {
-            std::lock_guard<std::mutex> lk(hm);
-            for (HashQueue& q : queues) q.closed = true;            // also after a failure or an early stop
-        }
-        hcv.notify_all();
-        for (std::thread& t : hashers) t.join();
+        if (e == cudaSuccess) e = run_chunks(P, p.chunks.size(), P.NS - 1, queue, finish, &stop);
+        if (e == cudaSuccess) e = feed_until(p.chunks.size());     // the rest, landed by the drain
     }
+    hasher.join();
     if (e != cudaSuccess) return (size_t)err(E_GENERIC);
     for (size_t f = 0; f < nFrames; f++) {
-        if (verdict[f]) { hResults[f] = verdict[f]; continue; }
-        if (walks[f].verdict) { hResults[f] = walks[f].verdict; continue; }
-        u32 const hash = onDevice[f] && !shortFrame[f] ? devHash[f] : hostHash[f].digest();
+        if (verdict[f] || walks[f].verdict) { hResults[f] = verdict[f] ? verdict[f] : walks[f].verdict; continue; }
+        // a device-hashed frame that decoded short is hashed here: its device hash covered the nominal layout, gaps included
+        u32 const hash = !p.onDevice[f] ? hasher.digest(f) : done[f] != nominal[f] ? FSEB200_XXH32(dst + region[f], done[f], 0) : devHash[f];
         hResults[f] = trailer_checksum(hash) != walks[f].checksum ? (size_t)err(E_CORRUPT) : (size_t)done[f];   // exit 44
     }
     return 0;
@@ -871,7 +864,8 @@ FSEB_API size_t FSEB200_frame_compress_host_batch(int codec, unsigned blockSizeI
     if (nFrames == 0) return 0;
     if (!hOut || !hOffsets || !hResults || !hSrcSizes) return (size_t)err(E_SRC_WRONG);
     if (!hSrc) for (size_t f = 0; f < nFrames; f++) if (hSrcSizes[f]) return (size_t)err(E_SRC_WRONG);
-    return frame_compress_batch(codec, blockSizeId, nFrames, (u8*)hOut, outCapacity, hOffsets, hResults, (const u8*)hSrc, hSrcSizes);
+    return frame_compress_batch(Spanning::BATCH, codec, blockSizeId, nFrames, (u8*)hOut, outCapacity, hOffsets, hResults, (const u8*)hSrc,
+                                hSrcSizes);
 }
 
 FSEB_API size_t FSEB200_frame_compress_host(int codec, unsigned blockSizeId, void* hFrame, size_t frameCapacity,
@@ -880,7 +874,8 @@ FSEB_API size_t FSEB200_frame_compress_host(int codec, unsigned blockSizeId, voi
     if (codec < 0 || codec > 1 || blockSizeId > 6 || (!hSrc && srcSize) || (!hFrame && frameCapacity)) return (size_t)err(E_SRC_WRONG);
     if (frameCapacity < FRAME_HEADER + FRAME_TRAILER) return (size_t)err(E_DST_TOO_SMALL);
     size_t result = 0;
-    size_t const r = frame_compress_batch(codec, blockSizeId, 1, (u8*)hFrame, frameCapacity, nullptr, &result, (const u8*)hSrc, &srcSize);
+    size_t const r = frame_compress_batch(Spanning::ONE_FRAME, codec, blockSizeId, 1, (u8*)hFrame, frameCapacity, nullptr, &result,
+                                          (const u8*)hSrc, &srcSize);
     return r ? r : result;
 }
 

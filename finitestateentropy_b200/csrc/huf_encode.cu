@@ -762,7 +762,7 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
     u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch
     if constexpr (packed) {
-        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * (((size_t)step + pack::PACK_TILE - 1) / pack::PACK_TILE), &e);
+        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * pack::tiles_of(step), &e);
         if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
     }
     for (u32 b0 = 0; b0 < g.nBlocks; b0 += step) {
@@ -771,11 +771,7 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
         unsigned const grid = (sb.g.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
         hufe::huf_plan_kernel<Geo, NS><<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(sb.g, sb.cbuf, cs, sb.src, msv, tlog, plans + b0);
         if constexpr (packed) {                                     // offsets, capacity verdicts, RLE bytes, raw copies; then emit
-            unsigned const tiles = (sb.g.nBlocks + pack::PACK_TILE - 1) / pack::PACK_TILE;
-            pack::pack_sums_kernel<hufe::HufPlace><<<tiles, pack::PACK_THREADS, 0, stream>>>(sb.g, tileSum);
-            pack::pack_scan_tiles_kernel<<<1, pack::PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, b0 ? sb.g.offset : nullptr,
-                                                                                     sb.g.offset + sb.g.nBlocks);
-            pack::pack_place_kernel<hufe::HufPlace><<<tiles, pack::PACK_THREADS, 0, stream>>>(sb.g, tileSum, plans + b0);
+            pack::launch_pack<hufe::HufPlace>(sb.g, tileSum, b0 ? sb.g.offset : nullptr, sb.g.offset + sb.g.nBlocks, plans + b0, stream);
             hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g);
         }
         hufe::huf_emit_kernel<Geo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);

@@ -106,6 +106,26 @@ pack_place_kernel(typename P::Geo g, const u64* __restrict__ tileOff, typename P
     }
 }
 
+inline unsigned tiles_of(u64 n) { return (unsigned)((n + PACK_TILE - 1) / PACK_TILE); }
+// the three steps for P; tileSum: tiles_of(g.nBlocks) words; the scan starts from *carryIn (nullptr: 0), its total to *totalOut
+template <class P>
+void launch_pack(const typename P::Geo& g, u64* tileSum, const u64* carryIn, u64* totalOut, typename P::Aux aux, cudaStream_t stream)
+{
+    unsigned const tiles = tiles_of(g.nBlocks);
+    pack_sums_kernel<P><<<tiles, PACK_THREADS, 0, stream>>>(g, tileSum);
+    pack_scan_tiles_kernel<<<1, PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, carryIn, totalOut);
+    pack_place_kernel<P><<<tiles, PACK_THREADS, 0, stream>>>(g, tileSum, aux);
+}
+
+// kernel(args..., b0), one CTA of COPY_THREADS per block b0 + blockIdx.x of [0, n), in launches of at most GRID_MAX CTAs
+constexpr u64 GRID_MAX = 1ull << 30;
+template <class... K, class... A>
+void launch_per_block(void (*kernel)(K...), u64 n, cudaStream_t stream, A... args)
+{
+    for (u64 b0 = 0; b0 < n; b0 += GRID_MAX)
+        kernel<<<(unsigned)(n - b0 < GRID_MAX ? n - b0 : GRID_MAX), COPY_THREADS, 0, stream>>>(args..., b0);
+}
+
 // n bytes from s to d by the NT threads of one CTA (n < 2^32; any alignment of either).  The destination's 16-byte aligned
 // interior is written in whole 16-byte stores, the bytes before and after it one by one.  Every interior chunk's source bytes
 // sit at the same misalignment sh in the source, so they are the bytes [sh, sh + 16) of two consecutive aligned 16-byte source
