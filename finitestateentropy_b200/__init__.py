@@ -84,6 +84,9 @@ def _declare(L):
     sig("FSEB200_frame_decompress_host", c_sz, c_vp, c_sz, c_vp, c_sz)
     sig("FSEB200_frame_compress_host_batch", c_sz, C.c_int, C.c_uint, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp)
     sig("FSEB200_frame_decompress_host_batch", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_frame_compress_device", c_sz, C.c_int, C.c_uint, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_frame_decompress_bound_device", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_frame_decompress_device", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     sig("FSEB200_XXH32", C.c_uint, c_vp, c_sz, C.c_uint)
     for name in ("FSEB200_HUF_compress_batch", "FSEB200_FSE_compress_batch", "FSEB200_FSE_decompress_batch",
                  "FSEB200_FSEU16_compress_batch", "FSEB200_FSEU16_decompress_batch"):
@@ -103,4 +106,4 @@ from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch
                     fse_compress_packed, fseu16_compress_packed, fse_decompress_packed, fseu16_decompress_packed,
                     fse_packed_workspace, huf_decompress_packed, huf_decompress1x_packed,
                     host_compress_packed, host_decompress_packed, frame_compress, frame_decompress,
-                    frame_compress_batch, frame_decompress_batch)
+                    frame_compress_batch, frame_decompress_batch, frame_compress_device, frame_decompress_device)

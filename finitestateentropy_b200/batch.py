@@ -469,3 +469,85 @@ def frame_decompress_batch(frames, offsets, capacities=None):
                                                   offsets.data_ptr())
     _ret(r, "FSEB200_frame_decompress_host_batch")
     return out, results
+
+
+def _device_check(t, dtype):
+    """the device frame calls' tensor check: the dtype, then a contiguous CUDA tensor"""
+    assert t.dtype == dtype, ("dtype", t.dtype, dtype)
+    assert t.is_cuda and t.is_contiguous(), ("device", t.device, t.is_contiguous())
+
+
+def _device_sizes(sizes):
+    """host int64 sizes or offsets: the device calls take their geometry from the host"""
+    if isinstance(sizes, torch.Tensor):
+        assert sizes.dtype == torch.int64, sizes.dtype
+        sizes = sizes.cpu()
+    return _host_sizes(sizes)
+
+
+def frame_compress_device(src, sizes, codec="fse", block_size_id=5, out=None):
+    """Many .fse frames of DEVICE data in one call on the current stream, each exactly what frame_compress_batch gives for it:
+    frame f is sizes[f] bytes of `src` (a CUDA uint8 tensor) right after frame f - 1.  `sizes`: int64, on the host or read back
+    from a tensor.  With out=None the output holds the sum of the frames' compressBound, always enough; a frame that does not
+    fit `out` is not written and its result is dstSize_tooSmall.  Asynchronous.  Returns (out, offsets, results), CUDA int64
+    offsets (n + 1 entries) and results (each frame's size or error code)."""
+    from . import lib
+    cid = FRAME_CODECS[codec]
+    sizes = _device_sizes(sizes)
+    n = sizes.numel()
+    _device_check(src, torch.uint8)
+    assert bool((sizes >= 0).all()), "sizes must not be negative"
+    assert src.numel() >= int(sizes.sum()), (src.numel(), int(sizes.sum()))
+    assert 0 <= block_size_id <= 6, block_size_id
+    if out is None:
+        cap = sum(int(lib().FSEB200_frame_compressBound(int(x), block_size_id)) for x in sizes.tolist())
+        out = torch.empty(cap, dtype=torch.uint8, device=src.device)
+    _device_check(out, torch.uint8)
+    assert out.device == src.device, (out.device, src.device)
+    offsets = torch.zeros(n + 1, dtype=torch.int64, device=src.device)  # nFrames == 0 writes nothing
+    results = torch.empty(n, dtype=torch.int64, device=src.device)
+    with torch.cuda.device(src.device):
+        r = lib().FSEB200_frame_compress_device(cid, block_size_id, n, out.data_ptr() if out.numel() else offsets.data_ptr(), out.numel(),
+                                                offsets.data_ptr(), results.data_ptr(), src.data_ptr() if src.numel() else None,
+                                                _host_ptr(sizes), _stream_ptr())
+    _ret(r, "FSEB200_frame_compress_device")
+    return out, offsets, results
+
+
+def frame_decompress_device(frames, offsets, capacities=None, out=None):
+    """Many .fse frames of DEVICE data in one call on the current stream, each exactly what frame_decompress_batch gives for it:
+    frame f is frames[offsets[f]:offsets[f + 1]] (a CUDA uint8 tensor; offsets int64 on the host or read back from a tensor,
+    n + 1 entries, non-decreasing).  Frame f decodes into out[start_f : start_f + capacities[f]], start_f the sum of the earlier
+    capacities; capacities default to each frame's decompress bound (0 for a frame its header walk rejects), from the device's
+    header walk.  Synchronises the stream once, after the walk.  Returns (out, results): results (CUDA int64) as
+    frame_decompress_batch's."""
+    from . import lib, is_error
+    offsets = _device_sizes(offsets)
+    _device_check(frames, torch.uint8)
+    n = offsets.numel() - 1
+    assert n >= 0, "offsets needs n + 1 entries"
+    o = offsets.tolist()
+    assert all(o[i] <= o[i + 1] for i in range(n)) and (n == 0 or (o[0] >= 0 and o[-1] <= frames.numel())), "offsets"
+    # every frame empty: no byte is read, but the C call refuses NULL, so a 1-byte buffer stands in (as _host_ptr does)
+    stand_in = None if frames.numel() else torch.zeros(1, dtype=torch.uint8, device=frames.device)
+    live = (frames if stand_in is None else stand_in).data_ptr()
+    with torch.cuda.device(frames.device):
+        if capacities is None:
+            bounds = torch.zeros(n, dtype=torch.int64)
+            if n:
+                r = lib().FSEB200_frame_decompress_bound_device(n, bounds.data_ptr(), live, offsets.data_ptr(), _stream_ptr())
+                _ret(r, "FSEB200_frame_decompress_bound_device")
+            capacities = [0 if is_error(b % (1 << 64)) else int(b) for b in bounds.tolist()]
+        capacities = _device_sizes(capacities)
+        assert capacities.numel() == n and bool((capacities >= 0).all()), (capacities.numel(), n)
+        total = int(capacities.sum())
+        if out is None:
+            out = torch.empty(max(total, 1), dtype=torch.uint8, device=frames.device)
+        _device_check(out, torch.uint8)
+        assert out.device == frames.device and out.numel() >= total, (out.device, out.numel(), total)
+        results = torch.empty(n, dtype=torch.int64, device=frames.device)
+        if n:
+            r = lib().FSEB200_frame_decompress_device(n, out.data_ptr(), _host_ptr(capacities), results.data_ptr(), live,
+                                                      offsets.data_ptr(), _stream_ptr())
+            _ret(r, "FSEB200_frame_decompress_device")
+    return out[:total], results

@@ -9,14 +9,17 @@
 // Compress, per chunk of whole frames or pieces of one frame, after the device packed compress of its blocks (fse_packed.cu /
 // huf_encode.cu): the payloads are already the packed stream's stored blocks, in order, so the chunk's frame bodies are that
 // stream with a block header in front of each block, a frame header in front of each frame's first block and a trailer behind
-// its last.  A scan of those lengths (pack_dev.cuh) gives each block's offset and writes the headers; one CTA per block then
-// moves its payload from the packed buffer behind them and, for a frame whose hash xxh32_kernel computed, writes the trailer.
+// its last.  A scan of those lengths (pack_dev.cuh) gives each block's offset; one CTA per block then writes its headers, moves
+// its payload from the packed buffer behind them and, for a frame whose hash xxh32_kernel computed, writes the trailer.  The
+// device-memory call (frame_device.cu) lays out whole batches at once and decides per frame, between the scan and the writes,
+// whether the frame is stored: a frame of an error block takes no bytes, and a frame that ends past the capacity is not written.
 // Decompress, per chunk: the compressed blocks go to the descriptor decoders with pointers into the chunk's frame bytes (the host
 // builds the descriptors); raw and RLE blocks come from frame_stored_kernel, one CTA per block of a compact index.
 //
 // xxh32_kernel hashes many byte ranges of one device buffer in one launch: the frames' data, before the compress writes the frame
 // bodies over it, or the decoded output.  It is the public xxHash specification's XXH32 at seed 0, bit for bit.
 #include "common.cuh"
+#include "frame_walk.h"
 #include "launchers.h"
 #include "launch_util.cuh"
 #include "pack_dev.cuh"
@@ -24,28 +27,32 @@
 namespace fseb {
 namespace frame {
 
-// the packed compress's outputs for a chunk (offset: nBlocks + 1 entries) and the frame bodies they become.  role[b]: FIRST if
-// block b starts a frame, LAST if it ends one, and HASHED with the frame's index into hash[] in the upper 32 bits if the trailer
-// is written here (otherwise the host writes it)
+// the packed compress's outputs for a chunk (offset: nBlocks + 1 entries) and the frame bodies they become.  role[b]: ROLE_FIRST
+// if block b starts a frame, ROLE_LAST if it ends one, and ROLE_HASHED with the frame's index into hash[] in the upper 32 bits if the trailer
+// is written here (otherwise the host writes it).  A block of 0 source bytes is the placeholder of an empty frame: no block
+// header, no payload.
 struct Body {
     const u8* packed; const u64* offset; const u64* value; const u64* srcSize; const u64* role; const u64* hash;
-    u8* out; u64* bodyOff;                                          // bodyOff[b]: where block b's bytes start; stream scratch
+    u8* out; u64* bodyOff;                                          // bodyOff[b]: where block b's bytes start; scratch
     u64 blockSize; u32 nBlocks; u32 magic; u32 blockSizeId;
+    // FrameStore only (else nullptr: every frame is written, and the host settles error frames): role[b] >> 32 is block b's
+    // frame for every block; errBlock[f], the first block of frame f with an error value (~0: none); stored[f], frame f is written
+    const u64* errBlock; const u8* stored;
 };
 
-enum : u64 { FIRST = 1, LAST = 2, HASHED = 4 };
-constexpr u32 FRAME_HEADER = 5, FRAME_TRAILER = 3;
+using namespace fmt;
 
 // frame header and trailer bytes around block b
 __device__ __forceinline__ u32 frame_len(u64 role)
 {
-    return (role & FIRST ? FRAME_HEADER : 0) + (role & LAST ? FRAME_TRAILER : 0);
+    return (u32)((role & ROLE_FIRST ? FRAME_HEADER : 0) + (role & ROLE_LAST ? FRAME_TRAILER : 0));
 }
 
-// header bytes of a block with compress value v and n source bytes; an error value stores nothing (the host reports it)
+// header bytes of a block with compress value v and n source bytes; an error value stores nothing (the host reports it), and
+// neither does an empty frame's placeholder
 __device__ __forceinline__ u32 header_len(u64 v, u64 n, u64 blockSize)
 {
-    if (is_err(v)) return 0;
+    if (is_err(v) || n == 0) return 0;
     return 1 + (n == blockSize ? 0 : 2) + (v >= 2 ? 2 : 0);
 }
 
@@ -55,38 +62,64 @@ struct Headers {
     static __device__ __forceinline__ u64 value(const Body& g, u64 b) { return g.value[b]; }
     static __device__ __forceinline__ u64 len(const Body& g, u64 b, u64 v)
     {
+        if (g.errBlock && g.errBlock[g.role[b] >> 32] != ~0ull) return 0;
         return frame_len(g.role[b]) + header_len(v, g.srcSize[b], g.blockSize) + (g.offset[b + 1] - g.offset[b]);
     }
-    static __device__ __forceinline__ void place(const Body& g, u64*, u64 b, u64 v, u64 off, u64)
-    {
-        g.bodyOff[b] = off;
-        u8* h = g.out + off;
-        if (g.role[b] & FIRST) {
-            for (int i = 0; i < 4; i++) *h++ = (u8)(g.magic >> (8 * i));
-            *h++ = (u8)g.blockSizeId;
-        }
-        if (is_err(v)) return;
-        u64 const n = g.srcSize[b];
-        bool const full = n == g.blockSize;
-        *h++ = (u8)(((v == 0 ? 1u : v == 1 ? 2u : 0u) << 6) | (full ? 0x20u : 0u));
-        if (!full) { *h++ = (u8)(n >> 8); *h++ = (u8)n; }
-        if (v >= 2) { *h++ = (u8)(v >> 8); *h++ = (u8)v; }
-    }
+    static __device__ __forceinline__ void place(const Body& g, u64*, u64 b, u64, u64 off, u64) { g.bodyOff[b] = off; }
 };
 
-// one CTA per block (blocks b0 + blockIdx.x): the stored payload behind its header, and the trailer of a frame it ends
+// one CTA per block (blocks b0 + blockIdx.x) of a stored frame: its headers, the stored payload behind them, and the trailer of
+// a frame it ends
 __global__ void __launch_bounds__(pack::COPY_THREADS) frame_payload_kernel(Body g, u64 b0)
 {
     u64 const b = b0 + blockIdx.x;
     u64 const v = g.value[b], role = g.role[b];
+    if (g.stored && !g.stored[role >> 32]) return;
+    u64 const n = g.srcSize[b];
     u32 const L = (u32)(g.offset[b + 1] - g.offset[b]);             // at most a block, 64 KB
-    u8* const at = g.out + g.bodyOff[b] + (role & FIRST ? FRAME_HEADER : 0) + header_len(v, g.srcSize[b], g.blockSize);
-    if ((role & (LAST | HASHED)) == (LAST | HASHED) && threadIdx.x == 0) {
+    u32 const hl = header_len(v, n, g.blockSize);
+    u8* h = g.out + g.bodyOff[b];
+    u8* const at = h + (role & ROLE_FIRST ? FRAME_HEADER : 0) + hl;
+    if (threadIdx.x == 0) {
+        if (role & ROLE_FIRST) {
+            for (int i = 0; i < 4; i++) *h++ = (u8)(g.magic >> (8 * i));
+            *h++ = (u8)g.blockSizeId;
+        }
+        if (hl) {
+            bool const full = n == g.blockSize;
+            *h++ = (u8)(((v == 0 ? 1u : v == 1 ? 2u : 0u) << 6) | (full ? 0x20u : 0u));
+            if (!full) { *h++ = (u8)(n >> 8); *h++ = (u8)n; }
+            if (v >= 2) { *h++ = (u8)(v >> 8); *h++ = (u8)v; }
+        }
+    }
+    if ((role & (ROLE_LAST | ROLE_HASHED)) == (ROLE_LAST | ROLE_HASHED) && threadIdx.x == 0) {
         u32 const c = ((u32)g.hash[role >> 32] >> 5) & ((1u << 22) - 1);
         at[L] = (u8)((c >> 16) | 0xC0u); at[L + 1] = (u8)(c >> 8); at[L + 2] = (u8)c;
     }
     if (is_err(v) || L == 0) return;
     pack::cta_copy<pack::COPY_THREADS, pack::COPY_UNROLL>(at, g.packed + g.offset[b], L);
+}
+
+// FrameStore: errBlock[f] = the first block of frame f whose value is an error (errBlock starts at ~0)
+__global__ void frame_errors_kernel(Body g)
+{
+    u64 const b = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < g.nBlocks && is_err(g.value[b])) atomicMin(const_cast<u64*>(g.errBlock) + (g.role[b] >> 32), b);
+}
+
+// FrameStore, one thread per frame once the scan has placed every block: the frame's offset (its first block's), its length
+// (up to the next frame's offset, or the total), its result and whether it is written
+__global__ void frame_settle_kernel(Body g, FrameStore o, const u64* total, u8* stored)
+{
+    u32 const f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= o.nFrames) return;
+    u64 const off = g.bodyOff[o.first[f]], end = f + 1 < o.nFrames ? g.bodyOff[o.first[f + 1]] : *total;
+    u64 const e = g.errBlock[f];
+    bool const fits = e == ~0ull && end <= o.capacity;
+    o.offsets[f] = off;
+    if (f + 1 == o.nFrames) o.offsets[o.nFrames] = end;
+    o.results[f] = e != ~0ull ? g.value[e] : fits ? end - off : err(E_DST_TOO_SMALL);
+    stored[f] = fits;
 }
 
 // raw and RLE blocks of a chunk: index[3 j .. 3 j + 2] = output offset, payload offset in the chunk's frame bytes, and
@@ -192,21 +225,36 @@ __global__ void __launch_bounds__(xxh::THREADS) xxh32_kernel(const u8* __restric
 
 }  // namespace frame
 
+size_t frame_body_work(u32 nBlocks, u32 nFrames)
+{
+    return sizeof(u64) * ((size_t)nBlocks + pack::tiles_of(nBlocks) + 1 + nFrames) + nFrames;
+}
+
 cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, const u64* value, const u64* srcSize, const u64* role,
-                              const u64* hash, u32 nBlocks, u64 blockSize, u32 magic, u32 blockSizeId, cudaStream_t stream)
+                              const u64* hash, u32 nBlocks, u64 blockSize, u32 magic, u32 blockSizeId, cudaStream_t stream,
+                              const FrameStore* store)
 {
     if (nBlocks == 0) return cudaSuccess;
     size_t const n = nBlocks;
     unsigned const tiles = pack::tiles_of(n);
-    cudaError_t e;
-    u64* const s = (u64*)stream_scratch(8, stream, sizeof(u64) * (n + tiles + 1), &e);
+    cudaError_t e = cudaSuccess;
+    u64* const s = store ? (u64*)store->work : (u64*)stream_scratch(8, stream, frame_body_work(nBlocks, 0), &e);
     if (e != cudaSuccess) return e;
     frame::Body g;
     g.packed = packed; g.offset = offset; g.value = value; g.srcSize = srcSize;
     g.role = role; g.hash = hash; g.magic = magic; g.blockSizeId = blockSizeId;
     g.out = out; g.bodyOff = s; g.blockSize = blockSize; g.nBlocks = nBlocks;
+    g.errBlock = nullptr; g.stored = nullptr;
     u64* const tileSum = s + n;                                     // tiles + 1 words: the body's length goes to the last
-    pack::launch_pack<frame::Headers>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+    if (store) {
+        u64* const errBlock = tileSum + tiles + 1;
+        u8* const stored = (u8*)(errBlock + store->nFrames);
+        g.errBlock = errBlock; g.stored = stored;
+        if ((e = cudaMemsetAsync(errBlock, 0xFF, sizeof(u64) * store->nFrames, stream)) != cudaSuccess) return e;
+        frame::frame_errors_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(g);
+        pack::launch_pack<frame::Headers>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+        frame::frame_settle_kernel<<<(store->nFrames + 255) / 256, 256, 0, stream>>>(g, *store, tileSum + tiles, stored);
+    } else pack::launch_pack<frame::Headers>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
     pack::launch_per_block(frame::frame_payload_kernel, n, stream, g);
     return cudaGetLastError();
 }

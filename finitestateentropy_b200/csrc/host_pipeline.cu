@@ -4,6 +4,7 @@
 // so that PCIe transfers overlap the kernels; one driver, run_chunks, runs the chunks of every call.
 #include "capi_common.h"
 #include "fse_b200.h"
+#include "frame_walk.h"
 #include "launch_util.cuh"
 #include "xxh32.h"
 #include <algorithm>
@@ -380,10 +381,7 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
 // one-frame calls are batches of one), through the packed pair's ring and chunk budget; DESIGN 5b describes the pipeline.
 // ================================================================================================
 namespace {
-constexpr u32 MAGIC_FSE = 0x183E2309u, MAGIC_HUF = 0x183E3309u;
-constexpr u64 FRAME_HEADER = 5, FRAME_TRAILER = 3;
-enum { BT_COMPRESSED = 0, BT_RAW = 1, BT_RLE = 2, BT_END = 3 };
-enum : u64 { ROLE_FIRST = 1, ROLE_LAST = 2, ROLE_HASHED = 4 };   // frame.cu's Body::role
+using namespace fmt;
 
 // Frames of at most this many bytes that lie in one chunk are hashed on the device, the rest on host threads.  One frame is a
 // serial chain on either side, slower on the device than on a host core, so the device wins while a chunk holds many frames to
@@ -391,16 +389,12 @@ enum : u64 { ROLE_FIRST = 1, ROLE_LAST = 2, ROLE_HASHED = 4 };   // frame.cu's B
 // the device is faster up to 1 MiB, the host from 4 MiB, and at 2 MiB each wins one direction.
 constexpr u64 DEVICE_HASH_MAX = 1ull << 20;
 
-u32 trailer_checksum(u32 h) { return (h >> 5) & ((1u << 22) - 1); }
-u64 be16(const u8* p) { return (u64)p[0] << 8 | p[1]; }
 void put_trailer(u8* t, u32 hash)
 {
     u32 const crc = trailer_checksum(hash);
     t[0] = (u8)((crc >> 16) | (BT_END << 6)); t[1] = (u8)(crc >> 8); t[2] = (u8)crc;
 }
 u64 block_header_len(u64 v, u64 n, u64 bs) { return 1 + (n == bs ? 0 : 2) + (v >= 2 ? 2 : 0); }
-
-struct FrameBlock { u64 head, payload, rSize, cSize; int type; };   // header and payload offsets in the frame
 
 struct FrameWalk {
     size_t verdict = 0;             // 0, or the verdict where the walk stopped (the point FIO_decompressFilename stops at)
@@ -409,43 +403,16 @@ struct FrameWalk {
     u32 checksum = 0;               // the trailer's 22 bits (verdict 0)
 };
 
-// the reference's header walk, with its exit codes as verdicts; blocks that would overrun its buffers are corruption_detected
+// the reference's header walk, with its exit codes as verdicts (frame_walk.h)
 FrameWalk walk_frame(const u8* f, u64 size)
 {
     FrameWalk w;
-    auto stop = [&w](unsigned code) { w.verdict = (size_t)err(code); };
-    if (size < FRAME_HEADER) { stop(E_SRC_WRONG); return w; }                                  // exit 30
-    u32 const magic = (u32)f[0] | (u32)f[1] << 8 | (u32)f[2] << 16 | (u32)f[3] << 24;
-    if (magic != MAGIC_FSE && magic != MAGIC_HUF) { stop(E_GENERIC); return w; }             // 31 (zlibh too)
-    if (f[4] > 6) { stop(E_GENERIC); return w; }                                              // 32
-    w.codec = magic == MAGIC_HUF;
-    u64 const bs = (u64)1024 << f[4];
-    u64 pos = FRAME_HEADER;
-    if (pos >= size) { stop(E_SRC_WRONG); return w; }                                         // 34
-    for (;;) {
-        FrameBlock k;
-        k.head = pos;
-        k.type = f[pos] >> 6;
-        if (k.type == BT_END) break;
-        bool const full = f[pos] & 0x20;
-        pos++;
-        k.rSize = bs;
-        if (!full) {
-            if (pos + 2 > size) { stop(E_SRC_WRONG); return w; }                              // 35
-            k.rSize = be16(f + pos); pos += 2;
-        }
-        if (k.type == BT_COMPRESSED) {
-            if (pos + 2 > size) { stop(E_SRC_WRONG); return w; }                              // 36
-            k.cSize = be16(f + pos); pos += 2;
-        } else k.cSize = k.type == BT_RAW ? k.rSize : 1;
-        if (k.cSize > bs + 4) { stop(E_CORRUPT); return w; }                                  // past its input buffer
-        if (pos + k.cSize + 1 > size) { stop(E_SRC_WRONG); return w; }                        // 38: payload + next header byte
-        if (k.type != BT_RAW && k.rSize > bs) { stop(E_CORRUPT); return w; }                  // past its output buffer
-        k.payload = pos; pos += k.cSize;
-        w.blocks.push_back(k);
-    }
-    if (pos + FRAME_TRAILER > size) { stop(E_SRC_WRONG); return w; }                          // 43
-    w.checksum = (u32)be16(f + pos + 1) | (u32)(f[pos] & 0x3F) << 16;
+    WalkState s;
+    FrameBlock k;
+    u64 r;
+    while ((r = walk_step(f, size, s, k)) == WALK_BLOCK) w.blocks.push_back(k);
+    if (r != WALK_END) w.verdict = (size_t)r;
+    w.codec = s.codec; w.checksum = s.checksum;
     return w;
 }
 

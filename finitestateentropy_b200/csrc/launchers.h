@@ -31,8 +31,14 @@ cudaError_t launch_fse_decompress_packed(u8* const* dst, const u64* dstSize, u64
                                          u32 nBlocks, bool wide, cudaStream_t stream);
 cudaError_t launch_huf_decompress_packed(u8* const* dst, const u64* dstSize, u64* result, const u8* in, const u64* offset,
                                          u32 nBlocks, int nStreams, cudaStream_t stream);
+// A whole batch of frames laid out at once (the device-memory call): frame f is blocks [first[f], first[f + 1]), role[b] >> 32
+// is block b's frame, and every frame has a block (an empty frame a placeholder of 0 source bytes).  offsets (nFrames + 1) and
+// results get the batch call's values, and only frames that end at or before `capacity` are written; work: frame_body_work bytes.
+struct FrameStore { u32 nFrames; const u64* first; u64 capacity; u64* offsets; u64* results; void* work; };
+size_t frame_body_work(u32 nBlocks, u32 nFrames);
 cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, const u64* value, const u64* srcSize, const u64* role,
-                              const u64* hash, u32 nBlocks, u64 blockSize, u32 magic, u32 blockSizeId, cudaStream_t stream);
+                              const u64* hash, u32 nBlocks, u64 blockSize, u32 magic, u32 blockSizeId, cudaStream_t stream,
+                              const FrameStore* store = nullptr);
 cudaError_t launch_frame_stored(u8* out, const u8* in, const u64* index, u64 nStored, cudaStream_t stream);
 cudaError_t launch_xxh32_ranges(const u8* base, const u64* desc, u32 n, u64* hash, cudaStream_t stream);
 

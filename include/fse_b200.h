@@ -358,6 +358,52 @@ size_t   FSEB200_frame_decompress_host_batch(size_t nFrames, void* hDst, const s
                                              const void* hIn, const size_t* hOffsets);
 unsigned FSEB200_XXH32(const void* src, size_t srcSize, unsigned seed);
 
+/* Tier 1, frames on DEVICE memory: the frame batches above for data already on the GPU.  Geometry on the host, bytes on the
+ * device: arguments starting with h are host arrays, read only during the call; arguments starting with d are device memory, at
+ * any byte alignment.  Per frame, each call gives exactly what the matching host call gives for the same frames -- every result
+ * value, offset, verdict and stored byte, and the capacity rule -- so only the differences are stated here.
+ *   compress_device: as FSEB200_frame_compress_host_batch.  Frame f's source is hSrcSizes[f] bytes at dSrc + hSrcSizes[0] + ...
+ *               + hSrcSizes[f - 1]; dOffsets (nFrames + 1 entries) and dResults are written on the device.  A frame is stored,
+ *               at dOut + dOffsets[f], only if it ends at or before outCapacity; otherwise its result is dstSize_tooSmall.
+ *               Nothing outside the stored frames is written (the host call's exception for frames that span chunks does not
+ *               apply: there are no chunks).  An empty source gives the 8-byte frame; the blocks are coded at (255, 11).
+ *               Fully asynchronous on `stream`: the host never reads device memory and never waits for the device.  The block
+ *               layout is uploaded from a pinned host image of the library's.  The checksums run on a second stream that the
+ *               library keeps for `stream`, forked from it and joined back into it by events on the device, so everything the
+ *               call does is ordered by `stream` and calls on different streams do not wait for each other.  (The packed
+ *               coders keep per-stream scratch whose growth synchronises that stream and frees device memory, as the device
+ *               packed calls do: the first calls on a stream, or a larger batch than before, may wait.)
+ *   decompress_device: as FSEB200_frame_decompress_host_batch.  Frame f is dIn[hOffsets[f], hOffsets[f + 1]); its region starts
+ *               at dDst plus the earlier capacities and holds hDstCapacities[f] bytes.  A failing frame leaves its region
+ *               unspecified and does not stop the others; nothing outside the regions is written.  The call SYNCHRONISES
+ *               `stream` once: after the header walk on the device, to learn how many blocks to launch.  Everything after it
+ *               is enqueued, and dResults is valid when the stream reaches it.  (As in compress, the decoders' per-stream
+ *               scratch synchronises the stream again, and frees device memory, when it grows.)  dIn must be readable up to the end
+ *               of the 32-byte sector that holds the last frame's last byte (every cudaMalloc and torch allocation is).
+ *   decompress_bound_device: synchronous; the header walk alone, writing FSEB200_frame_decompress_bound's value (or verdict)
+ *               for each frame to hBounds.
+ * Checksums: every frame is hashed on the device by one kernel, four lanes per frame, whatever its length.  One frame's hash
+ * is a serial chain, measured at about 0.5 GB/s on an H100 80GB HBM3 at 700 W (DESIGN.md 5b): a single large frame is bound by
+ * it, and runs several times slower than through the host batch calls, which hash such frames on host threads.
+ * Scratch, all stream-ordered (cudaMallocAsync on `stream`), no chunking: compress, the source's size plus 32 bytes for the
+ * packed blocks, FSEB200_FSE_packed_workspace(blocks, source size) for FSE, about 6 words per block and 6 per frame;
+ * decompress, 5 words per compressed block, 3 per raw or RLE block and 2 per block, 19 words per frame, and the nominal output
+ * of every frame with compressed blocks whose nominal output passes its capacity (it decodes there and its true bytes are
+ * then copied in).  That nominal output is what the frame's block headers claim, up to 64 KiB per 3-byte header, so a
+ * malformed or hostile frame with a small capacity can ask for far more scratch than its size; when the allocation fails
+ * the whole call returns generic, where the host batch call would give that frame its verdict.  A caller decoding untrusted
+ * frames can run FSEB200_frame_decompress_bound_device first and reject frames whose bound passes its capacity by too much.  Calls on different streams or host threads may run at once; they take no lock the host calls hold.
+ * Return value: 0 (also for nFrames == 0, which launches nothing); srcSize_wrong for a bad codec, blockSizeId > 6, nFrames >
+ * 0xFFFFFFFF, more than 0xFFFFFFFF blocks, a NULL pointer while nFrames > 0 (dSrc may be NULL when every size is 0), or
+ * offsets that decrease (decompress, bound); these checks touch no device.  generic if a CUDA call fails. */
+size_t FSEB200_frame_compress_device(int codec, unsigned blockSizeId, size_t nFrames,
+                                     void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dResults,
+                                     const void* dSrc, const size_t* hSrcSizes, void* stream);
+size_t FSEB200_frame_decompress_bound_device(size_t nFrames, size_t* hBounds,
+                                             const void* dIn, const size_t* hOffsets, void* stream);
+size_t FSEB200_frame_decompress_device(size_t nFrames, void* dDst, const size_t* hDstCapacities, size_t* dResults,
+                                       const void* dIn, const size_t* hOffsets, void* stream);
+
 /* Measurement inputs generated directly in device memory: byte i of the output equals byte
  * (streamOffset + i) of the reference generator's stream (programs/probaGenerator.c:95-126 with
  * probability p, seed 1; programs/fuzzerU16.c:107-134 with the given start / p / seed). */
