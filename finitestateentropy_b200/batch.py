@@ -151,6 +151,63 @@ def huf_decompress1x_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=
     return _codec_blocks("FSEB200_HUF_decompress1X_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes), results)
 
 
+def huf_compress_repeat_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, repeats, prefer, csizes=None,
+                               max_symbol_value=255, table_log=12):
+    """HUF_compress4X_repeat on every block b: src_ptrs[b] / src_sizes[b] into dst_ptrs[b] of capacity dst_caps[b], with the
+    table at ctables[b] (int64 device address of 256 uint32 cells), the flag repeats[b] (int32 HUF_repeat: none 0, check 1,
+    valid 2) and prefer[b] (int32 preferRepeat), on the current stream.  Updates the tables and flags where the reference does.
+    Returns csizes (int64).  A block of 2 or more bytes with repeats[b] != 0 afterwards carries no tree header."""
+    return _repeat_blocks("FSEB200_HUF_compress4X_repeat_blocks", src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, repeats,
+                          prefer, csizes, max_symbol_value, table_log)
+
+
+def huf_compress1x_repeat_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, repeats, prefer, csizes=None,
+                                 max_symbol_value=255, table_log=12):
+    """huf_compress_repeat_blocks in the single-stream format (HUF_compress1X_repeat per block)"""
+    return _repeat_blocks("FSEB200_HUF_compress1X_repeat_blocks", src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, repeats,
+                          prefer, csizes, max_symbol_value, table_log)
+
+
+def _repeat_blocks(fn_name, src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, repeats, prefer, csizes, msv, tlog):
+    from . import lib
+    if csizes is None:
+        csizes = torch.empty(src_ptrs.numel(), dtype=torch.int64, device=src_ptrs.device)
+    n = _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, ctables)
+    for a in (repeats, prefer):
+        _check(a, torch.int32)
+        assert a.numel() == n and a.device == src_ptrs.device, (a.numel(), n, a.device)
+    r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
+                                src_sizes.data_ptr(), ctables.data_ptr(), repeats.data_ptr(), prefer.data_ptr(), msv, tlog,
+                                _stream_ptr())
+    _ret(r, fn_name)
+    return csizes
+
+
+def huf_decompress_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results=None):
+    """Every block b of csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of dst_sizes[b] bytes, on the current stream: with
+    hdr_sizes[b] == 0, HUF_decompress4X1_DCtx (the block's own tree header); otherwise HUF_readDTableX1 on hdr_ptrs[b] /
+    hdr_sizes[b] and HUF_decompress4X1_usingDTable on the block.  Returns results (int64)."""
+    return _header_blocks("FSEB200_HUF_decompress4X_repeat_blocks", csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs,
+                          hdr_sizes, results)
+
+
+def huf_decompress1x_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results=None):
+    """huf_decompress_repeat_blocks in the single-stream format (HUF_decompress1X1_DCtx / HUF_decompress1X1_usingDTable)"""
+    return _header_blocks("FSEB200_HUF_decompress1X_repeat_blocks", csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs,
+                          hdr_sizes, results)
+
+
+def _header_blocks(fn_name, csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results):
+    from . import lib
+    if results is None:
+        results = torch.empty(csrc_ptrs.numel(), dtype=torch.int64, device=csrc_ptrs.device)
+    n = _blocks_args(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results, hdr_ptrs, hdr_sizes)
+    r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), csrc_ptrs.data_ptr(),
+                                csrc_sizes.data_ptr(), hdr_ptrs.data_ptr(), hdr_sizes.data_ptr(), _stream_ptr())
+    _ret(r, fn_name)
+    return results
+
+
 def huf_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, max_symbol_value=255, table_log=12):
     """HUF_compress2 on every block b (src_ptrs[b] / src_sizes[b]) at capacity HUF_compressBound, the results stored back to
     back in `out` (capacity out.numel()), on the current stream.  Returns (out, offsets, csizes): offsets (int64, n + 1 entries)

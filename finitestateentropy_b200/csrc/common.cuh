@@ -81,6 +81,28 @@ __host__ __forceinline__ BlockDescs slice(const BlockDescs& g, u32 b0, u32 n)   
     return s;
 }
 
+// Table reuse (Huff0 compress only): a descriptor batch whose block b also carries its stream's (table, repeat flag) pair --
+// ctable[b] = 256 HUF_CElt cells (val | nbBits << 16), repeat[b] = HUF_repeat as an int, prefer[b] = preferRepeat.  The plan
+// kernel reads and writes the pair; the emit kernel sees the batch as the BlockDescs it derives from.
+struct RepeatDescs : BlockDescs {
+    u32* const* ctable;
+    int* repeat;
+    const int* prefer;
+};
+__host__ __forceinline__ RepeatDescs slice(const RepeatDescs& g, u32 b0, u32 n)
+{
+    RepeatDescs s = g;
+    static_cast<BlockDescs&>(s) = slice(static_cast<const BlockDescs&>(g), b0, n);
+    s.ctable += b0; s.repeat += b0; s.prefer += b0;
+    return s;
+}
+// Header-less decode (Huff0 only): block b's tree header is read from hdr[b] (hdrSize[b] bytes, the table's bound) and its
+// payload starts at src[b][0]; hdrSize[b] == 0 means the block carries its own header.
+struct HeaderDescs : BlockDescs {
+    const u8* const* hdr;
+    const u64* hdrSize;
+};
+
 // -------------------------------------------------------------------------------------------
 // Packed geometry (Huff0 compress only): sources by descriptor, outputs back to back in one buffer.  Block b is stored at
 // out + offset[b], offset[] being the exclusive prefix sum of the stored lengths (include/fse_b200.h); its capacity is

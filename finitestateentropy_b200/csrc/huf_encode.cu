@@ -1,7 +1,7 @@
 // huf_encode.cu -- batched Huff0 4-stream encode for sm_90a.
 //
 // Replaces, per block, the CPU chain
-//   HUF_compress2 / HUF_compress_internal  lib/huf_compress.c:637-724,787-793 (no table reuse)
+//   HUF_compress2 / HUF_compress_internal  lib/huf_compress.c:637-724,787-793 (table reuse: RepeatDescs, huf_plan_kernel)
 //   HIST_count_wksp                        lib/hist.c:163-173
 //   HUF_optimalTableLog                    lib/huf_compress.c:48-51
 //   HUF_buildCTable_wksp (+HUF_sort, HUF_setMaxHeight)  lib/huf_compress.c:215-410
@@ -159,6 +159,11 @@ __device__ __forceinline__ void warp_hist4_pipelined(u32 (*count4)[256], const u
 
 // NS = streams per block: 4 (HUF_compress2, the 4X format) or 1 (HUF_compress1X, descriptor batches only).  Phases 1 and 2 are
 // the same for both; phase 3 sizes NS streams and applies that format's capacity rule.
+// Geo = RepeatDescs: HUF_compress{4X,1X}_repeat per block (huf_compress.c:653-724), with the block's (table, flag) pair.  Phase 1
+// takes the old-table exits that need no tree (prefer + valid before the histogram exits, validation under check, prefer + any
+// flag after them) and marks the block; phase 2 builds trees only for the other blocks; phase 3 compares the estimates, saves a
+// new table, and sizes the streams with the chosen table (hSize 0 for the old one).  S.live then also tells the three apart:
+// 1 = new table, 2 = new table unless the estimates prefer the old one, 3 = old table.
 template <class Geo, int NS>
 __global__ void __launch_bounds__(32 * PLAN_WARPS, 3)
 huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8* __restrict__ src,
@@ -169,6 +174,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
     PlanCta& S = *reinterpret_cast<PlanCta*>(smem_raw);
     unsigned const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     u32 const b0 = blockIdx.x * GROUP;
+    constexpr bool REP = std::is_same_v<Geo, RepeatDescs>;
 #define FSEB_FINAL(v) { if (lane == 0) { P.state = 1; enc_out(g, csizes, b) = (v); S.live[c] = 0; } continue; }   // next block of the loop
 
     // ---- phase 1: one warp per block ----
@@ -189,6 +195,9 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         if (tlogReq > HUF_MAX_TLOG) FSEB_FINAL(err(E_TLOG_TOO_LARGE));
         if (msvReq > HUF_MAX_SV) FSEB_FINAL(err(E_MSV_TOO_LARGE));
         unsigned const msvDecl = msvReq ? msvReq : HUF_MAX_SV;
+        int flag = 0; bool prefer = false;
+        if constexpr (REP) { flag = g.repeat[b]; prefer = g.prefer[b] != 0; }
+        bool const oldNow = REP && prefer && flag == 2;                                           // :665-669: no histogram exit
 
         // histograms, one per 4X segment (HIST_count_wksp semantics for their sum, hist.c:163-173,128)
         u32 const seg = (n + 3) / 4;
@@ -213,18 +222,33 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         }
         #pragma unroll
         for (int dlt = 16; dlt; dlt >>= 1) { top = max(top, __shfl_xor_sync(FULL, top, dlt)); best = max(best, __shfl_xor_sync(FULL, best, dlt)); }
-        if (msvDecl < 255 && top > msvDecl) FSEB_FINAL(err(E_MSV_TOO_SMALL));                     // hist.c:128
-        if (best == n) {                                                                          // huf_compress.c:673
-            if constexpr (!std::is_same_v<Geo, PackedDescs>) { if (lane == 0) enc_dst(g, cbuf, b)[0] = s[0]; }   // packed: placement writes it
-            FSEB_FINAL(1);
+        if (!oldNow) {
+            if (msvDecl < 255 && top > msvDecl) FSEB_FINAL(err(E_MSV_TOO_SMALL));                 // hist.c:128
+            if (best == n) {                                                                      // huf_compress.c:673
+                if constexpr (!std::is_same_v<Geo, PackedDescs>) { if (lane == 0) enc_dst(g, cbuf, b)[0] = s[0]; }   // packed: placement writes it
+                FSEB_FINAL(1);
+            }
+            if (best <= (n >> 7) + 4) FSEB_FINAL(0);                                              // :674
         }
-        if (best <= (n >> 7) + 4) FSEB_FINAL(0);                                                  // :674
         u32 const msv = top;
         // segment counts for phase 3, compacted to u16
         #pragma unroll
         for (u32 k = 0; k < 4; k++)
             #pragma unroll
             for (u32 i = 0; i < 8; i++) P.segCount[k][i * 32 + lane] = (u16)count4[k][i * 32 + lane];
+        if constexpr (REP) {
+            if (!oldNow && flag == 1) {                                                           // :679-683 HUF_validateCTable
+                const u32* const old = g.ctable[b];
+                bool bad = false;
+                #pragma unroll
+                for (u32 i = 0; i < 8; i++) { u32 const sy = i * 32 + lane; bad |= sy <= msv && cnt[i] && ((old[sy] >> 16) & 0xFFu) == 0; }
+                if (__any_sync(FULL, bad)) { flag = 0; if (lane == 0) g.repeat[b] = 0; }
+            }
+            if (oldNow || (prefer && flag != 0)) {                                                // :685-689
+                if (lane == 0) { S.msv[c] = (u16)msv; S.live[c] = 3; }
+                continue;
+            }
+        }
         // HUF_sort (huf_compress.c:307-329): decreasing count, ties by increasing symbol == decreasing (count << 8 | 255 - symbol)
         u32 key[8], nnz = 0;
         #pragma unroll
@@ -237,7 +261,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         }
         if (lane == 0) {
             S.nd[0][c] = 0;
-            S.msv[c] = (u16)msv; S.last[c] = (u8)(nnz - 1); S.live[c] = 1;
+            S.msv[c] = (u16)msv; S.last[c] = (u8)(nnz - 1); S.live[c] = (REP && flag != 0) ? 2 : 1;
             S.tlog[c] = (u8)d_optimal_tablelog(tlogReq ? tlogReq : HUF_DEF_TLOG, n, msv, 1);     // huf_compress.c:691
         }
     }
@@ -246,7 +270,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
     // ---- phase 2: warp 0, lane c builds block c's table (huf_compress.c:338-410, then :703-716) ----
     if (warp == 0) {
         u32 const c = lane;
-        bool const live = S.live[c];
+        bool const live = REP ? (S.live[c] == 1 || S.live[c] == 2) : S.live[c];     // REP: no tree for an old-table block
         u32 const msv = S.msv[c];
         u32* const col = &S.nd[1][c];                                   // node i at col[i * GROUP]
         auto at = [&](int i) -> u32& { return col[i * (int)GROUP]; };
@@ -311,15 +335,49 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         u32 const n = enc_len(g, b);
         u64 const cap = enc_cap(g, b);
         Plan& P = plans[b];
-        u64 const hs = S.res[c];
-        if (is_err(hs)) FSEB_FINAL(hs);
-        if (hs + 12 >= n) FSEB_FINAL(0);
+        u64 hs = S.res[c];
+        bool useOld = false;
+        if constexpr (REP) useOld = S.live[c] == 3;
+        if (!useOld) {
+            if (is_err(hs)) FSEB_FINAL(hs);
+            if constexpr (REP) {
+                u32 const msv = S.msv[c];
+                u32* const tab = g.ctable[b];
+                if (S.live[c] == 2) {                                                             // :703-713 HUF_estimateCompressedSize, old and new
+                    u32 oldBits = 0, newBits = 0;
+                    #pragma unroll
+                    for (u32 i = 0; i < 8; i++) {
+                        u32 const sy = i * 32 + lane;
+                        if (sy > msv) continue;
+                        u32 const cnt = (u32)P.segCount[0][sy] + P.segCount[1][sy] + P.segCount[2][sy] + P.segCount[3][sy];
+                        oldBits += cnt * ((tab[sy] >> 16) & 0xFFu);
+                        newBits += cnt * (S.nd[CT_ROW + sy][c] >> 16);
+                    }
+                    #pragma unroll
+                    for (int dlt = 16; dlt; dlt >>= 1) { oldBits += __shfl_xor_sync(FULL, oldBits, dlt); newBits += __shfl_xor_sync(FULL, newBits, dlt); }
+                    useOld = (oldBits >> 3) <= hs + (newBits >> 3) || hs + 12 >= n;
+                }
+                if (!useOld && hs + 12 < n) {                                                     // :716-719 the new table is saved, the flag set to none
+                    #pragma unroll
+                    for (u32 i = 0; i < 8; i++) { u32 const sy = i * 32 + lane; tab[sy] = sy <= msv ? S.nd[CT_ROW + sy][c] : 0u; }
+                    if (lane == 0) g.repeat[b] = 0;
+                }
+            }
+            if (!useOld && hs + 12 >= n) FSEB_FINAL(0);
+        }
+        if (useOld) hs = 0;                                                                       // HUF_compressCTable_internal at ostart
         u64 const capLeft = cap - hs;
         if (NS == 4 && (capLeft < 6 + 1 + 1 + 1 + 8 || n < 12)) FSEB_FINAL(0);                    // :564-565
         u32 const msv = S.msv[c];
         u32 cell[8];
         #pragma unroll
         for (u32 i = 0; i < 8; i++) cell[i] = (i * 32 + lane <= msv) ? S.nd[CT_ROW + i * 32 + lane][c] : 0u;
+        if constexpr (REP) {                                                                      // every cell: prefer + valid codes symbols above msv
+            if (useOld) {
+                #pragma unroll
+                for (u32 i = 0; i < 8; i++) cell[i] = g.ctable[b][i * 32 + lane] & 0xFFFFFFu;      // byte 3 is padding
+            }
+        }
         u32 bits[NS];
         #pragma unroll
         for (int k = 0; k < NS; k++) {
@@ -734,6 +792,8 @@ struct SubDescs { BlockDescs g; u8* cbuf; const u8* src; };
 SubDescs sub_batch(const BlockDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
 struct SubPacked { PackedDescs g; u8* cbuf; const u8* src; };
 SubPacked sub_batch(const PackedDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
+struct SubRepeat { RepeatDescs g; u8* cbuf; const u8* src; };
+SubRepeat sub_batch(const RepeatDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
 
 template <class Geo, int NS>
 cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, unsigned msv, unsigned tlog, cudaStream_t stream)
@@ -760,6 +820,7 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     if (e != cudaSuccess) return e;
     u32 const step = (subBatch && subBatch < g.nBlocks) ? subBatch : g.nBlocks;
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
+    using EmitGeo = std::conditional_t<std::is_same_v<Geo, RepeatDescs>, BlockDescs, Geo>;   // the plan holds the chosen table
     u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch
     if constexpr (packed) {
         tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * pack::tiles_of(step), &e);
@@ -774,7 +835,7 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
             pack::launch_pack<hufe::HufPlace>(sb.g, tileSum, b0 ? sb.g.offset : nullptr, sb.g.offset + sb.g.nBlocks, plans + b0, stream);
             hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g);
         }
-        hufe::huf_emit_kernel<Geo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);
+        hufe::huf_emit_kernel<EmitGeo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);
     }
     e = cudaGetLastError();
     cudaError_t const e2 = asyncScratch ? cudaFreeAsync(plans, stream) : cudaSuccess;
@@ -794,6 +855,13 @@ cudaError_t launch_huf_encode_blocks(const BlockDescs& g, int nStreams, unsigned
 {
     return nStreams == 1 ? huf_encode<BlockDescs, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
                          : huf_encode<BlockDescs, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+}
+
+// table reuse (RepeatDescs): HUF_compress4X_repeat (nStreams 4) or HUF_compress1X_repeat (1) per block, the same kernels
+cudaError_t launch_huf_encode_repeat(const RepeatDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return nStreams == 1 ? huf_encode<RepeatDescs, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
+                         : huf_encode<RepeatDescs, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
 }
 
 // packed output (PackedDescs): the same kernels with the scan and placement between plan and emit
