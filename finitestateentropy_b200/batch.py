@@ -183,6 +183,52 @@ def _repeat_blocks(fn_name, src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, re
     return csizes
 
 
+def huf_compress_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, ctables, repeats, chain_hdr_ptrs,
+                               chain_hdr_sizes, csizes=None, hdr_ptrs=None, hdr_sizes=None, max_symbol_value=255, table_log=12):
+    """HUF_compress4X_repeat block after block along each chain, on the current stream: chain c is blocks
+    [chain_starts[c], chain_starts[c + 1]) (int64, n_chains + 1 entries), coded into dst_ptrs[b] of capacity dst_caps[b] with
+    prefer[b] (int32); the stream's state is ctables[c] (int64 device address of 256 uint32 cells), repeats[c] (int32 HUF_repeat)
+    and its header chain_hdr_ptrs[c] / chain_hdr_sizes[c] (int64), read at the start and updated at the end of the chain.
+    Returns (csizes, hdr_ptrs, hdr_sizes) (int64): block b's value and the header it was coded with (0 / 0: its own, or none),
+    as FSEB200_HUF_decompress4X_repeat_blocks takes them."""
+    return _repeat_chains("FSEB200_HUF_compress4X_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer,
+                          ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, max_symbol_value, table_log)
+
+
+def huf_compress1x_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, ctables, repeats, chain_hdr_ptrs,
+                                 chain_hdr_sizes, csizes=None, hdr_ptrs=None, hdr_sizes=None, max_symbol_value=255, table_log=12):
+    """huf_compress_repeat_chains in the single-stream format (HUF_compress1X_repeat per block)"""
+    return _repeat_chains("FSEB200_HUF_compress1X_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer,
+                          ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, max_symbol_value, table_log)
+
+
+def _repeat_chains(fn_name, chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, ctables, repeats, chain_hdr_ptrs,
+                   chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, msv, tlog):
+    from . import lib
+    n = src_ptrs.numel()
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=src_ptrs.device)
+    if hdr_ptrs is None:
+        hdr_ptrs = torch.empty(n, dtype=torch.int64, device=src_ptrs.device)
+    if hdr_sizes is None:
+        hdr_sizes = torch.empty(n, dtype=torch.int64, device=src_ptrs.device)
+    _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, hdr_ptrs, hdr_sizes)
+    _check(prefer, torch.int32)
+    assert prefer.numel() == n and prefer.device == src_ptrs.device, (prefer.numel(), n, prefer.device)
+    _check(chain_starts, torch.int64)
+    n_chains = chain_starts.numel() - 1
+    assert n_chains >= 0 and chain_starts.device == src_ptrs.device, (chain_starts.numel(), chain_starts.device)
+    for a, dtype in ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64)):
+        _check(a, dtype)
+        assert a.numel() == n_chains and a.device == src_ptrs.device, (a.numel(), n_chains, a.device)
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(),
+                                src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(), ctables.data_ptr(),
+                                repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(), hdr_ptrs.data_ptr(),
+                                hdr_sizes.data_ptr(), msv, tlog, _stream_ptr())
+    _ret(r, fn_name)
+    return csizes, hdr_ptrs, hdr_sizes
+
+
 def huf_decompress_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results=None):
     """Every block b of csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of dst_sizes[b] bytes, on the current stream: with
     hdr_sizes[b] == 0, HUF_decompress4X1_DCtx (the block's own tree header); otherwise HUF_readDTableX1 on hdr_ptrs[b] /

@@ -235,6 +235,45 @@ FSEB_API size_t FSEB200_HUF_compress1X_repeat_blocks(size_t nBlocks, void* const
     return huf_repeat_blocks(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, dCTables, dRepeats, dPreferRepeat, 1,
                              maxSymbolValue, tableLog, stream);
 }
+// Chains: blocks of one stream in one call, the stream's state carried from block to block on the device (common.cuh ChainDescs).
+namespace {
+size_t huf_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities,
+                         size_t* dCSizes, const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                         unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                         const void** dHeaders, size_t* dHeaderSizes, int nStreams, unsigned msv, unsigned tlog, void* stream)
+{
+    if (nBlocks && (nChains > 0xFFFFFFFFull || !dChainStarts || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders ||
+                    !dChainHeaderSizes || !dHeaders || !dHeaderSizes)) return (size_t)err(E_SRC_WRONG);
+    return blocks_call(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, [&](const BlockDescs& d) {
+        ChainDescs g;
+        static_cast<BlockDescs&>(g) = d;
+        g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
+        g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.hdr = (const u8**)dChainHeaders; g.hdrSize = (u64*)dChainHeaderSizes;
+        g.blkHdr = (const u8**)dHeaders; g.blkHdrSize = (u64*)dHeaderSizes; g.fact = nullptr;
+        return launch_huf_encode_chains(g, nStreams, msv, tlog, (cudaStream_t)stream);
+    });
+}
+}
+FSEB_API size_t FSEB200_HUF_compress4X_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
+                                                     const size_t* dDstCapacities, size_t* dCSizes, const void* const* dSrcs,
+                                                     const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables,
+                                                     int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                     const void** dHeaders, size_t* dHeaderSizes, unsigned maxSymbolValue,
+                                                     unsigned tableLog, void* stream)
+{
+    return huf_repeat_chains(nChains, dChainStarts, nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, dPreferRepeat, dCTables,
+                             dRepeats, dChainHeaders, dChainHeaderSizes, dHeaders, dHeaderSizes, 4, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_HUF_compress1X_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
+                                                     const size_t* dDstCapacities, size_t* dCSizes, const void* const* dSrcs,
+                                                     const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables,
+                                                     int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                     const void** dHeaders, size_t* dHeaderSizes, unsigned maxSymbolValue,
+                                                     unsigned tableLog, void* stream)
+{
+    return huf_repeat_chains(nChains, dChainStarts, nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, dPreferRepeat, dCTables,
+                             dRepeats, dChainHeaders, dChainHeaderSizes, dHeaders, dHeaderSizes, 1, maxSymbolValue, tableLog, stream);
+}
 FSEB_API size_t FSEB200_HUF_decompress4X_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                                        const void* const* dCSrcs, const size_t* dCSrcSizes, const void* const* dHeaders,
                                                        const size_t* dHeaderSizes, void* stream)

@@ -96,6 +96,31 @@ __host__ __forceinline__ RepeatDescs slice(const RepeatDescs& g, u32 b0, u32 n)
     s.ctable += b0; s.repeat += b0; s.prefer += b0;
     return s;
 }
+// Chains of table reuse (Huff0 compress only): chain c is blocks [start[c], start[c + 1]) of one stream, in order; the stream's
+// (table, flag, header) state comes in through ctable[c] / repeat[c] / hdr[c] / hdrSize[c] and goes back out there, and block b
+// gets the header it was coded with in blkHdr[b] / blkHdrSize[b].  The plan kernel sees only the blocks and writes nothing but
+// scratch: the state-independent facts of block b go to fact[b], and huf_chain_kernel walks each chain's decisions from them.
+struct __align__(16) ChainFact {
+    u64 exitValue;                 // kind CF_ARGS / CF_HIST: the verdict of that exit
+    u64 hSize;                     // kind CF_TREE: the new table's header size, or an error
+    u64 newValue;                  // kind CF_TREE with hSize + 12 < srcSize: the verdict with the new table (its plan is complete)
+    u32 newBits;                   // ... and its HUF_estimateCompressedSize in bits
+    u16 msv;                       // largest symbol present (kinds CF_HIST and CF_TREE)
+    u8 kind;
+};
+enum : u8 { CF_ARGS = 0, CF_HIST = 1, CF_TREE = 2 };   // an argument verdict, a histogram exit, a tree was built
+struct ChainDescs : BlockDescs {
+    const u64* start;              // nChains + 1 entries
+    u32 nChains;
+    const int* prefer;             // per block
+    u32* const* ctable;            // per chain, in-out
+    int* repeat;
+    const u8** hdr;
+    u64* hdrSize;
+    const u8** blkHdr;             // per block, out
+    u64* blkHdrSize;
+    ChainFact* fact;               // per block, scratch
+};
 // Header-less decode (Huff0 only): block b's tree header is read from hdr[b] (hdrSize[b] bytes, the table's bound) and its
 // payload starts at src[b][0]; hdrSize[b] == 0 means the block carries its own header.
 struct HeaderDescs : BlockDescs {

@@ -90,6 +90,35 @@ static_assert(ROWS >= 1 + 511 && CT_ROW >= 1 + 256, "node rows");
 static_assert(HUF_BLOCK_MAX < (1u << 24), "node counts share a word with an 8-bit parent / length");
 static_assert(sizeof(PlanCta) <= 76 * 1024, "three CTAs per SM");
 
+// Stream sizes of a block coded with the table whose cells (val | nbBits << 16) the lane holds for symbols i * 32 + lane, from
+// count(k, i) = that symbol's count in segment k (4X) or in the whole block (1X), header of hs bytes, capLeft bytes after it;
+// then the writer's capacity rule stream after stream (huf_compress.c:566-600, bitstream.h:190,246,258).  One warp.
+template <int NS, class Count>
+__device__ __forceinline__ bool size_streams(const u32 (&cell)[8], Count count, u64 hs, u64 capLeft, u32 (&bits)[NS], u32 (&offs)[NS],
+                                             u32 (&lens)[NS], u64& total)
+{
+    #pragma unroll
+    for (int k = 0; k < NS; k++) {
+        u32 acc = 0;
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) acc += count(k, i) * (cell[i] >> 16);
+        #pragma unroll
+        for (int dlt = 16; dlt; dlt >>= 1) acc += __shfl_xor_sync(FULL, acc, dlt);
+        bits[k] = acc;
+    }
+    u64 op = (NS == 4) ? 6 : 0; bool fits = true;
+    #pragma unroll
+    for (int t = 0; t < NS; t++) {
+        u64 const capk = capLeft - op;
+        u64 const tot = (u64)bits[t] + 1;                                    // + end mark
+        if (fits && (capk <= 8 || (tot >> 3) >= capk - 8)) fits = false;
+        offs[t] = (u32)(hs + op); lens[t] = (u32)((tot + 7) >> 3);
+        op += lens[t];
+    }
+    total = hs + op;
+    return fits;
+}
+
 // histogram of src[begin, end) into cnt[256] (shared memory), one warp
 __device__ __forceinline__ void warp_hist_range(u32* cnt, const u8* s, u32 begin, u32 end, unsigned lane)
 {
@@ -164,6 +193,9 @@ __device__ __forceinline__ void warp_hist4_pipelined(u32 (*count4)[256], const u
 // flag after them) and marks the block; phase 2 builds trees only for the other blocks; phase 3 compares the estimates, saves a
 // new table, and sizes the streams with the chosen table (hSize 0 for the old one).  S.live then also tells the three apart:
 // 1 = new table, 2 = new table unless the estimates prefer the old one, 3 = old table.
+// Geo = ChainDescs: the same phases with no flag, for every block of every chain; they write nothing but scratch.  Phase 1 records
+// the argument verdict or the histogram exit that would apply (and keeps the counts either way: prefer + valid skips the exits),
+// phase 2 builds every tree the exits leave, phase 3 plans the block with its new table.  huf_chain_kernel then decides.
 template <class Geo, int NS>
 __global__ void __launch_bounds__(32 * PLAN_WARPS, 3)
 huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8* __restrict__ src,
@@ -175,7 +207,11 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
     unsigned const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     u32 const b0 = blockIdx.x * GROUP;
     constexpr bool REP = std::is_same_v<Geo, RepeatDescs>;
-#define FSEB_FINAL(v) { if (lane == 0) { P.state = 1; enc_out(g, csizes, b) = (v); S.live[c] = 0; } continue; }   // next block of the loop
+    constexpr bool CHAIN = std::is_same_v<Geo, ChainDescs>;
+#define FSEB_FINAL(v) { if (lane == 0) {                                                                            \
+        if constexpr (CHAIN) { g.fact[b].kind = CF_ARGS; g.fact[b].exitValue = (v); }                                  \
+        else { P.state = 1; enc_out(g, csizes, b) = (v); }                                                             \
+        S.live[c] = 0; } continue; }                                                    // next block of the loop
 
     // ---- phase 1: one warp per block ----
     u32 (*const count4)[256] = reinterpret_cast<u32 (*)[256]>(&S.nd[257][0] + warp * 4 * 256);
@@ -222,7 +258,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         }
         #pragma unroll
         for (int dlt = 16; dlt; dlt >>= 1) { top = max(top, __shfl_xor_sync(FULL, top, dlt)); best = max(best, __shfl_xor_sync(FULL, best, dlt)); }
-        if (!oldNow) {
+        if (!CHAIN && !oldNow) {
             if (msvDecl < 255 && top > msvDecl) FSEB_FINAL(err(E_MSV_TOO_SMALL));                 // hist.c:128
             if (best == n) {                                                                      // huf_compress.c:673
                 if constexpr (!std::is_same_v<Geo, PackedDescs>) { if (lane == 0) enc_dst(g, cbuf, b)[0] = s[0]; }   // packed: placement writes it
@@ -230,12 +266,23 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
             }
             if (best <= (n >> 7) + 4) FSEB_FINAL(0);                                              // :674
         }
+        bool histExit = false;
+        if constexpr (CHAIN) {                                                                    // the exit that applies unless prefer + valid
+            bool const mst = msvReq != 0 && msvReq < 255 && top > msvReq;                        // msvDecl < 255 && top > msvDecl
+            histExit = mst || best == n || best <= (n >> 7) + 4;
+            if (lane == 0) {
+                ChainFact& F = g.fact[b];
+                F.kind = histExit ? CF_HIST : CF_TREE; F.msv = (u16)top;
+                F.exitValue = mst ? err(E_MSV_TOO_SMALL) : best == n ? 1 : 0;
+            }
+        }
         u32 const msv = top;
         // segment counts for phase 3, compacted to u16
         #pragma unroll
         for (u32 k = 0; k < 4; k++)
             #pragma unroll
             for (u32 i = 0; i < 8; i++) P.segCount[k][i * 32 + lane] = (u16)count4[k][i * 32 + lane];
+        if (CHAIN && histExit) { if (lane == 0) S.live[c] = 0; continue; }                     // its counts kept: prefer + valid skips the exit
         if constexpr (REP) {
             if (!oldNow && flag == 1) {                                                           // :679-683 HUF_validateCTable
                 const u32* const old = g.ctable[b];
@@ -335,6 +382,34 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         u32 const n = enc_len(g, b);
         u64 const cap = enc_cap(g, b);
         Plan& P = plans[b];
+        if constexpr (CHAIN) {                   // the plan with the new table (its cells also for saving it) and its verdict
+            u64 const hs = S.res[c];
+            ChainFact& F = g.fact[b];
+            if (lane == 0) F.hSize = hs;
+            if (is_err(hs) || hs + 12 >= n) continue;                                             // :714, or the old table
+            u32 const msv = S.msv[c];
+            u32 cell[8];
+            #pragma unroll
+            for (u32 i = 0; i < 8; i++) { cell[i] = (i * 32 + lane <= msv) ? S.nd[CT_ROW + i * 32 + lane][c] : 0u; P.ctable[i * 32 + lane] = cell[i]; }
+            u32 bits[NS], offs[NS], lens[NS];
+            u64 total;
+            bool const fits = size_streams<NS>(cell, [&](int k, u32 i) {
+                u32 const sy = i * 32 + lane;
+                return NS == 4 ? (u32)P.segCount[k][sy] : (u32)P.segCount[0][sy] + P.segCount[1][sy] + P.segCount[2][sy] + P.segCount[3][sy];
+            }, hs, cap - hs, bits, offs, lens, total);
+            bool const ok = !(NS == 4 && (cap - hs < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;   // :564-565, :625
+            u32 newBits = 0;
+            #pragma unroll
+            for (int k = 0; k < NS; k++) newBits += bits[k];
+            if (lane == 0) { F.newBits = newBits; F.newValue = ok ? total : 0; }
+            if (!ok) continue;
+            const u8* const hdr = reinterpret_cast<const u8*>(&S.nd[0][0] + c * HDR_STRIDE);
+            for (u32 i = lane; i < (u32)hs; i += 32) P.header[i] = hdr[i];
+            #pragma unroll
+            for (int k = 0; k < NS; k++) if (lane == (unsigned)k) { P.streamOff[k] = offs[k]; P.streamBytes[k] = lens[k]; }
+            if (lane == 0) { P.hSize = (u32)hs; P.total = (u32)total; }
+            continue;
+        }
         u64 hs = S.res[c];
         bool useOld = false;
         if constexpr (REP) useOld = S.live[c] == 3;
@@ -378,32 +453,12 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
                 for (u32 i = 0; i < 8; i++) cell[i] = g.ctable[b][i * 32 + lane] & 0xFFFFFFu;      // byte 3 is padding
             }
         }
-        u32 bits[NS];
-        #pragma unroll
-        for (int k = 0; k < NS; k++) {
-            u32 acc = 0;
-            #pragma unroll
-            for (u32 i = 0; i < 8; i++) {
-                u32 const sy = i * 32 + lane;                                // 1X: the four segment counts of a symbol add up to its block count
-                u32 const cnt = (NS == 4) ? (u32)P.segCount[k][sy]
-                                          : (u32)P.segCount[0][sy] + P.segCount[1][sy] + P.segCount[2][sy] + P.segCount[3][sy];
-                acc += cnt * (cell[i] >> 16);
-            }
-            #pragma unroll
-            for (int dlt = 16; dlt; dlt >>= 1) acc += __shfl_xor_sync(FULL, acc, dlt);
-            bits[k] = acc;
-        }
-        u64 op = (NS == 4) ? 6 : 0; bool fits = true;
-        u32 offs[NS], lens[NS];
-        #pragma unroll
-        for (int t = 0; t < NS; t++) {
-            u64 const capk = capLeft - op;
-            u64 const tot = (u64)bits[t] + 1;                                    // + end mark
-            if (fits && (capk <= 8 || (tot >> 3) >= capk - 8)) fits = false;
-            offs[t] = (u32)(hs + op); lens[t] = (u32)((tot + 7) >> 3);
-            op += lens[t];
-        }
-        u64 const total = hs + op;
+        u32 bits[NS], offs[NS], lens[NS];
+        u64 total;
+        bool const fits = size_streams<NS>(cell, [&](int k, u32 i) {
+            u32 const sy = i * 32 + lane;                                    // 1X: the four segment counts of a symbol add up to its block count
+            return (NS == 4) ? (u32)P.segCount[k][sy] : (u32)P.segCount[0][sy] + P.segCount[1][sy] + P.segCount[2][sy] + P.segCount[3][sy];
+        }, hs, capLeft, bits, offs, lens, total);
         if (!fits || total >= (u64)n - 1) FSEB_FINAL(0);
         #pragma unroll
         for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = cell[i];
@@ -413,6 +468,144 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         if (lane == 0) { P.hSize = (u32)hs; P.state = 0; P.total = (u32)total; enc_out(g, csizes, b) = total; }
     }
 #undef FSEB_FINAL
+}
+
+// ---------------------------------------------------------------------------------------------
+// Chains (ChainDescs): the decisions HUF_compress_internal takes with a stream's (table, flag) state (huf_compress.c:653-724), one
+// warp per chain walking its blocks in order, from the facts the plan kernel recorded.  The state lives in registers: lane l holds
+// the table's cells for symbols i * 32 + l, as the plan kernel's phase 3 does.  Nothing a decision reads from memory depends on
+// the state, so the next block's facts, counts and new cells are loaded while the current block is decided.
+// ---------------------------------------------------------------------------------------------
+constexpr int CHAIN_WARPS = 4;
+
+// Chain geometry: start[0] == 0, start[nChains] == nBlocks, never decreasing.  One CTA; *malformed gets the verdict.
+__global__ void __launch_bounds__(1024)
+huf_chain_check_kernel(const u64* __restrict__ start, u32 nChains, u32 nBlocks, u32* __restrict__ malformed)
+{
+    bool bad = threadIdx.x == 0 && (start[0] != 0 || start[nChains] != nBlocks);
+    for (u64 c = threadIdx.x; c < nChains; c += blockDim.x) bad |= start[c + 1] < start[c];
+    bad = __syncthreads_or(bad);
+    if (threadIdx.x == 0) *malformed = bad;
+}
+
+struct ChainBlock {                // what the decision for one block reads
+    ChainFact f;
+    u32 cnt[4][8];                 // segment counts of symbols i * 32 + lane
+    u32 cell[8];                   // the new table's cells (CF_TREE with hSize + 12 < srcSize)
+    u8* dst;
+    u64 cap;
+    u32 n;
+    int prefer;
+};
+__device__ __forceinline__ void chain_load(const ChainDescs& g, const Plan* plans, u32 b, ChainBlock& x, unsigned lane)
+{
+    x.f = g.fact[b];
+    const Plan& P = plans[b];      // read whatever the kind: a plan the block did not fill is never used
+    #pragma unroll
+    for (int k = 0; k < 4; k++)
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) x.cnt[k][i] = P.segCount[k][i * 32 + lane];
+    #pragma unroll
+    for (u32 i = 0; i < 8; i++) x.cell[i] = P.ctable[i * 32 + lane];
+    x.dst = enc_dst(g, nullptr, b); x.cap = enc_cap(g, b); x.n = enc_len(g, b); x.prefer = g.prefer[b];
+}
+
+template <int NS>
+__global__ void __launch_bounds__(32 * CHAIN_WARPS)
+huf_chain_kernel(ChainDescs g, Plan* __restrict__ plans, const u32* __restrict__ malformed)
+{
+    unsigned const lane = threadIdx.x & 31u;
+    if (*malformed) {              // every verdict srcSize_wrong, nothing else written and nothing emitted
+        for (u64 b = blockIdx.x * (u64)blockDim.x + threadIdx.x; b < g.nBlocks; b += (u64)gridDim.x * blockDim.x) {
+            g.result[b] = err(E_SRC_WRONG);
+            plans[b].state = 1;
+        }
+        return;
+    }
+    u64 const c = blockIdx.x * (u64)CHAIN_WARPS + (threadIdx.x >> 5);
+    if (c >= g.nChains) return;
+    u32 const b0 = (u32)g.start[c], b1 = (u32)g.start[c + 1];
+    if (b0 == b1) return;
+    u32 T[8];                      // the chain's table (byte 3, padding, cleared), flag and header
+    const u32* const t0 = g.ctable[c];
+    #pragma unroll
+    for (u32 i = 0; i < 8; i++) T[i] = t0[i * 32 + lane] & 0xFFFFFFu;
+    int F = g.repeat[c];
+    const u8* H = g.hdr[c];
+    u64 HS = g.hdrSize[c];
+    bool saved = false;
+    ChainBlock nx;
+    chain_load(g, plans, b0, nx, lane);
+    #pragma unroll 1
+    for (u32 b = b0; b < b1; b++) {
+        ChainBlock const x = nx;
+        if (b + 1 < b1) chain_load(g, plans, b + 1, nx, lane);
+        ChainFact const& f = x.f;
+        u32 const n = x.n;
+        u32 sum[8];                                                                               // block counts
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) sum[i] = x.cnt[0][i] + x.cnt[1][i] + x.cnt[2][i] + x.cnt[3][i];
+        auto const count = [&](int k, u32 i) { return NS == 4 ? x.cnt[k][i] : sum[i]; };
+        u64 r = 0;
+        bool useOld = false, emit = false;
+        if (f.kind == CF_ARGS) r = f.exitValue;                                                   // huf_compress.c:656-664
+        else if (x.prefer && F == 2) useOld = true;                                               // :665-669
+        else if (f.kind == CF_HIST) {                                                             // hist.c:128, :673-674
+            r = f.exitValue;
+            if (r == 1 && lane == 0) x.dst[0] = g.src[b][0];                                  // the RLE byte
+        } else {
+            if (F == 1) {                                                                         // :679-683 HUF_validateCTable
+                bool bad = false;
+                #pragma unroll
+                for (u32 i = 0; i < 8; i++) bad |= sum[i] && (T[i] >> 16) == 0;
+                if (__any_sync(FULL, bad)) F = 0;
+            }
+            if (x.prefer && F != 0) useOld = true;                                                // :685-689
+            else if (is_err(f.hSize)) r = f.hSize;
+            else {
+                if (F != 0) {                                                                     // :703-713 HUF_estimateCompressedSize, old and new
+                    u32 oldBits = 0;
+                    #pragma unroll
+                    for (u32 i = 0; i < 8; i++) oldBits += sum[i] * (T[i] >> 16);
+                    oldBits = __reduce_add_sync(FULL, oldBits);
+                    useOld = (oldBits >> 3) <= f.hSize + (f.newBits >> 3) || f.hSize + 12 >= n;
+                }
+                if (!useOld && f.hSize + 12 < n) {                                                // :716-719 the new table is saved, the flag set to none
+                    #pragma unroll
+                    for (u32 i = 0; i < 8; i++) T[i] = x.cell[i];
+                    saved = true; F = 0; r = f.newValue; emit = r != 0;
+                }
+            }
+        }
+        Plan& P = plans[b];
+        if (useOld) {                                                                             // HUF_compressCTable_internal with the old table
+            u32 bits[NS], offs[NS], lens[NS];
+            u64 total;
+            bool const fits = size_streams<NS>(T, count, 0, x.cap, bits, offs, lens, total);
+            bool const ok = !(NS == 4 && (x.cap < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;   // :564-565, :625
+            r = ok ? total : 0; emit = ok;
+            if (ok) {
+                #pragma unroll
+                for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = T[i];
+                #pragma unroll
+                for (int k = 0; k < NS; k++) if (lane == (unsigned)k) { P.streamOff[k] = offs[k]; P.streamBytes[k] = lens[k]; }
+                if (lane == 0) { P.hSize = 0; P.total = (u32)total; }
+            }
+        }
+        bool const coded = !is_err(r) && r >= 2;                                                  // 1X: a 1-byte stream is emitted, not coded
+        if (lane == 0) {
+            P.state = emit ? 0 : 1;
+            g.result[b] = r;
+            g.blkHdr[b] = coded && F != 0 ? H : nullptr;
+            g.blkHdrSize[b] = coded && F != 0 ? HS : 0;
+        }
+        if (coded && F == 0) { F = 1; H = x.dst; HS = r; }                                        // the block carries the new table: check it next
+    }
+    if (saved) {
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) g.ctable[c][i * 32 + lane] = T[i];
+    }
+    if (lane == 0) { g.repeat[c] = F; g.hdr[c] = H; g.hdrSize[c] = HS; }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -794,6 +987,8 @@ struct SubPacked { PackedDescs g; u8* cbuf; const u8* src; };
 SubPacked sub_batch(const PackedDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
 struct SubRepeat { RepeatDescs g; u8* cbuf; const u8* src; };
 SubRepeat sub_batch(const RepeatDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
+struct SubChain { ChainDescs g; u8* cbuf; const u8* src; };
+SubChain sub_batch(const ChainDescs& g, u8*, const u8*, u32, u32) { return { g, nullptr, nullptr }; }   // always the whole batch
 
 template <class Geo, int NS>
 cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, unsigned msv, unsigned tlog, cudaStream_t stream)
@@ -818,22 +1013,35 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     static SmemOptIn optin;
     e = optin.ensure(hufe::huf_plan_kernel<Geo, NS>, current_device(), (int)smem);
     if (e != cudaSuccess) return e;
-    u32 const step = (subBatch && subBatch < g.nBlocks) ? subBatch : g.nBlocks;
+    constexpr bool chain = std::is_same_v<Geo, ChainDescs>;        // every plan must exist before the chains' decisions: no sub-batches
+    u32 const step = (!chain && subBatch && subBatch < g.nBlocks) ? subBatch : g.nBlocks;
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
-    using EmitGeo = std::conditional_t<std::is_same_v<Geo, RepeatDescs>, BlockDescs, Geo>;   // the plan holds the chosen table
+    using EmitGeo = std::conditional_t<std::is_same_v<Geo, RepeatDescs> || chain, BlockDescs, Geo>;   // the plan holds the chosen table
     u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch
     if constexpr (packed) {
         tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * pack::tiles_of(step), &e);
         if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
     }
+    Geo gx = g;
+    u32* malformed = nullptr;                                       // chains: the geometry verdict, then one fact per block
+    if constexpr (chain) {
+        malformed = (u32*)stream_scratch(9, stream, sizeof(u32), &e);
+        if (e == cudaSuccess) gx.fact = (ChainFact*)stream_scratch(10, stream, sizeof(ChainFact) * (size_t)g.nBlocks, &e);
+        if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
+    }
     for (u32 b0 = 0; b0 < g.nBlocks; b0 += step) {
-        auto const sb = sub_batch(g, (u8*)cbuf, (const u8*)src, b0, (g.nBlocks - b0 < step) ? g.nBlocks - b0 : step);
+        auto const sb = sub_batch(gx, (u8*)cbuf, (const u8*)src, b0, (g.nBlocks - b0 < step) ? g.nBlocks - b0 : step);
         u64* const cs = csizes ? csizes + b0 : nullptr;
         unsigned const grid = (sb.g.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
         hufe::huf_plan_kernel<Geo, NS><<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(sb.g, sb.cbuf, cs, sb.src, msv, tlog, plans + b0);
         if constexpr (packed) {                                     // offsets, capacity verdicts, RLE bytes, raw copies; then emit
             pack::launch_pack<hufe::HufPlace>(sb.g, tileSum, b0 ? sb.g.offset : nullptr, sb.g.offset + sb.g.nBlocks, plans + b0, stream);
             hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g);
+        }
+        if constexpr (chain) {
+            hufe::huf_chain_check_kernel<<<1, 1024, 0, stream>>>(sb.g.start, sb.g.nChains, sb.g.nBlocks, malformed);
+            u64 const cgrid = ((u64)sb.g.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
+            hufe::huf_chain_kernel<NS><<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(sb.g, plans, malformed);
         }
         hufe::huf_emit_kernel<EmitGeo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);
     }
@@ -862,6 +1070,13 @@ cudaError_t launch_huf_encode_repeat(const RepeatDescs& g, int nStreams, unsigne
 {
     return nStreams == 1 ? huf_encode<RepeatDescs, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
                          : huf_encode<RepeatDescs, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+}
+
+// chains of table reuse (ChainDescs): plan, the chains' decisions, emit -- HUF_compress{4X,1X}_repeat block after block per chain
+cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return nStreams == 1 ? huf_encode<ChainDescs, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
+                         : huf_encode<ChainDescs, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
 }
 
 // packed output (PackedDescs): the same kernels with the scan and placement between plan and emit

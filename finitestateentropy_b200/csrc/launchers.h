@@ -21,6 +21,7 @@ cudaError_t launch_huf_encode_blocks(const BlockDescs& g, int nStreams, unsigned
 cudaError_t launch_huf_encode_packed(const PackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_decode_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_huf_encode_repeat(const RepeatDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
+cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_fse_encode_blocks(const BlockDescs& g, bool wide, unsigned msv, unsigned tlog, cudaStream_t s);

@@ -148,6 +148,46 @@ size_t FSEB200_HUF_compress1X_repeat_blocks(size_t nBlocks, void* const* dDsts, 
                                             const void* const* dSrcs, const size_t* dSrcSizes,
                                             unsigned* const* dCTables, int* dRepeats, const int* dPreferRepeat,
                                             unsigned maxSymbolValue, unsigned tableLog, void* stream);
+/* Tier 1, chains of table reuse (Huff0, 4X and 1X): whole runs of one stream's blocks in one call, the stream's state carried
+ * from block to block on the device -- one long stream of literal blocks, as a zstd-style compressor makes from one file, needs
+ * no call per block.  All arrays and buffers are in device memory, the call is asynchronous on `stream`, and the host never reads
+ * the arrays.  Chain c is blocks [dChainStarts[c], dChainStarts[c+1]) in order (dChainStarts has nChains + 1 entries); block
+ * descriptors (dDsts .. dSrcSizes), dPreferRepeat, dHeaders and dHeaderSizes are per block; dCTables[c], dRepeats[c],
+ * dChainHeaders[c] and dChainHeaderSizes[c] are per chain, in-out: the stream's state when the chain starts, and when it ends.
+ * Each chain gives exactly what this loop gives, from T = dCTables[c], F = dRepeats[c], H = (dChainHeaders[c], dChainHeaderSizes[c]):
+ *     for (b = dChainStarts[c]; b < dChainStarts[c+1]; b++) {
+ *         r = HUF_compress4X_repeat(dDsts[b], dDstCapacities[b], dSrcs[b], dSrcSizes[b], maxSymbolValue, tableLog,
+ *                                   wksp, sizeof wksp, T, &F, dPreferRepeat[b], 0);          (1X: HUF_compress1X_repeat)
+ *         dCSizes[b] = r;
+ *         if (!isError(r) && r >= 2 && F != 0) { dHeaders[b] = H.ptr; dHeaderSizes[b] = H.size; }    coded with the old table
+ *         else                                  { dHeaders[b] = NULL;  dHeaderSizes[b] = 0; }
+ *         if (!isError(r) && r >= 2 && F == 0) { F = 1; H = (dDsts[b], r); }                        carries a new table: check it next
+ *     }
+ * and then writes T (only if a block saved a table), F and H back to the chain's entries; an empty chain writes nothing.  Each step
+ * has the single-block semantics of FSEB200_HUF_compress{4X,1X}_repeat_blocks (a zeroed workspace, a table written only where the
+ * reference saves one, byte 3 of stored cells 0, flag values taken literally, a capacity above 2^32 acting as 0xFFFFFF00).
+ * dHeaders / dHeaderSizes are exactly the header arrays FSEB200_HUF_decompress{4X,1X}_repeat_blocks take: the blocks with
+ * dCSizes[b] >= 2 decode in one such call; the caller handles those stored raw (0) or as RLE (1) itself.  A chain that enters with
+ * F != 0 needs dChainHeaderSizes[c] = the size of that table's header source; its old-table blocks inherit it as given.
+ * Returns 0 for nBlocks == 0 (nothing launched); srcSize_wrong, the device untouched, for nBlocks or nChains above 0xFFFFFFFF or a
+ * NULL array while nBlocks > 0; generic if a launch fails.  Malformed chain geometry (dChainStarts[0] != 0,
+ * dChainStarts[nChains] != nBlocks, or a decrease) is found on the device: then every dCSizes[b] is srcSize_wrong and nothing
+ * else is written -- no destination, table, flag or header.
+ * Contract: that of FSEB200_HUF_compress{4X,1X}_repeat_blocks, and no per-chain state array overlaps another array, and no table
+ * belongs to two chains.  The decisions of a chain run one block after another on one warp: a single chain of many blocks takes
+ * time in proportion to its length (DESIGN.md 4.2). */
+size_t FSEB200_HUF_compress4X_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                            void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                            const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                            unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                            const void** dHeaders, size_t* dHeaderSizes,
+                                            unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_compress1X_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                            void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                            const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                            unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                            const void** dHeaders, size_t* dHeaderSizes,
+                                            unsigned maxSymbolValue, unsigned tableLog, void* stream);
 size_t FSEB200_HUF_decompress4X_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                               const void* const* dCSrcs, const size_t* dCSrcSizes,
                                               const void* const* dHeaders, const size_t* dHeaderSizes, void* stream);
