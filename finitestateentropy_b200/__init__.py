@@ -70,6 +70,10 @@ def _declare(L):
         sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     for name in ("FSEB200_HUF_compress4X_repeat_chains", "FSEB200_HUF_compress1X_repeat_chains"):
         sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
+    for name in ("FSEB200_HUF_compress4X_repeat_chains_packed", "FSEB200_HUF_compress1X_repeat_chains_packed"):
+        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
+    for name in ("FSEB200_HUF_decompress4X_repeat_packed", "FSEB200_HUF_decompress1X_repeat_packed"):
+        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     for name in ("FSEB200_HUF_decompress4X_repeat_blocks", "FSEB200_HUF_decompress1X_repeat_blocks"):
         sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     for name in ("FSEB200_HUF_compress_packed", "FSEB200_HUF_compress1X_packed"):
@@ -110,6 +114,8 @@ from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch
                     huf_compress_repeat_blocks, huf_compress1x_repeat_blocks,
                     huf_decompress_repeat_blocks, huf_decompress1x_repeat_blocks,
                     huf_compress_repeat_chains, huf_compress1x_repeat_chains,
+                    huf_compress_repeat_chains_packed, huf_compress1x_repeat_chains_packed,
+                    huf_decompress_repeat_packed, huf_decompress1x_repeat_packed,
                     huf_compress_packed, huf_compress1x_packed, packed_pointers,
                     fse_compress_blocks, fse_decompress_blocks, fseu16_compress_blocks, fseu16_decompress_blocks,
                     fse_compress_packed, fseu16_compress_packed, fse_decompress_packed, fseu16_decompress_packed,

@@ -229,6 +229,95 @@ def _repeat_chains(fn_name, chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_cap
     return csizes, hdr_ptrs, hdr_sizes
 
 
+def huf_compress_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
+                                      out=None, offsets=None, csizes=None, kinds=None, max_symbol_value=255, table_log=12):
+    """huf_compress_repeat_chains at capacities HUF_compressBound with every block stored back to back in `out` (capacity
+    out.numel()), on the current stream.  The chain and state arguments are huf_compress_repeat_chains's; a chain header that
+    comes back points into `out`.  Returns (out, offsets, csizes, kinds): offsets (int64, n + 1 entries) the prefix sum of the
+    stored lengths, csizes the loop's value per block (dstSize_tooSmall for a block that does not fit `out`), kinds (uint8) 0 raw,
+    1 RLE, 2 own tree header, 3 the previous table's header, 4 nothing stored.  With out=None, `out` is allocated at
+    sum(src_sizes) + 32 bytes, always enough: reading that sum costs one host synchronisation."""
+    return _repeat_chains_packed("FSEB200_HUF_compress4X_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer, ctables,
+                                 repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds, max_symbol_value, table_log)
+
+
+def huf_compress1x_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
+                                        out=None, offsets=None, csizes=None, kinds=None, max_symbol_value=255, table_log=12):
+    """huf_compress_repeat_chains_packed in the single-stream format (HUF_compress1X_repeat per block)"""
+    return _repeat_chains_packed("FSEB200_HUF_compress1X_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer, ctables,
+                                 repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds, max_symbol_value, table_log)
+
+
+def _chain_args(chain_starts, dev, per_chain):
+    _check(chain_starts, torch.int64)
+    n_chains = chain_starts.numel() - 1
+    assert n_chains >= 0 and chain_starts.device == dev, (chain_starts.numel(), chain_starts.device)
+    for a, dtype in per_chain:
+        _check(a, dtype)
+        assert a.numel() == n_chains and a.device == dev, (a.numel(), n_chains, a.device)
+    return n_chains
+
+
+def _repeat_chains_packed(fn_name, chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
+                          out, offsets, csizes, kinds, msv, tlog):
+    from . import lib
+    n = _blocks_args(src_ptrs, src_sizes)
+    dev = src_ptrs.device
+    _check(prefer, torch.int32)
+    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
+    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
+                                               (chain_hdr_sizes, torch.int64)))
+    if out is None:
+        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
+    if offsets is None:
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    if kinds is None:
+        kinds = torch.empty(n, dtype=torch.uint8, device=dev)
+    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64); _check(kinds, torch.uint8)
+    assert offsets.numel() == n + 1 and csizes.numel() == n and kinds.numel() == n and out.device == dev, (offsets.numel(), n)
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, out.data_ptr(), out.numel(), offsets.data_ptr(),
+                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(),
+                                ctables.data_ptr(), repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(),
+                                msv, tlog, _stream_ptr())
+    _ret(r, fn_name)
+    return out, offsets, csizes, kinds
+
+
+def huf_decompress_repeat_packed(chain_starts, packed, offsets, kinds, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes,
+                                 results=None):
+    """every block of a packed chain buffer (huf_compress_repeat_chains_packed's out, offsets and kinds) into dst_ptrs[b],
+    regenerating dst_sizes[b] bytes, on the current stream: a kind-3 block takes the header of the last kind-2 block before it
+    in its chain, or chain_hdr_ptrs[c] / chain_hdr_sizes[c] (int64, the headers the chains entered the compress call with).
+    Returns results (int64; the regenerated size or an error code per block)."""
+    return _repeat_unpack("FSEB200_HUF_decompress4X_repeat_packed", chain_starts, packed, offsets, kinds, chain_hdr_ptrs,
+                          chain_hdr_sizes, dst_ptrs, dst_sizes, results)
+
+
+def huf_decompress1x_repeat_packed(chain_starts, packed, offsets, kinds, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes,
+                                   results=None):
+    """huf_decompress_repeat_packed in the single-stream format (huf_compress1x_repeat_chains_packed's buffers)"""
+    return _repeat_unpack("FSEB200_HUF_decompress1X_repeat_packed", chain_starts, packed, offsets, kinds, chain_hdr_ptrs,
+                          chain_hdr_sizes, dst_ptrs, dst_sizes, results)
+
+
+def _repeat_unpack(fn_name, chain_starts, packed, offsets, kinds, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes, results):
+    from . import lib
+    n = _blocks_args(dst_ptrs, dst_sizes)
+    dev = dst_ptrs.device
+    n_chains = _chain_args(chain_starts, dev, ((chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64)))
+    if results is None:
+        results = torch.empty(n, dtype=torch.int64, device=dev)
+    _check(packed, torch.uint8); _check(offsets, torch.int64); _check(kinds, torch.uint8); _check(results, torch.int64)
+    assert offsets.numel() == n + 1 and kinds.numel() == n and results.numel() == n and packed.device == dev, (offsets.numel(), n)
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(),
+                                packed.data_ptr(), offsets.data_ptr(), kinds.data_ptr(), chain_hdr_ptrs.data_ptr(),
+                                chain_hdr_sizes.data_ptr(), _stream_ptr())
+    _ret(r, fn_name)
+    return results
+
+
 def huf_decompress_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results=None):
     """Every block b of csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of dst_sizes[b] bytes, on the current stream: with
     hdr_sizes[b] == 0, HUF_decompress4X1_DCtx (the block's own tree header); otherwise HUF_readDTableX1 on hdr_ptrs[b] /

@@ -274,6 +274,76 @@ FSEB_API size_t FSEB200_HUF_compress1X_repeat_chains(size_t nChains, const size_
     return huf_repeat_chains(nChains, dChainStarts, nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, dPreferRepeat, dCTables,
                              dRepeats, dChainHeaders, dChainHeaderSizes, dHeaders, dHeaderSizes, 1, maxSymbolValue, tableLog, stream);
 }
+// Packed chains: the chain calls with every block stored back to back in one buffer and a kind byte per block
+// (common.cuh ChainPackedDescs), and the decoders of that buffer.
+namespace {
+size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut, size_t outCapacity,
+                                size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs,
+                                const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats,
+                                const void** dChainHeaders, size_t* dChainHeaderSizes, int nStreams, unsigned msv, unsigned tlog,
+                                void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dOut || !dOffsets || !dCSizes || !dKinds || !dSrcs ||
+        !dSrcSizes || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes) return (size_t)err(E_SRC_WRONG);
+    ChainPackedDescs g;
+    g.dst = nullptr; g.dstCap = nullptr; g.result = (u64*)dCSizes; g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes;
+    g.nBlocks = (u32)nBlocks;
+    g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
+    g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.hdr = (const u8**)dChainHeaders; g.hdrSize = (u64*)dChainHeaderSizes;
+    g.blkHdr = nullptr; g.blkHdrSize = nullptr; g.fact = nullptr;
+    g.pk.out = (u8*)dOut; g.pk.outCap = outCapacity; g.pk.offset = (u64*)dOffsets; g.pk.result = g.result;
+    g.pk.src = g.src; g.pk.srcSize = g.srcSize; g.pk.nBlocks = g.nBlocks;
+    g.kind = dKinds; g.end = nullptr; g.malformed = nullptr;
+    return ok_or_generic(launch_huf_encode_chains_packed(g, nStreams, msv, tlog, (cudaStream_t)stream));
+}
+size_t huf_repeat_unpack(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstSizes,
+                         size_t* dResults, const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
+                         const void* const* dChainHeaders, const size_t* dChainHeaderSizes, int nStreams, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dDsts || !dDstSizes || !dResults || !dIn ||
+        !dOffsets || !dKinds || !dChainHeaders || !dChainHeaderSizes) return (size_t)err(E_SRC_WRONG);
+    return ok_or_generic(launch_huf_decompress_repeat_packed((const u64*)dChainStarts, (u32)nChains, (u8* const*)dDsts,
+                                                             (const u64*)dDstSizes, (u64*)dResults, (const u8*)dIn,
+                                                             (const u64*)dOffsets, dKinds, (const u8* const*)dChainHeaders,
+                                                             (const u64*)dChainHeaderSizes, (u32)nBlocks, nStreams, (cudaStream_t)stream));
+}
+}
+FSEB_API size_t FSEB200_HUF_compress4X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
+                                                            size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                            const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                            unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders,
+                                                            size_t* dChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 4, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_HUF_compress1X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
+                                                            size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                            const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                            unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders,
+                                                            size_t* dChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 1, maxSymbolValue, tableLog, stream);
+}
+FSEB_API size_t FSEB200_HUF_decompress4X_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
+                                                       const size_t* dDstSizes, size_t* dResults, const void* dIn, const size_t* dOffsets,
+                                                       const unsigned char* dKinds, const void* const* dChainHeaders,
+                                                       const size_t* dChainHeaderSizes, void* stream)
+{
+    return huf_repeat_unpack(nChains, dChainStarts, nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, dKinds, dChainHeaders,
+                             dChainHeaderSizes, 4, stream);
+}
+FSEB_API size_t FSEB200_HUF_decompress1X_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
+                                                       const size_t* dDstSizes, size_t* dResults, const void* dIn, const size_t* dOffsets,
+                                                       const unsigned char* dKinds, const void* const* dChainHeaders,
+                                                       const size_t* dChainHeaderSizes, void* stream)
+{
+    return huf_repeat_unpack(nChains, dChainStarts, nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, dKinds, dChainHeaders,
+                             dChainHeaderSizes, 1, stream);
+}
 FSEB_API size_t FSEB200_HUF_decompress4X_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                                        const void* const* dCSrcs, const size_t* dCSrcSizes, const void* const* dHeaders,
                                                        const size_t* dHeaderSizes, void* stream)

@@ -178,6 +178,28 @@ __device__ __forceinline__ u8* enc_dst(const PackedDescs& g, u8*, u32 b) { retur
 __device__ __forceinline__ u64 enc_cap(const PackedDescs& g, u32 b) { u64 const n = enc_len(g, b); return 129 + n + (n >> 8) + 8; }   // HUF_compressBound
 __device__ __forceinline__ u64& enc_out(const PackedDescs& g, u64*, u32 b) { return g.result[b]; }
 
+// -------------------------------------------------------------------------------------------
+// Packed chains of table reuse (Huff0 compress only): the chains of ChainDescs with every block's capacity HUF_compressBound(srcSize)
+// and its bytes stored as PackedDescs stores them (`pk` is that view of the same call: out, outCap, offset, result, src, srcSize),
+// plus one kind byte per block (include/fse_b200.h).  dst, dstCap, blkHdr and blkHdrSize are unused: a block's place is fixed
+// only by the scan after the decisions, so huf_chain_kernel records per chain what the state write-back needs in end[c] instead
+// of writing the state, and chainState writes it once the total is known to fit.
+// -------------------------------------------------------------------------------------------
+constexpr u32 CHAIN_NONE = 0xFFFFFFFFu;
+struct ChainEnd {
+    u32 lastNew;                   // the chain's last block coded with a new table (kind 2), or CHAIN_NONE
+    u32 lastSaved;                 // the chain's last block that saved a table, or CHAIN_NONE
+    int flag;                      // the flag after the chain's last block
+};
+struct ChainPackedDescs : ChainDescs {
+    PackedDescs pk;
+    u8* kind;                      // per block, out
+    ChainEnd* end;                 // per chain, scratch
+    const u32* malformed;          // scratch: the chain geometry's verdict
+};
+__device__ __forceinline__ u64 enc_cap(const ChainPackedDescs& g, u32 b) { u64 const n = enc_len(g, b); return 129 + n + (n >> 8) + 8; }   // HUF_compressBound
+__device__ __forceinline__ u8* enc_dst(const ChainPackedDescs& g, u8*, u32 b) { return g.pk.out + g.pk.offset[b]; }   // after placement
+
 // decoder: compressed source, its size, the output, the regenerated size, the result; `orig` (stored blocks) is uniform-only
 __device__ __forceinline__ const u8* dec_src(const BatchGeom& g, const u8* cbuf, u32 b) { return cbuf + (u64)b * g.slot; }
 __device__ __forceinline__ u64 dec_csize(const BatchGeom&, const u64* csizes, u32 b) { return csizes[b]; }

@@ -196,6 +196,7 @@ __device__ __forceinline__ void warp_hist4_pipelined(u32 (*count4)[256], const u
 // Geo = ChainDescs: the same phases with no flag, for every block of every chain; they write nothing but scratch.  Phase 1 records
 // the argument verdict or the histogram exit that would apply (and keeps the counts either way: prefer + valid skips the exits),
 // phase 2 builds every tree the exits leave, phase 3 plans the block with its new table.  huf_chain_kernel then decides.
+// Geo = ChainPackedDescs: the same, at capacities HUF_compressBound(srcSize).
 template <class Geo, int NS>
 __global__ void __launch_bounds__(32 * PLAN_WARPS, 3)
 huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8* __restrict__ src,
@@ -207,7 +208,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
     unsigned const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     u32 const b0 = blockIdx.x * GROUP;
     constexpr bool REP = std::is_same_v<Geo, RepeatDescs>;
-    constexpr bool CHAIN = std::is_same_v<Geo, ChainDescs>;
+    constexpr bool CHAIN = std::is_base_of_v<ChainDescs, Geo>;                              // ChainDescs or ChainPackedDescs
 #define FSEB_FINAL(v) { if (lane == 0) {                                                                            \
         if constexpr (CHAIN) { g.fact[b].kind = CF_ARGS; g.fact[b].exitValue = (v); }                                  \
         else { P.state = 1; enc_out(g, csizes, b) = (v); }                                                             \
@@ -497,7 +498,8 @@ struct ChainBlock {                // what the decision for one block reads
     u32 n;
     int prefer;
 };
-__device__ __forceinline__ void chain_load(const ChainDescs& g, const Plan* plans, u32 b, ChainBlock& x, unsigned lane)
+template <class Geo>
+__device__ __forceinline__ void chain_load(const Geo& g, const Plan* plans, u32 b, ChainBlock& x, unsigned lane)
 {
     x.f = g.fact[b];
     const Plan& P = plans[b];      // read whatever the kind: a plan the block did not fill is never used
@@ -507,13 +509,18 @@ __device__ __forceinline__ void chain_load(const ChainDescs& g, const Plan* plan
         for (u32 i = 0; i < 8; i++) x.cnt[k][i] = P.segCount[k][i * 32 + lane];
     #pragma unroll
     for (u32 i = 0; i < 8; i++) x.cell[i] = P.ctable[i * 32 + lane];
-    x.dst = enc_dst(g, nullptr, b); x.cap = enc_cap(g, b); x.n = enc_len(g, b); x.prefer = g.prefer[b];
+    if constexpr (std::is_same_v<Geo, ChainDescs>) x.dst = enc_dst(g, nullptr, b);
+    else x.dst = nullptr;                                                                   // packed: no place yet, and none needed
+    x.cap = enc_cap(g, b); x.n = enc_len(g, b); x.prefer = g.prefer[b];
 }
 
-template <int NS>
+// Geo = ChainDescs: the state goes back to the chain's entries, the RLE byte to the block, its header to blkHdr / blkHdrSize.
+// Geo = ChainPackedDescs: none of these (the placement writes the RLE byte and the kinds); end[c] records what chainState needs.
+template <int NS, class Geo>
 __global__ void __launch_bounds__(32 * CHAIN_WARPS)
-huf_chain_kernel(ChainDescs g, Plan* __restrict__ plans, const u32* __restrict__ malformed)
+huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malformed)
 {
+    constexpr bool PACKED = std::is_same_v<Geo, ChainPackedDescs>;
     unsigned const lane = threadIdx.x & 31u;
     if (*malformed) {              // every verdict srcSize_wrong, nothing else written and nothing emitted
         for (u64 b = blockIdx.x * (u64)blockDim.x + threadIdx.x; b < g.nBlocks; b += (u64)gridDim.x * blockDim.x) {
@@ -534,6 +541,7 @@ huf_chain_kernel(ChainDescs g, Plan* __restrict__ plans, const u32* __restrict__
     const u8* H = g.hdr[c];
     u64 HS = g.hdrSize[c];
     bool saved = false;
+    u32 lastNew = CHAIN_NONE, lastSaved = CHAIN_NONE;                                             // packed only
     ChainBlock nx;
     chain_load(g, plans, b0, nx, lane);
     #pragma unroll 1
@@ -552,7 +560,7 @@ huf_chain_kernel(ChainDescs g, Plan* __restrict__ plans, const u32* __restrict__
         else if (x.prefer && F == 2) useOld = true;                                               // :665-669
         else if (f.kind == CF_HIST) {                                                             // hist.c:128, :673-674
             r = f.exitValue;
-            if (r == 1 && lane == 0) x.dst[0] = g.src[b][0];                                  // the RLE byte
+            if constexpr (!PACKED) { if (r == 1 && lane == 0) x.dst[0] = g.src[b][0]; }       // the RLE byte (packed: the placement's)
         } else {
             if (F == 1) {                                                                         // :679-683 HUF_validateCTable
                 bool bad = false;
@@ -574,6 +582,7 @@ huf_chain_kernel(ChainDescs g, Plan* __restrict__ plans, const u32* __restrict__
                     #pragma unroll
                     for (u32 i = 0; i < 8; i++) T[i] = x.cell[i];
                     saved = true; F = 0; r = f.newValue; emit = r != 0;
+                    if constexpr (PACKED) lastSaved = b;
                 }
             }
         }
@@ -596,10 +605,17 @@ huf_chain_kernel(ChainDescs g, Plan* __restrict__ plans, const u32* __restrict__
         if (lane == 0) {
             P.state = emit ? 0 : 1;
             g.result[b] = r;
-            g.blkHdr[b] = coded && F != 0 ? H : nullptr;
-            g.blkHdrSize[b] = coded && F != 0 ? HS : 0;
+            if constexpr (!PACKED) {
+                g.blkHdr[b] = coded && F != 0 ? H : nullptr;
+                g.blkHdrSize[b] = coded && F != 0 ? HS : 0;
+            }
         }
+        if constexpr (PACKED) { if (coded && F == 0) lastNew = b; }
         if (coded && F == 0) { F = 1; H = x.dst; HS = r; }                                        // the block carries the new table: check it next
+    }
+    if constexpr (PACKED) {
+        if (lane == 0) g.end[c] = ChainEnd{ lastNew, lastSaved, F };
+        return;
     }
     if (saved) {
         #pragma unroll
@@ -904,6 +920,54 @@ huf_pack_raw_kernel(PackedDescs g)
 }
 
 // ---------------------------------------------------------------------------------------------
+// Packed chains (ChainPackedDescs): the placement runs after huf_chain_kernel, whose decisions fix every value.  It is HufPlace's
+// (offsets, capacity verdict, RLE byte) plus the kind: 0 raw, 1 RLE, 2 coded with its own tree header, 3 coded with the stream's
+// previous table (the chain kernel left hSize 0 in its plan), 4 nothing stored.  Malformed geometry writes only the kinds (4, as
+// every value is srcSize_wrong).  The raw copies and the emit then run as for PackedDescs, and chainState writes the streams' state.
+// ---------------------------------------------------------------------------------------------
+struct HufChainPlace {
+    typedef ChainPackedDescs Geo;
+    typedef Plan* Aux;
+    static __device__ __forceinline__ u64 value(const ChainPackedDescs& g, u64 b) { return g.result[b]; }
+    static __device__ __forceinline__ u64 len(const ChainPackedDescs& g, u64 b, u64 v) { return packed_len(v, g.srcSize[b]); }
+    static __device__ __forceinline__ void place(const ChainPackedDescs& g, Plan* plans, u64 b, u64 v, u64 off, u64 len)
+    {
+        u8 kind = is_err(v) ? 4 : v == 0 ? 0 : v == 1 ? 1 : plans[b].hSize ? 2 : 3;
+        if (!*g.malformed) {
+            g.pk.offset[b] = off;
+            if (!is_err(v) && off + len > g.pk.outCap) { g.result[b] = err(E_DST_TOO_SMALL); plans[b].state = 1; kind = 4; }
+            else if (v == 1) g.pk.out[off] = g.src[b][0];                   // a 1X block coded into one byte: emit overwrites it
+        }
+        g.kind[b] = kind;
+    }
+};
+
+// The streams' state, one warp per chain, once every block's place is known: nothing unless the geometry is sound and the total
+// (*total, which also becomes offset[nBlocks]) fits.  Then the chain's flag, the table of its last block that saved one (that
+// block's plan holds it, whatever its value), and the header of its last kind-2 block, at its place in out.
+__global__ void __launch_bounds__(32 * CHAIN_WARPS)
+huf_chain_state_kernel(ChainPackedDescs g, const Plan* __restrict__ plans, const u64* __restrict__ total)
+{
+    if (*g.malformed) return;
+    u64 const tot = *total;
+    if (blockIdx.x == 0 && threadIdx.x == 0) g.pk.offset[g.nBlocks] = tot;
+    if (tot > g.pk.outCap) return;
+    unsigned const lane = threadIdx.x & 31u;
+    u64 const c = blockIdx.x * (u64)CHAIN_WARPS + (threadIdx.x >> 5);
+    if (c >= g.nChains || g.start[c] == g.start[c + 1]) return;
+    ChainEnd const e = g.end[c];
+    if (e.lastSaved != CHAIN_NONE) {
+        const u32* const t = plans[e.lastSaved].ctable;
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) g.ctable[c][i * 32 + lane] = t[i * 32 + lane];
+    }
+    if (lane == 0) {
+        g.repeat[c] = e.flag;
+        if (e.lastNew != CHAIN_NONE) { g.hdr[c] = g.pk.out + g.pk.offset[e.lastNew]; g.hdrSize[c] = g.result[e.lastNew]; }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Table reuse (SURVEY.md 8f-3): every block of the batch coded with ONE caller-supplied HUF_CElt table, i.e. per block
 // HUF_compress4X_usingCTable (lib/huf_compress.c:552-610).  No histogram, no tree, no header: the plan kernel disappears and
 // this warp-per-block pass only sums the code lengths of each 4X segment (stream sizes, the writer's capacity rule).
@@ -989,6 +1053,11 @@ struct SubRepeat { RepeatDescs g; u8* cbuf; const u8* src; };
 SubRepeat sub_batch(const RepeatDescs& g, u8*, const u8*, u32 b0, u32 n) { return { slice(g, b0, n), nullptr, nullptr }; }
 struct SubChain { ChainDescs g; u8* cbuf; const u8* src; };
 SubChain sub_batch(const ChainDescs& g, u8*, const u8*, u32, u32) { return { g, nullptr, nullptr }; }   // always the whole batch
+struct SubChainPacked { ChainPackedDescs g; u8* cbuf; const u8* src; };
+SubChainPacked sub_batch(const ChainPackedDescs& g, u8*, const u8*, u32, u32) { return { g, nullptr, nullptr }; }
+// the emit kernel's geometry argument: packed chains are emitted as the packed blocks they are, everything else as itself
+template <class Geo> const Geo& emit_view(const Geo& g) { return g; }
+const PackedDescs& emit_view(const ChainPackedDescs& g) { return g.pk; }
 
 template <class Geo, int NS>
 cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, unsigned msv, unsigned tlog, cudaStream_t stream)
@@ -1013,13 +1082,15 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     static SmemOptIn optin;
     e = optin.ensure(hufe::huf_plan_kernel<Geo, NS>, current_device(), (int)smem);
     if (e != cudaSuccess) return e;
-    constexpr bool chain = std::is_same_v<Geo, ChainDescs>;        // every plan must exist before the chains' decisions: no sub-batches
+    constexpr bool chain = std::is_base_of_v<ChainDescs, Geo>;     // every plan must exist before the chains' decisions: no sub-batches
+    constexpr bool chainPacked = std::is_same_v<Geo, ChainPackedDescs>;
     u32 const step = (!chain && subBatch && subBatch < g.nBlocks) ? subBatch : g.nBlocks;
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
-    using EmitGeo = std::conditional_t<std::is_same_v<Geo, RepeatDescs> || chain, BlockDescs, Geo>;   // the plan holds the chosen table
-    u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch
-    if constexpr (packed) {
-        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * pack::tiles_of(step), &e);
+    using EmitGeo = std::conditional_t<chainPacked, PackedDescs,    // the plan holds the chosen table
+                                       std::conditional_t<std::is_same_v<Geo, RepeatDescs> || chain, BlockDescs, Geo>>;
+    u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch (packed chains: + the total)
+    if constexpr (packed || chainPacked) {
+        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * (pack::tiles_of(step) + chainPacked), &e);
         if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
     }
     Geo gx = g;
@@ -1027,6 +1098,10 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     if constexpr (chain) {
         malformed = (u32*)stream_scratch(9, stream, sizeof(u32), &e);
         if (e == cudaSuccess) gx.fact = (ChainFact*)stream_scratch(10, stream, sizeof(ChainFact) * (size_t)g.nBlocks, &e);
+        if constexpr (chainPacked) {                                // and one end record per chain
+            gx.malformed = malformed;
+            if (e == cudaSuccess) gx.end = (ChainEnd*)stream_scratch(11, stream, sizeof(ChainEnd) * ((size_t)g.nChains + 1), &e);
+        }
         if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
     }
     for (u32 b0 = 0; b0 < g.nBlocks; b0 += step) {
@@ -1041,9 +1116,18 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
         if constexpr (chain) {
             hufe::huf_chain_check_kernel<<<1, 1024, 0, stream>>>(sb.g.start, sb.g.nChains, sb.g.nBlocks, malformed);
             u64 const cgrid = ((u64)sb.g.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
-            hufe::huf_chain_kernel<NS><<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(sb.g, plans, malformed);
+            hufe::huf_chain_kernel<NS, Geo><<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(sb.g, plans, malformed);
         }
-        hufe::huf_emit_kernel<EmitGeo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(sb.g, sb.cbuf, sb.src, plans + b0, nullptr);
+        if constexpr (chainPacked) {                                // offsets, kinds, capacity verdicts, RLE bytes, raw copies; then emit
+            pack::launch_pack<hufe::HufChainPlace>(sb.g, tileSum, nullptr, tileSum + pack::tiles_of(sb.g.nBlocks), plans, stream);
+            hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g.pk);
+        }
+        hufe::huf_emit_kernel<EmitGeo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(emit_view(sb.g), sb.cbuf, sb.src, plans + b0, nullptr);
+        if constexpr (chainPacked) {                                // the streams' state, if the total fits
+            u64 const cgrid = ((u64)sb.g.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
+            hufe::huf_chain_state_kernel<<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(
+                sb.g, plans, tileSum + pack::tiles_of(sb.g.nBlocks));
+        }
     }
     e = cudaGetLastError();
     cudaError_t const e2 = asyncScratch ? cudaFreeAsync(plans, stream) : cudaSuccess;
@@ -1077,6 +1161,20 @@ cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned
 {
     return nStreams == 1 ? huf_encode<ChainDescs, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
                          : huf_encode<ChainDescs, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+}
+
+// packed chains (ChainPackedDescs): plan, the chains' decisions, the placement scan and raw copies, emit, the streams' state
+cudaError_t launch_huf_encode_chains_packed(const ChainPackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return nStreams == 1 ? huf_encode<ChainPackedDescs, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
+                         : huf_encode<ChainPackedDescs, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+}
+
+// the chain geometry's verdict (start[0] == 0, start[nChains] == nBlocks, never decreasing) to *malformed, for the decoders
+cudaError_t launch_huf_chain_check(const u64* start, u32 nChains, u32 nBlocks, u32* malformed, cudaStream_t stream)
+{
+    hufe::huf_chain_check_kernel<<<1, 1024, 0, stream>>>(start, nChains, nBlocks, malformed);
+    return cudaGetLastError();
 }
 
 // packed output (PackedDescs): the same kernels with the scan and placement between plan and emit

@@ -22,6 +22,8 @@ cudaError_t launch_huf_encode_packed(const PackedDescs& g, int nStreams, unsigne
 cudaError_t launch_huf_decode_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_huf_encode_repeat(const RepeatDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
+cudaError_t launch_huf_encode_chains_packed(const ChainPackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
+cudaError_t launch_huf_chain_check(const u64* start, u32 nChains, u32 nBlocks, u32* malformed, cudaStream_t stream);
 cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_fse_encode_blocks(const BlockDescs& g, bool wide, unsigned msv, unsigned tlog, cudaStream_t s);
@@ -34,6 +36,9 @@ cudaError_t launch_fse_decompress_packed(u8* const* dst, const u64* dstSize, u64
                                          u32 nBlocks, bool wide, cudaStream_t stream);
 cudaError_t launch_huf_decompress_packed(u8* const* dst, const u64* dstSize, u64* result, const u8* in, const u64* offset,
                                          u32 nBlocks, int nStreams, cudaStream_t stream);
+cudaError_t launch_huf_decompress_repeat_packed(const u64* start, u32 nChains, u8* const* dst, const u64* dstSize, u64* result,
+                                                const u8* in, const u64* offset, const u8* kind, const u8* const* chainHdr,
+                                                const u64* chainHdrSize, u32 nBlocks, int nStreams, cudaStream_t stream);
 // A whole batch of frames laid out at once (the device-memory call): frame f is blocks [first[f], first[f + 1]), role[b] >> 32
 // is block b's frame, and every frame has a block (an empty frame a placeholder of 0 source bytes).  offsets (nFrames + 1) and
 // results get the batch call's values, and only frames that end at or before `capacity` are written; work: frame_body_work bytes.

@@ -243,6 +243,78 @@ size_t FSEB200_HUF_decompress_packed(size_t nBlocks, void* const* dDsts, const s
 size_t FSEB200_HUF_decompress1X_packed(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                        const void* dIn, const size_t* dOffsets, void* stream);
 
+/* Tier 1, packed chains of table reuse (Huff0, 4X and 1X): FSEB200_HUF_compress{4X,1X}_repeat_chains with every block stored back
+ * to back in one buffer, as the packed calls above store blocks, and one kind byte per block -- a stream a caller can write, send
+ * or move as it is: bytes, nBlocks + 1 offsets and nBlocks kinds are all its decoder needs, and no header is named by a pointer.
+ * Kinds are numbered as zstd numbers its literal block types:
+ *   0 raw (n bytes of source), 1 RLE (one byte), 2 compressed with its own tree header, 3 compressed with the stream's previous
+ *   table and no header ("treeless"), 4 nothing stored.
+ * Chain geometry (dChainStarts, nChains + 1 entries), the per-block dSrcs / dSrcSizes / dPreferRepeat, the per-chain in-out state
+ * (dCTables, dRepeats, dChainHeaders, dChainHeaderSizes), the asynchrony and the argument verdicts are those of
+ * FSEB200_HUF_compress{4X,1X}_repeat_chains, and each chain runs the loop documented there with dDstCapacities[b] =
+ * HUF_compressBound(n) (n = dSrcSizes[b]), so no value is ever "does not fit its destination".  Per block b, with r its value:
+ *   dCSizes[b]  = r, except for a block that does not fit dOut (below).
+ *   stored length L[b] = that of FSEB200_HUF_compress_packed: r for r >= 2, 1 for r == 1 (the byte the reference leaves at dst[0]:
+ *                 src[0] for RLE), n (a raw copy) for r == 0, 0 for an error.  L[b] <= n, so sum(n) + 32 bytes of slack always fits.
+ *   dKinds[b]   = 0 for r == 0; 1 for r == 1; for r >= 2, 2 if the stream's flag is 0 after the step (a new table, its header
+ *                 first) and 3 if it is not (the old table, no header: what the chain call reports as dHeaderSizes[b] != 0);
+ *                 4 when dCSizes[b] is an error.  (A 1X block coded with the old table into a single byte also has r == 1, as in
+ *                 the reference, whose decoders read a 1-byte block as RLE.)
+ *   dOffsets    the packed calls' rule: the exclusive prefix sum of L, dOffsets[nBlocks] the total, written in full even when
+ *                 blocks do not fit.
+ *   capacity    block b is stored at dOut + dOffsets[b] only if dOffsets[b] + L[b] <= outCapacity; otherwise dCSizes[b] =
+ *                 dstSize_tooSmall and dKinds[b] = 4.  Nothing outside [dOut, dOut + min(total, outCapacity)) is ever written.
+ * Per-chain state on return:
+ *   if dOffsets[nBlocks] <= outCapacity: what the loop leaves (table, flag), and the chain header (dOut + dOffsets[j], L[j]) for the
+ *     chain's last kind-2 block j, or as it came in if the chain has none;
+ *   otherwise every per-chain entry exactly as it came in, so the same call can be repeated with a buffer of dOffsets[nBlocks]
+ *     bytes.  Storage is monotone in offset order: when the total does not fit, the blocks that are stored are exactly those
+ *     before the first that does not, so a stored kind-3 block's header (the last kind-2 block before it in its chain, or the
+ *     chain's entry header) is stored too; and since the state is left as it came in, no later call can be handed a header
+ *     that was never stored.
+ * Malformed chain geometry (as for the chain calls): every dCSizes[b] is srcSize_wrong, every dKinds[b] is 4, and nothing else is
+ * written -- no byte of dOut, no offset, table, flag or header.
+ * Contract: that of FSEB200_HUF_compress{4X,1X}_repeat_chains and of the packed calls; dKinds overlaps no other array.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing and writes nothing); srcSize_wrong, the device untouched, for
+ * nBlocks or nChains above 0xFFFFFFFF or a NULL array while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_HUF_compress4X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                                   void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                   const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                   unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                   unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_compress1X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                                   void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                   const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                   unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                   unsigned maxSymbolValue, unsigned tableLog, void* stream);
+/* Packed chains decompress (Huff0, 4X and 1X): every block of a buffer the calls above wrote, from its offsets and kinds.  Per block
+ * b of chain c, with L = dOffsets[b+1] - dOffsets[b], n = dDstSizes[b] (the regenerated size) and p = dIn + dOffsets[b]:
+ *   n above 128 KB: srcSize_wrong, whatever the kind (the repeat decoders' limit);
+ *   kind 0: L == n: the block is copied and the result is n (n == 0 included); otherwise corruption_detected;
+ *   kind 1: L == 1: n copies of p[0], the result n; otherwise corruption_detected;
+ *   kind 2: exactly what FSEB200_HUF_decompress{4X,1X}_repeat_blocks gives for (p, L) with header size 0;
+ *   kind 3: exactly what that call gives with the header (dIn + dOffsets[j], L[j]), j the last kind-2 block before b in chain c,
+ *           or (dChainHeaders[c], dChainHeaderSizes[c]) if there is none -- corruption_detected if that size is 0;
+ *   any other kind: corruption_detected.
+ * Malformed chain geometry makes every result srcSize_wrong, and nothing else is written.  So every block the calls above stored
+ * with a value that is not an error decodes back to its source, but for the weight-12 exception of the packed calls, and the
+ * kind-3 blocks that take their table from such a block.  dChainHeaders / dChainHeaderSizes are what the chains entered the
+ * compress call with; a chain cut into several calls enters the next with a header inside the previous call's buffer.
+ * All arrays and buffers are in DEVICE memory; the calls are asynchronous on `stream`, the host never reads the arrays, and the
+ * only memory they take is stream-ordered scratch of about 50 bytes per block.
+ * Contract: that of FSEB200_HUF_decompress_packed (dIn, and every header, readable up to the end of the 32-byte sector that holds
+ * its last byte; no destination overlaps another destination, dIn, a header or the arrays; dResults overlaps no other array).
+ * Return value: 0 (also for nBlocks == 0, which launches nothing and writes nothing); srcSize_wrong if nBlocks or nChains is
+ * above 0xFFFFFFFF or a pointer is NULL while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_HUF_decompress4X_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                              void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                              const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
+                                              const void* const* dChainHeaders, const size_t* dChainHeaderSizes, void* stream);
+size_t FSEB200_HUF_decompress1X_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                              void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                              const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
+                                              const void* const* dChainHeaders, const size_t* dChainHeaderSizes, void* stream);
+
 /* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
  * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
  * DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).
