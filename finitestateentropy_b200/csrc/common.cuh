@@ -150,6 +150,8 @@ __host__ __forceinline__ PackedDescs slice(const PackedDescs& g, u32 b0, u32 n)
     s.offset += b0; s.result += b0; s.src += b0; s.srcSize += b0; s.nBlocks = n;
     return s;
 }
+// HUF_compressBound (lib/huf.h:131-133): the capacity of a packed block of n source bytes
+__host__ __device__ __forceinline__ u64 huf_bound(u64 n) { return 129 + n + (n >> 8) + 8; }
 // bytes a block takes in the packed output, from its compress verdict: the compressed size, the RLE byte, a raw copy of the
 // source when the verdict is 0 (0 bytes for an empty block), nothing for an error
 __host__ __device__ __forceinline__ u64 packed_len(u64 v, u64 n) { return is_err(v) ? 0 : (v ? v : n); }
@@ -175,7 +177,7 @@ __device__ __forceinline__ u64& enc_out(const BlockDescs& g, u64*, u32 b) { retu
 __device__ __forceinline__ const u8* enc_src(const PackedDescs& g, const u8*, u32 b) { return g.src[b]; }
 __device__ __forceinline__ u32 enc_len(const PackedDescs& g, u32 b) { return clamp_len(g.srcSize[b]); }
 __device__ __forceinline__ u8* enc_dst(const PackedDescs& g, u8*, u32 b) { return g.out + g.offset[b]; }
-__device__ __forceinline__ u64 enc_cap(const PackedDescs& g, u32 b) { u64 const n = enc_len(g, b); return 129 + n + (n >> 8) + 8; }   // HUF_compressBound
+__device__ __forceinline__ u64 enc_cap(const PackedDescs& g, u32 b) { return huf_bound(enc_len(g, b)); }
 __device__ __forceinline__ u64& enc_out(const PackedDescs& g, u64*, u32 b) { return g.result[b]; }
 
 // -------------------------------------------------------------------------------------------
@@ -197,7 +199,7 @@ struct ChainPackedDescs : ChainDescs {
     ChainEnd* end;                 // per chain, scratch
     const u32* malformed;          // scratch: the chain geometry's verdict
 };
-__device__ __forceinline__ u64 enc_cap(const ChainPackedDescs& g, u32 b) { u64 const n = enc_len(g, b); return 129 + n + (n >> 8) + 8; }   // HUF_compressBound
+__device__ __forceinline__ u64 enc_cap(const ChainPackedDescs& g, u32 b) { return huf_bound(enc_len(g, b)); }
 __device__ __forceinline__ u8* enc_dst(const ChainPackedDescs& g, u8*, u32 b) { return g.pk.out + g.pk.offset[b]; }   // after placement
 
 // decoder: compressed source, its size, the output, the regenerated size, the result; `orig` (stored blocks) is uniform-only
