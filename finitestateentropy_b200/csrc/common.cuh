@@ -74,12 +74,6 @@ struct BlockDescs {
     const u64* srcSize;
     u32 nBlocks;
 };
-__host__ __forceinline__ BlockDescs slice(const BlockDescs& g, u32 b0, u32 n)   // blocks [b0, b0 + n) as a batch of their own
-{
-    BlockDescs s = g;
-    s.dst += b0; s.dstCap += b0; s.result += b0; s.src += b0; s.srcSize += b0; s.nBlocks = n;
-    return s;
-}
 
 // Table reuse (Huff0 compress only): a descriptor batch whose block b also carries its stream's (table, repeat flag) pair --
 // ctable[b] = 256 HUF_CElt cells (val | nbBits << 16), repeat[b] = HUF_repeat as an int, prefer[b] = preferRepeat.  The plan
@@ -89,13 +83,6 @@ struct RepeatDescs : BlockDescs {
     int* repeat;
     const int* prefer;
 };
-__host__ __forceinline__ RepeatDescs slice(const RepeatDescs& g, u32 b0, u32 n)
-{
-    RepeatDescs s = g;
-    static_cast<BlockDescs&>(s) = slice(static_cast<const BlockDescs&>(g), b0, n);
-    s.ctable += b0; s.repeat += b0; s.prefer += b0;
-    return s;
-}
 // Chains of table reuse (Huff0 compress only): chain c is blocks [start[c], start[c + 1]) of one stream, in order; the stream's
 // (table, flag, header) state comes in through ctable[c] / repeat[c] / hdr[c] / hdrSize[c] and goes back out there, and block b
 // gets the header it was coded with in blkHdr[b] / blkHdrSize[b].  The plan kernel sees only the blocks and writes nothing but
@@ -131,8 +118,7 @@ struct HeaderDescs : BlockDescs {
 // -------------------------------------------------------------------------------------------
 // Packed geometry (Huff0 compress only): sources by descriptor, outputs back to back in one buffer.  Block b is stored at
 // out + offset[b], offset[] being the exclusive prefix sum of the stored lengths (include/fse_b200.h); its capacity is
-// HUF_compressBound(srcSize), so its verdict is that of the reference at that capacity.  `offset` has nBlocks + 1 entries;
-// a slice keeps `out` and shifts `offset`, so offset[0] of a slice is the running total of the blocks before it.
+// HUF_compressBound(srcSize), so its verdict is that of the reference at that capacity.  `offset` has nBlocks + 1 entries.
 // -------------------------------------------------------------------------------------------
 struct PackedDescs {
     static constexpr bool DESCS = true;
@@ -144,12 +130,6 @@ struct PackedDescs {
     const u64* srcSize;
     u32 nBlocks;
 };
-__host__ __forceinline__ PackedDescs slice(const PackedDescs& g, u32 b0, u32 n)
-{
-    PackedDescs s = g;
-    s.offset += b0; s.result += b0; s.src += b0; s.srcSize += b0; s.nBlocks = n;
-    return s;
-}
 // HUF_compressBound (lib/huf.h:131-133): the capacity of a packed block of n source bytes
 __host__ __device__ __forceinline__ u64 huf_bound(u64 n) { return 129 + n + (n >> 8) + 8; }
 // bytes a block takes in the packed output, from its compress verdict: the compressed size, the RLE byte, a raw copy of the

@@ -252,9 +252,9 @@ cudaError_t launch_frame_body(u8* out, const u8* packed, const u64* offset, cons
         g.errBlock = errBlock; g.stored = stored;
         if ((e = cudaMemsetAsync(errBlock, 0xFF, sizeof(u64) * store->nFrames, stream)) != cudaSuccess) return e;
         frame::frame_errors_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(g);
-        pack::launch_pack<frame::Headers>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+        pack::launch_pack<frame::Headers>(g, tileSum, tileSum + tiles, nullptr, stream);
         frame::frame_settle_kernel<<<(store->nFrames + 255) / 256, 256, 0, stream>>>(g, *store, tileSum + tiles, stored);
-    } else pack::launch_pack<frame::Headers>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+    } else pack::launch_pack<frame::Headers>(g, tileSum, tileSum + tiles, nullptr, stream);
     pack::launch_per_block(frame::frame_payload_kernel, n, stream, g);
     return cudaGetLastError();
 }

@@ -160,14 +160,14 @@ cudaError_t compress_packed(FsePack g, unsigned msv, unsigned tlog, cudaStream_t
     g.stageDst = (u8**)s; g.stageCap = (u64*)(s + 8 * n); g.stageSize = (u64*)(s + 16 * n);
     u64* const tileSum = (u64*)(s + 24 * n);                        // tiles + 1 words: the slots' total goes to the last
     // 1. staging slots
-    pack::launch_pack<StageSlots<WIDE>>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+    pack::launch_pack<StageSlots<WIDE>>(g, tileSum, tileSum + tiles, nullptr, stream);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // 2. the descriptor encode into the slots
     BlockDescs st;
     st.dst = g.stageDst; st.dstCap = g.stageCap; st.result = g.result; st.src = g.src; st.srcSize = g.stageSize; st.nBlocks = g.nBlocks;
     if ((e = launch_fse_encode_blocks(st, WIDE, msv, tlog, stream)) != cudaSuccess) return e;
     // 3. offsets and verdicts
-    pack::launch_pack<PackedBlocks<WIDE>>(g, tileSum, nullptr, g.offset + n, nullptr, stream);
+    pack::launch_pack<PackedBlocks<WIDE>>(g, tileSum, g.offset + n, nullptr, stream);
     // 4. the bytes
     pack::launch_per_block(fse_pack_copy_kernel<WIDE>, n, stream, g);
     return cudaGetLastError();

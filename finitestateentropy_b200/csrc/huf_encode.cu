@@ -28,7 +28,6 @@
 //      histograms of the plan kernel.  (An earlier version gave each thread a contiguous run of
 //      symbols staged in shared memory: runs are 128 bytes apart, i.e. all 32 lanes of a warp in the
 //      same bank -- 525M bank conflicts per 256 MiB, short-scoreboard 38 stalls per issue.)
-#include <cstdlib>
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -906,8 +905,7 @@ huf_emit_kernel(Geo g, u8* __restrict__ cbuf, const u8* __restrict__ src, const 
 // Packed output (PackedDescs): the plan kernel has settled every block's verdict, so every block's stored length is known
 // before anything is written.  Between plan and emit, a device-wide exclusive scan of the stored lengths (pack_dev.cuh) gives
 // each block its offset, and placement settles what the plan kernel left open: the capacity verdict (the plan is made final,
-// emit skips the block), the RLE byte and the raw copy of a block whose verdict is 0.  The scan starts each sub-batch from the
-// total of the sub-batches before.
+// emit skips the block), the RLE byte and the raw copy of a block whose verdict is 0.
 // ---------------------------------------------------------------------------------------------
 struct HufPlace {
     typedef PackedDescs Geo;
@@ -1039,22 +1037,6 @@ cudaError_t launch_huf_encode_using_ctable(const BatchGeom& g, void* cbuf, u64* 
 }
 
 namespace {
-// blocks [b0, b0 + n) of a batch as a batch of their own: the same geometry over shifted buffers, or a slice of the arrays
-template <class G> struct Sub { G g; u8* cbuf; const u8* src; };
-Sub<BatchGeom> sub_batch(const BatchGeom& g, u8* cbuf, const u8* src, u32 b0, u32 n)
-{
-    BatchGeom gs = g;
-    gs.nBlocks = n;
-    u64 const off = (u64)b0 * g.blockSize;
-    u64 const span = (u64)n * g.blockSize;
-    gs.total = (g.total - off < span) ? g.total - off : span;
-    return { gs, cbuf + (u64)b0 * g.slot, src + off };
-}
-template <class G> Sub<G> sub_batch(const G& g, u8*, const u8*, u32 b0, u32 n)
-{
-    if constexpr (std::is_base_of_v<ChainDescs, G>) return { g, nullptr, nullptr };     // chains: always the whole batch
-    else return { slice(g, b0, n), nullptr, nullptr };
-}
 // the emit kernel's geometry argument: packed chains are emitted as the packed blocks they are, everything else as itself
 template <class Geo> const Geo& emit_view(const Geo& g) { return g; }
 const PackedDescs& emit_view(const ChainPackedDescs& g) { return g.pk; }
@@ -1064,34 +1046,22 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
 {
     if (g.nBlocks == 0) return cudaSuccess;
     cudaError_t e;
-    hufe::Plan* plans = nullptr;
     // Plan scratch (3.2 KB per block): the per-stream grow-only buffer launch_huf_encode_using_ctable also takes its plans from.
-    // FSEB200_SCRATCH_ASYNC=1 switches to cudaMallocAsync/FreeAsync.
-    static int asyncScratch = -1;
-    if (asyncScratch < 0) { const char* const v = getenv("FSEB200_SCRATCH_ASYNC"); asyncScratch = (v && atoi(v) == 1) ? 1 : 0; }
-    size_t const need = sizeof(hufe::Plan) * (size_t)g.nBlocks;
-    if (asyncScratch) e = cudaMallocAsync((void**)&plans, need, stream);
-    else plans = (hufe::Plan*)stream_scratch(2, stream, need, &e);
+    hufe::Plan* const plans = (hufe::Plan*)stream_scratch(2, stream, sizeof(hufe::Plan) * (size_t)g.nBlocks, &e);
     if (e != cudaSuccess) return e;
-    // The source is read twice, by the plan kernel (histogram) and by the emit kernel: 1.70x the algorithmic DRAM bytes.  Walking the
-    // batch in sub-batches whose source fits the 50 MB L2 (FSEB200_HUF_ENC_SUBBATCH = blocks per sub-batch) turns the second read into
-    // L2 hits, but every launch pair then pays the plan kernel's tail (its per-block serial chains drain with the SMs mostly idle).
-    // Both kernels are issue-bound, not DRAM-bound, so the default (0) keeps one launch pair for the whole batch.
-    static u32 const subBatch = [] { const char* const v = getenv("FSEB200_HUF_ENC_SUBBATCH"); long n = v ? atol(v) : 0; return (u32)(n < 0 ? 0 : n); }();
     size_t const smem = sizeof(hufe::PlanCta);
     static SmemOptIn optin;
     e = optin.ensure(hufe::huf_plan_kernel<Geo, NS>, current_device(), (int)smem);
     if (e != cudaSuccess) return e;
-    constexpr bool chain = std::is_base_of_v<ChainDescs, Geo>;     // every plan must exist before the chains' decisions: no sub-batches
+    constexpr bool chain = std::is_base_of_v<ChainDescs, Geo>;
     constexpr bool chainPacked = std::is_same_v<Geo, ChainPackedDescs>;
-    u32 const step = (!chain && subBatch && subBatch < g.nBlocks) ? subBatch : g.nBlocks;
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
     using EmitGeo = std::conditional_t<chainPacked, PackedDescs,    // the plan holds the chosen table
                                        std::conditional_t<std::is_same_v<Geo, RepeatDescs> || chain, BlockDescs, Geo>>;
-    u64* tileSum = nullptr;                                         // packed: one word per scan tile of a sub-batch (packed chains: + the total)
+    u64* tileSum = nullptr;                                         // packed: one word per scan tile (packed chains: + the total)
     if constexpr (packed || chainPacked) {
-        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * (pack::tiles_of(step) + chainPacked), &e);
-        if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
+        tileSum = (u64*)stream_scratch(4, stream, sizeof(u64) * (pack::tiles_of(g.nBlocks) + chainPacked), &e);
+        if (e != cudaSuccess) return e;
     }
     Geo gx = g;
     u32* malformed = nullptr;                                       // chains: the geometry verdict, then one fact per block
@@ -1102,36 +1072,30 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
             gx.malformed = malformed;
             if (e == cudaSuccess) gx.end = (ChainEnd*)stream_scratch(11, stream, sizeof(ChainEnd) * ((size_t)g.nChains + 1), &e);
         }
-        if (e != cudaSuccess) { if (asyncScratch) cudaFreeAsync(plans, stream); return e; }
+        if (e != cudaSuccess) return e;
     }
-    for (u32 b0 = 0; b0 < g.nBlocks; b0 += step) {
-        auto const sb = sub_batch(gx, (u8*)cbuf, (const u8*)src, b0, (g.nBlocks - b0 < step) ? g.nBlocks - b0 : step);
-        u64* const cs = csizes ? csizes + b0 : nullptr;
-        unsigned const grid = (sb.g.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
-        hufe::huf_plan_kernel<Geo, NS><<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(sb.g, sb.cbuf, cs, sb.src, msv, tlog, plans + b0);
-        if constexpr (packed) {                                     // offsets, capacity verdicts, RLE bytes, raw copies; then emit
-            pack::launch_pack<hufe::HufPlace>(sb.g, tileSum, b0 ? sb.g.offset : nullptr, sb.g.offset + sb.g.nBlocks, plans + b0, stream);
-            hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g);
-        }
-        if constexpr (chain) {
-            hufe::huf_chain_check_kernel<<<1, 1024, 0, stream>>>(sb.g.start, sb.g.nChains, sb.g.nBlocks, malformed);
-            u64 const cgrid = ((u64)sb.g.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
-            hufe::huf_chain_kernel<NS, Geo><<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(sb.g, plans, malformed);
-        }
-        if constexpr (chainPacked) {                                // offsets, kinds, capacity verdicts, RLE bytes, raw copies; then emit
-            pack::launch_pack<hufe::HufChainPlace>(sb.g, tileSum, nullptr, tileSum + pack::tiles_of(sb.g.nBlocks), plans, stream);
-            hufe::huf_pack_raw_kernel<<<sb.g.nBlocks, pack::COPY_THREADS, 0, stream>>>(sb.g.pk);
-        }
-        hufe::huf_emit_kernel<EmitGeo, NS><<<sb.g.nBlocks, 32 * NS, 0, stream>>>(emit_view(sb.g), sb.cbuf, sb.src, plans + b0, nullptr);
-        if constexpr (chainPacked) {                                // the streams' state, if the total fits
-            u64 const cgrid = ((u64)sb.g.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
-            hufe::huf_chain_state_kernel<<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(
-                sb.g, plans, tileSum + pack::tiles_of(sb.g.nBlocks));
-        }
+    unsigned const grid = (g.nBlocks + hufe::GROUP - 1) / hufe::GROUP;
+    hufe::huf_plan_kernel<Geo, NS><<<grid, 32 * hufe::PLAN_WARPS, smem, stream>>>(gx, (u8*)cbuf, csizes, (const u8*)src, msv, tlog, plans);
+    if constexpr (packed) {                                         // offsets, capacity verdicts, RLE bytes, raw copies; then emit
+        pack::launch_pack<hufe::HufPlace>(gx, tileSum, gx.offset + gx.nBlocks, plans, stream);
+        hufe::huf_pack_raw_kernel<<<gx.nBlocks, pack::COPY_THREADS, 0, stream>>>(gx);
     }
-    e = cudaGetLastError();
-    cudaError_t const e2 = asyncScratch ? cudaFreeAsync(plans, stream) : cudaSuccess;
-    return e != cudaSuccess ? e : e2;
+    if constexpr (chain) {
+        hufe::huf_chain_check_kernel<<<1, 1024, 0, stream>>>(gx.start, gx.nChains, gx.nBlocks, malformed);
+        u64 const cgrid = ((u64)gx.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
+        hufe::huf_chain_kernel<NS, Geo><<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(gx, plans, malformed);
+    }
+    if constexpr (chainPacked) {                                    // offsets, kinds, capacity verdicts, RLE bytes, raw copies; then emit
+        pack::launch_pack<hufe::HufChainPlace>(gx, tileSum, tileSum + pack::tiles_of(gx.nBlocks), plans, stream);
+        hufe::huf_pack_raw_kernel<<<gx.nBlocks, pack::COPY_THREADS, 0, stream>>>(gx.pk);
+    }
+    hufe::huf_emit_kernel<EmitGeo, NS><<<gx.nBlocks, 32 * NS, 0, stream>>>(emit_view(gx), (u8*)cbuf, (const u8*)src, plans, nullptr);
+    if constexpr (chainPacked) {                                    // the streams' state, if the total fits
+        u64 const cgrid = ((u64)gx.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
+        hufe::huf_chain_state_kernel<<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(
+            gx, plans, tileSum + pack::tiles_of(gx.nBlocks));
+    }
+    return cudaGetLastError();
 }
 }  // namespace
 

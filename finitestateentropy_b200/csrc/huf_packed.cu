@@ -145,7 +145,7 @@ cudaError_t launch_huf_decompress_repeat_packed(const u64* start, u32 nChains, u
     u32* const malformed = w;
     g.malformed = malformed; g.count = w + 2; g.newPos = w + 2 + n; g.act = (u8*)(w + 2 + 2 * n);
     if ((e = launch_huf_chain_check(start, nChains, nBlocks, malformed, stream)) != cudaSuccess) return e;
-    pack::launch_pack<hufp::CountNew>(g, tileSum, nullptr, tileSum + tiles, nullptr, stream);
+    pack::launch_pack<hufp::CountNew>(g, tileSum, tileSum + tiles, nullptr, stream);
     hufp::huf_chain_resolve_kernel<<<(unsigned)((n + hufp::THREADS - 1) / hufp::THREADS), hufp::THREADS, 0, stream>>>(g);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     HeaderDescs d;

@@ -2,9 +2,9 @@
 // (huf_encode.cu: Huff0 compress; fse_packed.cu: FSE / FSE-U16 compress and decompress) and the .fse frame calls (frame.cu).
 //
 // Offsets: a device-wide exclusive scan of per-block lengths, reduce-then-scan over tiles of PACK_TILE blocks -- the tiles'
-// sums (pack_sums_kernel), their exclusive scan in one CTA starting from a carried-in total (pack_scan_tiles_kernel), then the
-// scan inside each tile, handing every block its offset (pack_place_kernel) -- in u64, so totals above 2^32 and batches of up to
-// 2^32 - 1 blocks are exact.  What is scanned and what happens at the offsets is the caller's, through a placement P:
+// sums (pack_sums_kernel), their exclusive scan from 0 in one CTA (pack_scan_tiles_kernel), then the scan inside each tile,
+// handing every block its offset (pack_place_kernel) -- in u64, so totals above 2^32 and batches of up to 2^32 - 1 blocks are
+// exact.  What is scanned and what happens at the offsets is the caller's, through a placement P:
 //   P::Geo                                 the kernels' argument (it has nBlocks); P::Aux a pointer the place step may use
 //   P::value(g, b)                         the per-block word the length derives from (read once per block by the place step)
 //   P::len(g, b, v)                        the bytes block b takes
@@ -61,12 +61,12 @@ pack_sums_kernel(typename P::Geo g, u64* __restrict__ tileSum)
     if (threadIdx.x == 0) tileSum[blockIdx.x] = t;
 }
 
-// step 2, one CTA: tile sums -> tile offsets (in place), from *carryIn (nullptr: 0); the grand total goes to *totalOut
+// step 2, one CTA: tile sums -> tile offsets (in place), from 0; the grand total goes to *totalOut
 static __global__ void __launch_bounds__(PACK_SCAN_THREADS)
-pack_scan_tiles_kernel(u64* __restrict__ tileSum, u32 nTiles, const u64* __restrict__ carryIn, u64* __restrict__ totalOut)
+pack_scan_tiles_kernel(u64* __restrict__ tileSum, u32 nTiles, u64* __restrict__ totalOut)
 {
     __shared__ u64 sm[PACK_SCAN_THREADS / 32 + 1];
-    u64 run = carryIn ? *carryIn : 0;
+    u64 run = 0;
     for (u32 t0 = 0; t0 < nTiles; t0 += PACK_SCAN_THREADS) {
         u32 const t = t0 + threadIdx.x;
         u64 const v = t < nTiles ? tileSum[t] : 0;
@@ -107,13 +107,13 @@ pack_place_kernel(typename P::Geo g, const u64* __restrict__ tileOff, typename P
 }
 
 inline unsigned tiles_of(u64 n) { return (unsigned)((n + PACK_TILE - 1) / PACK_TILE); }
-// the three steps for P; tileSum: tiles_of(g.nBlocks) words; the scan starts from *carryIn (nullptr: 0), its total to *totalOut
+// the three steps for P; tileSum: tiles_of(g.nBlocks) words; the total goes to *totalOut
 template <class P>
-void launch_pack(const typename P::Geo& g, u64* tileSum, const u64* carryIn, u64* totalOut, typename P::Aux aux, cudaStream_t stream)
+void launch_pack(const typename P::Geo& g, u64* tileSum, u64* totalOut, typename P::Aux aux, cudaStream_t stream)
 {
     unsigned const tiles = tiles_of(g.nBlocks);
     pack_sums_kernel<P><<<tiles, PACK_THREADS, 0, stream>>>(g, tileSum);
-    pack_scan_tiles_kernel<<<1, PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, carryIn, totalOut);
+    pack_scan_tiles_kernel<<<1, PACK_SCAN_THREADS, 0, stream>>>(tileSum, tiles, totalOut);
     pack_place_kernel<P><<<tiles, PACK_THREADS, 0, stream>>>(g, tileSum, aux);
 }
 

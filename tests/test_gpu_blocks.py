@@ -1,10 +1,10 @@
 """Per-block descriptor calls (FSEB200_HUF_compress_blocks / FSEB200_HUF_decompress_blocks) against the compiled reference,
 block by block (-m gpu): ragged sizes, sources anywhere (overlapping too), every capacity and parameter verdict, packed
 compressed inputs and outputs at odd offsets, malformed blocks, the head decode at every residue, equivalence with the uniform
-calls, a batch of two pass-A rounds, the tuning knobs, and the call's own argument checks.
+calls, a batch of two pass-A rounds, the decoder's row budgets, and the call's own argument checks.
 
 Run as a script (`python tests/test_gpu_blocks.py --child`) it repeats subsets of the ragged tests under the environment it
-was started with: test_knobs starts it with FSEB200_HUF_ENC_SUBBATCH and FSEB200_HUFD_ROWS / _ROWS_B set."""
+was started with: test_knobs starts it with FSEB200_HUFD_ROWS / _ROWS_B set."""
 import os
 import subprocess
 import sys
@@ -368,12 +368,11 @@ def test_large_batch_two_rounds():
 
 
 def test_knobs():
-    """the sub-batched encoder and the single-pass decoder at the smallest row budget, each in a child process"""
+    """the single-pass decoder at the smallest row budget, in a child process"""
     _ref()
-    for env in ({"FSEB200_HUF_ENC_SUBBATCH": "7"}, {"FSEB200_HUFD_ROWS": "160", "FSEB200_HUFD_ROWS_B": "0"}):
-        e = dict(os.environ, **env)
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, capture_output=True, text=True, timeout=1200)
-        assert r.returncode == 0 and "child ok" in r.stdout, (env, r.stdout[-2000:], r.stderr[-4000:])
+    e = dict(os.environ, FSEB200_HUFD_ROWS="160", FSEB200_HUFD_ROWS_B="0")
+    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, capture_output=True, text=True, timeout=1200)
+    assert r.returncode == 0 and "child ok" in r.stdout, (r.stdout[-2000:], r.stderr[-4000:])
 
 
 def test_arguments_and_wrappers():

@@ -1,11 +1,11 @@
 """Single-stream per-block descriptor calls (FSEB200_HUF_compress1X_blocks / FSEB200_HUF_decompress1X_blocks) against the
 compiled reference's HUF_compress1X / HUF_decompress1X_DCtx, block by block (-m gpu): ragged sizes, sources anywhere
 (overlapping too), every capacity and parameter verdict, packed compressed inputs and outputs at odd offsets, malformed
-blocks, the head decode at every residue, a batch of two pass-A rounds, the tuning knobs and the calls' own argument checks.
-The block contents and layouts are those of tests/test_gpu_blocks.py (imported).
+blocks, the head decode at every residue, a batch of two pass-A rounds, the decoder's row budgets and the calls' own argument
+checks.  The block contents and layouts are those of tests/test_gpu_blocks.py (imported).
 
 Run as a script (`python tests/test_gpu_blocks_1x.py --child`) it repeats subsets of the ragged tests under the environment it
-was started with: test_knobs starts it with FSEB200_HUF_ENC_SUBBATCH and FSEB200_HUFD_ROWS / _ROWS_B set."""
+was started with: test_knobs_1x starts it with FSEB200_HUFD_ROWS / _ROWS_B set."""
 import ctypes as C
 import os
 import subprocess
@@ -311,12 +311,11 @@ def test_large_batch_two_rounds_1x():
 
 
 def test_knobs_1x():
-    """the sub-batched encoder and the single-pass decoder at the smallest row budget, each in a child process"""
+    """the single-pass decoder at the smallest row budget, in a child process"""
     _ref1x()
-    for env in ({"FSEB200_HUF_ENC_SUBBATCH": "7"}, {"FSEB200_HUFD_ROWS": "160", "FSEB200_HUFD_ROWS_B": "0"}):
-        e = dict(os.environ, **env)
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, capture_output=True, text=True, timeout=1200)
-        assert r.returncode == 0 and "child ok" in r.stdout, (env, r.stdout[-2000:], r.stderr[-4000:])
+    e = dict(os.environ, FSEB200_HUFD_ROWS="160", FSEB200_HUFD_ROWS_B="0")
+    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, capture_output=True, text=True, timeout=1200)
+    assert r.returncode == 0 and "child ok" in r.stdout, (r.stdout[-2000:], r.stderr[-4000:])
 
 
 def test_arguments_and_wrappers_1x():

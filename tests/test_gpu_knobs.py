@@ -26,9 +26,6 @@ SETTINGS = [
     {"FSEB200_HUFD_ROWS_B": "0"},
     {"FSEB200_HUFD_ROWS": "max"},
     {"FSEB200_HUFD_ROWS": "1700"},                                      # above the device maximum: clamped
-    {"FSEB200_HUF_ENC_SUBBATCH": "7"},
-    {"FSEB200_HUF_SERIAL_HEADER": "1"},
-    {"FSEB200_SCRATCH_ASYNC": "1"},
     {"FSEB200_ENC_EK": "8"},
     {"FSEB200_HOST_CHUNK_BLOCKS": "64"},
 ]

@@ -3,13 +3,8 @@ the whole output buffer is compared with the packed image the host model (tests/
 HUF_compress1X at HUF_compressBound(n), with the offsets and values exact and poisoned canaries around it.  Ragged, small-block
 and special-size layouts with overlapping sources, every output offset mod 16 the kernels branch on, capacities that cut the
 stream, bad parameters, a batch of more than one plan round, a total above 4 GiB, the round trip through packed_pointers and
-the descriptor decoders, and the calls' argument checks.  Block contents and layouts are those of tests/test_gpu_blocks.py.
-
-Run as a script (`python tests/test_gpu_packed.py --child`) it repeats a ragged subset under the environment it was started
-with: test_knobs starts it with FSEB200_HUF_ENC_SUBBATCH=37 (the scan's running total carried across sub-batches) and with
-FSEB200_SCRATCH_ASYNC=1."""
+the descriptor decoders, and the calls' argument checks.  Block contents and layouts are those of tests/test_gpu_blocks.py."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -233,15 +228,6 @@ def test_total_above_4gib():
         out[-n:].fill_(POISON)
 
 
-def test_knobs():
-    """the packed compress sub-batched (37 blocks per sub-batch) and with stream-ordered scratch, each in a child process"""
-    _ref()
-    for env in ({"FSEB200_HUF_ENC_SUBBATCH": "37"}, {"FSEB200_SCRATCH_ASYNC": "1"}):
-        e = dict(os.environ, **env)
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, capture_output=True, text=True, timeout=1200)
-        assert r.returncode == 0 and "child ok" in r.stdout, (env, r.stdout[-2000:], r.stderr[-4000:])
-
-
 def test_arguments_and_wrappers():
     import torch
     import finitestateentropy_b200 as fb
@@ -283,13 +269,3 @@ def test_arguments_and_wrappers():
         assert res.tolist() == n.tolist() and all(torch.equal(o, d) for o, d in zip(outs, data))
         with pytest.raises(AssertionError):
             enc(srcs, n, offsets=torch.empty(4, dtype=torch.int64, device="cuda"))
-
-
-def _child():
-    for onex in FORMATS:
-        ragged_check(onex, seed=608, count=400)
-    print("child ok")
-
-
-if __name__ == "__main__" and "--child" in sys.argv:
-    _child()
