@@ -580,6 +580,83 @@ def host_decompress_packed(packed, offsets, dst_sizes, codec, out=None, results=
     return out, results
 
 
+# Host-buffer packed chains of table reuse (FSEB200_{compress_host_repeat_chains,decompress_host_repeat}_packed): name -> C codec
+HOST_CHAIN_CODECS = {"huf": 1, "huf1x": 3}
+
+
+def _host_chain_args(chain_starts, per_chain):
+    chain_starts = _host_sizes(chain_starts)
+    n_chains = chain_starts.numel() - 1
+    assert n_chains >= 0, chain_starts.numel()
+    for a, dtype, shape in per_chain:
+        _host_check(a, dtype)
+        assert tuple(a.shape) == (n_chains,) + shape, (tuple(a.shape), n_chains)
+    return chain_starts, n_chains
+
+
+def host_compress_repeat_chains_packed(src, sizes, chain_starts, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
+                                       codec="huf", out=None, max_symbol_value=255, table_log=12):
+    """The packed chain compress of `codec` ("huf" or "huf1x") on HOST memory: block b is sizes[b] bytes of `src` (a CPU uint8
+    tensor, pinned or pageable) right after block b - 1, chain c is blocks [chain_starts[c], chain_starts[c + 1]), and prefer (int32,
+    one per block) is each block's preferRepeat.  The streams' state is in-out, in CPU tensors: ctables (uint32 or int32, n_chains x
+    256 HUF_CElt cells), repeats (int32 HUF_repeat), chain_hdr_ptrs (int64 host addresses) and chain_hdr_sizes (int64); it is
+    updated only when the whole stream fits `out`, and a header that comes back points into `out`.  `out` (capacity out.numel(),
+    allocated at sum(sizes) + 32 bytes if None, always enough), offsets, csizes and kinds are what the device call
+    huf_compress_repeat_chains_packed gives.  Synchronous.  Returns (out, offsets, csizes, kinds, (ctables, repeats,
+    chain_hdr_ptrs, chain_hdr_sizes))."""
+    from . import lib
+    cid = HOST_CHAIN_CODECS[codec]
+    sizes = _host_sizes(sizes)
+    n = sizes.numel()
+    _host_check(src, torch.uint8)
+    _host_check(prefer, torch.int32)
+    assert src.numel() >= int(sizes.sum()) and prefer.numel() == n, (src.numel(), prefer.numel(), n)
+    assert ctables.dtype in (torch.int32, torch.uint32), ctables.dtype
+    chain_starts, n_chains = _host_chain_args(chain_starts, ((ctables, ctables.dtype, (256,)), (repeats, torch.int32, ()),
+                                                             (chain_hdr_ptrs, torch.int64, ()), (chain_hdr_sizes, torch.int64, ())))
+    if out is None:
+        out = torch.empty(int(sizes.sum()) + 32, dtype=torch.uint8)
+    _host_check(out, torch.uint8)
+    offsets = torch.empty(n + 1, dtype=torch.int64)
+    csizes = torch.empty(n, dtype=torch.int64)
+    kinds = torch.empty(n, dtype=torch.uint8)
+    table_ptrs = torch.tensor([ctables.data_ptr() + 1024 * c for c in range(n_chains)], dtype=torch.int64)
+    r = lib().FSEB200_compress_host_repeat_chains_packed(
+        cid, n_chains, chain_starts.data_ptr(), n, _host_ptr(out), out.numel(), offsets.data_ptr(), _host_ptr(csizes), _host_ptr(kinds),
+        _host_ptr(src), _host_ptr(sizes), _host_ptr(prefer), _host_ptr(table_ptrs), _host_ptr(repeats), _host_ptr(chain_hdr_ptrs),
+        _host_ptr(chain_hdr_sizes), max_symbol_value, table_log)
+    _ret(r, "FSEB200_compress_host_repeat_chains_packed")
+    return out, offsets, csizes, kinds, (ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes)
+
+
+def host_decompress_repeat_packed(packed, offsets, kinds, chain_starts, dst_sizes, chain_hdr_ptrs, chain_hdr_sizes, codec="huf",
+                                  out=None, results=None):
+    """The packed chain decompress of `codec` on HOST memory: every block of `packed` (a CPU uint8 tensor,
+    host_compress_repeat_chains_packed's out) located by `offsets` and `kinds`, regenerating dst_sizes[b] bytes; block b lands in
+    `out` right after block b - 1.  chain_hdr_ptrs / chain_hdr_sizes (int64 CPU tensors, host addresses) are the headers the chains
+    entered the compress with.  With out=None it is allocated at sum(dst_sizes) bytes.  results (int64) equals the device call
+    huf_decompress_repeat_packed's.  Synchronous.  Returns (out, results)."""
+    from . import lib
+    cid = HOST_CHAIN_CODECS[codec]
+    dst_sizes = _host_sizes(dst_sizes)
+    n = dst_sizes.numel()
+    total = int(dst_sizes.sum())
+    _host_check(packed, torch.uint8); _host_check(offsets, torch.int64); _host_check(kinds, torch.uint8)
+    assert offsets.numel() == n + 1 and kinds.numel() == n and packed.numel() >= int(offsets[-1]), (offsets.numel(), kinds.numel(), n)
+    chain_starts, n_chains = _host_chain_args(chain_starts, ((chain_hdr_ptrs, torch.int64, ()), (chain_hdr_sizes, torch.int64, ())))
+    if out is None:
+        out = torch.empty(total, dtype=torch.uint8)
+    if results is None:
+        results = torch.empty(n, dtype=torch.int64)
+    _host_check(out, torch.uint8); _host_check(results, torch.int64)
+    assert out.numel() >= total and results.numel() == n, (out.numel(), total, results.numel(), n)
+    r = lib().FSEB200_decompress_host_repeat_packed(
+        cid, n_chains, chain_starts.data_ptr(), n, _host_ptr(out), _host_ptr(dst_sizes), _host_ptr(results), _host_ptr(packed),
+        offsets.data_ptr(), _host_ptr(kinds), _host_ptr(chain_hdr_ptrs), _host_ptr(chain_hdr_sizes))
+    _ret(r, "FSEB200_decompress_host_repeat_packed")
+    return out, results
+
+
 # .fse frames (FSEB200_frame_{compress,decompress}_host): codec name -> C codec number
 FRAME_CODECS = {"fse": 0, "huf": 1}
 

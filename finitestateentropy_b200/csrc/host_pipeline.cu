@@ -1,6 +1,7 @@
 // host_pipeline.cu -- whole-batch calls on HOST buffers (what an unmodified host program would hand over; declarations:
-// include/fse_b200.h): the slot pair FSEB200_{compress,decompress}_host, the packed pair FSEB200_{compress,decompress}_host_packed
-// and the .fse frame calls.  Each cuts its batch into chunks that are copied in, processed and copied out on a ring of streams,
+// include/fse_b200.h): the slot pair FSEB200_{compress,decompress}_host, the packed pair FSEB200_{compress,decompress}_host_packed,
+// the packed Huff0 chain pair FSEB200_compress_host_repeat_chains_packed / FSEB200_decompress_host_repeat_packed and the .fse
+// frame calls.  Each cuts its batch into chunks that are copied in, processed and copied out on a ring of streams,
 // so that PCIe transfers overlap the kernels; one driver, run_chunks, runs the chunks of every call.
 #include "capi_common.h"
 #include "fse_b200.h"
@@ -271,6 +272,29 @@ cudaError_t queue_packed_compress(Ring<3>& P, int k, const HostChunk& c, int cod
     g.src = src; g.srcSize = d + L.size; g.nBlocks = (u32)cb;
     return launch_huf_encode_packed(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
 }
+
+// The finish of a packed compress chunk c whose offsets `lo` (chunk-local, cb + 1) and values have landed in the pinned image:
+// global offsets, the capacity rule of one call over the whole batch (a block that does not fit gets dstSize_tooSmall and, where
+// there are kinds, kind 4), and the stored bytes -- a prefix of the chunk's packed bytes at dOut, since the blocks that fit come
+// first -- copied down on s.  `total` is the global offset of the chunk's first block and moves past the chunk.
+cudaError_t finish_packed(const HostChunk& c, const u64* lo, const u64* vals, const u8* kinds, const u8* dOut, cudaStream_t s,
+                          u8* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds, u64& total)
+{
+    size_t const cb = c.b1 - c.b0;
+    u64 end = 0;
+    for (size_t b = 0; b < cb; b++) {
+        u64 const off = total + lo[b], len = lo[b + 1] - lo[b];
+        u64 v = vals[b];
+        bool const over = !is_err(v) && off + len > outCapacity;
+        if (over) v = err(E_DST_TOO_SMALL);
+        else if (!is_err(v) && len) end = lo[b + 1];
+        hOffsets[c.b0 + b] = (size_t)off; hCSizes[c.b0 + b] = (size_t)v;
+        if (hKinds) hKinds[c.b0 + b] = over ? 4 : kinds[b];
+    }
+    u8* const at = hOut + total;
+    total += lo[cb];
+    return end ? cudaMemcpyAsync(at, dOut, end, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+}
 }
 
 FSEB_API size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
@@ -301,24 +325,11 @@ FSEB_API size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCa
     // finish: global offsets, the capacity rule of one call over the whole batch, and the stored bytes -- a prefix of the chunk's
     // packed bytes, since the blocks that fit come first -- copied down
     auto finish = [&](size_t ci, int k) -> cudaError_t {
-        const HostChunk& c = chunks[ci];
-        size_t const cb = c.b1 - c.b0;
-        PackedWords const L(cb);
-        cudaError_t r = cudaStreamSynchronize(P.st[k]);
+        PackedWords const L(chunks[ci].b1 - chunks[ci].b0);
+        cudaError_t const r = cudaStreamSynchronize(P.st[k]);
         if (r != cudaSuccess) return r;
-        const u64* const lo = P.hD[k] + L.offset;
-        const u64* const vals = P.hD[k] + L.value;
-        u64 end = 0;
-        for (size_t b = 0; b < cb; b++) {
-            u64 const off = total + lo[b], len = lo[b + 1] - lo[b];
-            u64 v = vals[b];
-            if (!is_err(v) && off + len > outCapacity) v = err(E_DST_TOO_SMALL);
-            else if (!is_err(v) && len) end = lo[b + 1];
-            hOffsets[c.b0 + b] = (size_t)off; hCSizes[c.b0 + b] = (size_t)v;
-        }
-        if (end && (r = cudaMemcpyAsync((u8*)hOut + total, P.dB[k], end, cudaMemcpyDeviceToHost, P.st[k])) != cudaSuccess) return r;
-        total += lo[cb];
-        return cudaSuccess;
+        return finish_packed(chunks[ci], P.hD[k] + L.offset, P.hD[k] + L.value, nullptr, P.dB[k], P.st[k], (u8*)hOut, outCapacity,
+                             hOffsets, hCSizes, nullptr, total);
     };
     if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish);
     if (e != cudaSuccess) return (size_t)err(E_GENERIC);
@@ -370,6 +381,282 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
         PackedWords const L(chunks[ci].b1 - chunks[ci].b0);
         cudaError_t const r = cudaStreamSynchronize(P.st[k]);
         if (r == cudaSuccess) std::memcpy(hResults + chunks[ci].b0, P.hD[k] + L.value, (L.end - L.value) * sizeof(u64));
+        return r;
+    };
+    if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS, queue, finish);
+    return e == cudaSuccess ? 0 : (size_t)err(E_GENERIC);
+}
+
+// ================================================================================================
+// packed chains of table reuse on HOST buffers: FSEB200_HUF_compress{4X,1X}_repeat_chains_packed and
+// FSEB200_HUF_decompress{4X,1X}_repeat_packed through the packed pair's ring and chunk budget, chain boundaries ignored; each
+// chunk runs the device call unchanged on chunk-local geometry.  Chains are contiguous ranges of blocks, so the chains that meet
+// a chunk are a contiguous range of which only the first can have started in an earlier chunk: at most one chain crosses each
+// chunk boundary, and its state (compress) or its last tree header (decompress) is all that passes from chunk to chunk.
+// codec: 1 = Huff0 4X, 3 = Huff0 1X.
+// ================================================================================================
+namespace {
+// The most of a tree header a Huff0 decoder reads (HUF_readStats: 1 + 127 bytes in the FSE form, 1 + 64 raw); a header's size
+// enters its verdict only through iSize + 1 > size, so a longer one is passed as its first HDR_MAX bytes with the same verdicts.
+constexpr u64 HDR_MAX = 128;
+constexpr size_t NONE = SIZE_MAX;
+
+// start[0] == 0, start[nChains] == nBlocks, never decreasing: the device calls' geometry check
+bool chains_sound(const size_t* start, size_t nChains, size_t nBlocks)
+{
+    if (start[0] != 0 || start[nChains] != nBlocks) return false;
+    for (size_t c = 0; c < nChains; c++) if (start[c + 1] < start[c]) return false;
+    return true;
+}
+
+// The chains [c0, c0 + n) that chunk c meets (sound geometry): c0 holds block b0, i.e. it is the last chain whose start is <= b0,
+// as the decoder assigns blocks, and the last holds b1 - 1.  Their chunk-local starts are start - b0 clamped at 0, then cb.
+struct ChunkChains {
+    size_t c0, n;
+    ChunkChains(const size_t* start, size_t nChains, const HostChunk& c)
+    {
+        auto holder = [&](size_t b) { return (size_t)(std::upper_bound(start, start + nChains + 1, b) - start) - 1; };
+        c0 = holder(c.b0); n = holder(c.b1 - 1) - c0 + 1;
+    }
+    void local_starts(const size_t* start, const HostChunk& c, u64* out) const
+    {
+        for (size_t i = 0; i < n; i++) out[i] = std::max(start[c0 + i], c.b0) - c.b0;
+        out[n] = c.b1 - c.b0;
+    }
+};
+
+// The chain compress, for cb blocks and nc chunk-local chains: source pointers, sizes, prefer flags (two per word) and chain starts
+// (nc + 1) go up; offsets (cb + 1), values and kinds (eight per word) come down.  The per-chain state views are ChainPool's at the
+// chunk's first chain.
+struct ChainCompressWords {
+    size_t ptr = 0, size, prefer, start, offset, value, kind, end;
+    ChainCompressWords(size_t cb, size_t nc) : size(cb), prefer(2 * cb), start(prefer + (cb + 1) / 2), offset(start + nc + 1),
+        value(offset + cb + 1), kind(value + cb), end(kind + (cb + 7) / 8) {}
+};
+// The chain decompress, for cb blocks, nc chunk-local chains and ne entry headers: destination pointers, sizes, offsets (cb + 1),
+// kinds, chain starts, the chains' entry header pointers and sizes, and ne header images of HDR_MAX bytes with a 32-byte sector
+// of slack behind them (the decoder reads whole sectors) go up; values come down.
+struct ChainDecompressWords {
+    size_t ptr = 0, size, offset, kind, start, hdr, hdrSize, hdrBytes, value, end;
+    ChainDecompressWords(size_t cb, size_t nc, size_t ne) : size(cb), offset(2 * cb), kind(3 * cb + 1), start(kind + (cb + 7) / 8),
+        hdr(start + nc + 1), hdrSize(hdr + nc), hdrBytes(hdrSize + nc), value(hdrBytes + ne * (HDR_MAX / 8) + 4), end(value + cb) {}
+};
+
+// A compress call's per-chain state on the device, in u64 words for nChains chains: the tables (256 cells, 1 KiB each), pointers
+// to them, the flags (two per word), the header pointers and the header sizes.  The device calls only carry a header pointer,
+// so those go up as 0, and the host derives the exit headers from the kinds.  `h` is its pinned host image: 32,768 chains take
+// 32 MiB each way, which pageable memory would copy at a fraction of the PCIe rate.  Grow-only, per device, used under the packed
+// ring's mutex.
+struct ChainPool {
+    struct Layout {
+        size_t table = 0, tptr, flag, hdr, hdrSize, end;
+        explicit Layout(size_t n) : tptr(128 * n), flag(129 * n), hdr(flag + (n + 1) / 2), hdrSize(hdr + n), end(hdrSize + n) {}
+    };
+    u64* d = nullptr;
+    u64* h = nullptr;
+    size_t cap = 0;
+    cudaError_t ensure(size_t words)
+    {
+        if (words <= cap) return cudaSuccess;
+        cudaError_t e = cudaSuccess;
+        if (d) e = cudaFree(d);
+        if (h && e == cudaSuccess) e = cudaFreeHost(h);
+        d = nullptr; h = nullptr; cap = 0;
+        if (e == cudaSuccess) e = cudaMalloc((void**)&d, words * sizeof(u64));
+        if (e == cudaSuccess) e = cudaMallocHost((void**)&h, words * sizeof(u64));
+        if (e == cudaSuccess) cap = words;
+        return e;
+    }
+};
+ChainPool& chain_pool() { static ChainPool p[MAX_DEVICES]; return p[current_device()]; }
+
+// one event per ring stream: chunk ci's chain call waits for chunk ci - 1's
+template <int NS>
+struct ChunkEvents {
+    cudaEvent_t ev[NS] = {};
+    cudaError_t create()
+    {
+        cudaError_t e = cudaSuccess;
+        for (int i = 0; i < NS && e == cudaSuccess; i++) e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming);
+        return e;
+    }
+    ~ChunkEvents() { for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x); }
+};
+
+// the header a chunk-local chain enters a decompress chunk with: `n` bytes at `p`
+struct EntryHeader { size_t chain; const u8* p; u64 n; };
+}
+
+FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                           void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
+                                                           unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
+                                                           const int* hPreferRepeat, unsigned* const* hCTables, int* hRepeats,
+                                                           const void** hChainHeaders, size_t* hChainHeaderSizes,
+                                                           unsigned maxSymbolValue, unsigned tableLog)
+{
+    if ((codec != 1 && codec != 3) || nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    if (nBlocks == 0) return 0;
+    if (!hChainStarts || !hOut || !hOffsets || !hCSizes || !hKinds || !hSrc || !hSrcSizes || !hPreferRepeat || !hCTables ||
+        !hRepeats || !hChainHeaders || !hChainHeaderSizes) return (size_t)err(E_SRC_WRONG);
+    if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
+        for (size_t b = 0; b < nBlocks; b++) { hCSizes[b] = (size_t)err(E_SRC_WRONG); hKinds[b] = 4; }
+        return 0;
+    }
+    auto const compress = codec == 1 ? FSEB200_HUF_compress4X_repeat_chains_packed : FSEB200_HUF_compress1X_repeat_chains_packed;
+    ChunkMax most;
+    std::vector<HostChunk> const chunks = cut_chunks(hSrcSizes, nBlocks, 1, [](size_t) { return (u64)0; }, most);
+    std::vector<ChunkChains> cc;
+    size_t words = 0;
+    for (const HostChunk& c : chunks) {
+        cc.emplace_back(hChainStarts, nChains, c);
+        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n).end);
+    }
+    auto& P = packed_ring();
+    std::lock_guard<std::mutex> lock(P.mu);
+    ChainPool& S = chain_pool();
+    ChainPool::Layout const SL(nChains);
+    ChunkEvents<Ring<3>::NS> ev;
+    cudaError_t e = P.ensure(most.bytes, most.bytes, 0, words, words);
+    if (e == cudaSuccess) e = S.ensure(SL.end);
+    if (e == cudaSuccess) e = ev.create();
+    // the caller's state up once, on the first chunk's stream, through the pool's pinned image, which also takes it back down
+    u64* const img = S.h;
+    int* const flags = reinterpret_cast<int*>(img + SL.flag);
+    if (e == cudaSuccess) {
+        std::fill(img + SL.flag, img + SL.end, (u64)0);
+        for (size_t c = 0; c < nChains; c++) {
+            std::memcpy(img + SL.table + 128 * c, hCTables[c], 1024);
+            img[SL.tptr + c] = reinterpret_cast<u64>(S.d + SL.table + 128 * c);
+            flags[c] = hRepeats[c];
+            img[SL.hdrSize + c] = hChainHeaderSizes[c];
+        }
+        e = cudaMemcpyAsync(S.d, img, SL.end * sizeof(u64), cudaMemcpyHostToDevice, P.st[0]);
+    }
+    // queue: the source and the descriptors up, then -- once chunk ci - 1's call has left the crossing chain's state -- the
+    // device call with room for every block on views of the state at the chunk's first chain, then offsets, values, kinds down
+    auto queue = [&](size_t ci, int k) -> cudaError_t {
+        const HostChunk& c = chunks[ci];
+        size_t const cb = c.b1 - c.b0, c0 = cc[ci].c0;
+        ChainCompressWords const L(cb, cc[ci].n);
+        u64 const bytes = c.a1 - c.a0;
+        cudaStream_t const s = P.st[k];
+        u64* const h = P.hD[k], * const d = P.dD[k];
+        for (size_t b = 0, a = 0; b < cb; b++) { h[L.ptr + b] = reinterpret_cast<u64>(P.dA[k] + a); h[L.size + b] = hSrcSizes[c.b0 + b]; a += hSrcSizes[c.b0 + b]; }
+        std::memcpy(h + L.prefer, hPreferRepeat + c.b0, cb * sizeof(int));
+        cc[ci].local_starts(hChainStarts, c, h + L.start);
+        cudaError_t r;
+        if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        if ((r = cudaMemcpyAsync(d, h, L.offset * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        if (ci && (r = cudaStreamWaitEvent(s, ev.ev[(ci - 1) % P.NS], 0)) != cudaSuccess) return r;
+        size_t const v = compress(cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
+                                  (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size),
+                                  (const int*)(d + L.prefer), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
+                                  (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, s);
+        if (v) return cudaErrorLaunchFailure;
+        if ((r = cudaEventRecord(ev.ev[k], s)) != cudaSuccess) return r;
+        return cudaMemcpyAsync(h + L.offset, d + L.offset, (L.end - L.offset) * sizeof(u64), cudaMemcpyDeviceToHost, s);
+    };
+    u64 total = 0;
+    auto finish = [&](size_t ci, int k) -> cudaError_t {
+        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n);
+        cudaError_t const r = cudaStreamSynchronize(P.st[k]);
+        if (r != cudaSuccess) return r;
+        return finish_packed(chunks[ci], P.hD[k] + L.offset, P.hD[k] + L.value, (const u8*)(P.hD[k] + L.kind), P.dB[k], P.st[k],
+                             (u8*)hOut, outCapacity, hOffsets, hCSizes, hKinds, total);
+    };
+    if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS - 1, queue, finish);
+    bool const fits = total <= outCapacity;
+    if (e == cudaSuccess && fits) e = cudaMemcpy(img, S.d, SL.hdr * sizeof(u64), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) return (size_t)err(E_GENERIC);
+    hOffsets[nBlocks] = (size_t)total;
+    // the state goes back only if the whole stream fits: the tables and flags the calls left, and the header of each chain's
+    // last kind-2 block, at its place in hOut, or the one it came in with
+    if (fits)
+        for (size_t c = 0; c < nChains; c++) {
+            std::memcpy(hCTables[c], img + SL.table + 128 * c, 1024);
+            hRepeats[c] = flags[c];
+            for (size_t j = hChainStarts[c + 1]; j-- > hChainStarts[c];)
+                if (hKinds[j] == 2) { hChainHeaders[c] = (const u8*)hOut + hOffsets[j]; hChainHeaderSizes[c] = hCSizes[j]; break; }
+        }
+    return 0;
+}
+
+FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                      void* hDst, const size_t* hDstSizes, size_t* hResults,
+                                                      const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
+                                                      const void* const* hChainHeaders, const size_t* hChainHeaderSizes)
+{
+    if ((codec != 1 && codec != 3) || nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    if (nBlocks == 0) return 0;
+    if (!hChainStarts || !hDst || !hDstSizes || !hResults || !hIn || !hOffsets || !hKinds || !hChainHeaders || !hChainHeaderSizes)
+        return (size_t)err(E_SRC_WRONG);
+    for (size_t b = 0; b < nBlocks; b++) if (hOffsets[b + 1] < hOffsets[b]) return (size_t)err(E_SRC_WRONG);
+    if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
+        for (size_t b = 0; b < nBlocks; b++) hResults[b] = (size_t)err(E_SRC_WRONG);
+        return 0;
+    }
+    auto const decompress = codec == 1 ? FSEB200_HUF_decompress4X_repeat_packed : FSEB200_HUF_decompress1X_repeat_packed;
+    ChunkMax most;
+    std::vector<HostChunk> const chunks = cut_chunks(hDstSizes, nBlocks, 1, [&](size_t b) { return (u64)(hOffsets[b + 1] - hOffsets[b]); }, most);
+    // The device decoder finds a kind-3 block's header in its chunk when a kind-2 block of its chain precedes it there.  Otherwise
+    // the chain's entry header is supplied: the chain's last kind-2 block before the chunk, or the caller's.  One walk over the
+    // blocks, with the chain that holds each block and that chain's last kind-2 block so far.
+    std::vector<ChunkChains> cc;
+    std::vector<std::vector<EntryHeader>> entries(chunks.size());
+    size_t words = 0;
+    for (size_t ci = 0, ch = 0, last2 = NONE; ci < chunks.size(); ci++) {
+        const HostChunk& c = chunks[ci];
+        cc.emplace_back(hChainStarts, nChains, c);
+        bool seen = false;                                          // chain ch has a kind-2 or kind-3 block in this chunk before b
+        for (size_t b = c.b0; b < c.b1; b++) {
+            while (hChainStarts[ch + 1] <= b) { ch++; last2 = NONE; seen = false; }
+            unsigned char const k = hKinds[b];
+            if (k == 3 && !seen)
+                entries[ci].push_back(last2 != NONE ? EntryHeader{ ch - cc[ci].c0, (const u8*)hIn + hOffsets[last2], hOffsets[last2 + 1] - hOffsets[last2] }
+                                                    : EntryHeader{ ch - cc[ci].c0, (const u8*)hChainHeaders[ch], hChainHeaderSizes[ch] });
+            seen |= k == 2 || k == 3;
+            if (k == 2) last2 = b;
+        }
+        words = std::max(words, ChainDecompressWords(c.b1 - c.b0, cc[ci].n, entries[ci].size()).end);
+    }
+    auto& P = packed_ring();
+    std::lock_guard<std::mutex> lock(P.mu);
+    cudaError_t e = P.ensure(most.bytes, most.packed, 0, words, words);
+    // queue: the chunk's packed bytes and descriptors up (offsets rebased to the chunk, entry headers as images of at most HDR_MAX
+    // bytes), the device decompress, the blocks and their values down
+    auto queue = [&](size_t ci, int k) -> cudaError_t {
+        const HostChunk& c = chunks[ci];
+        size_t const cb = c.b1 - c.b0;
+        ChainDecompressWords const L(cb, cc[ci].n, entries[ci].size());
+        u64 const in0 = hOffsets[c.b0], in = hOffsets[c.b1] - in0, bytes = c.a1 - c.a0;
+        cudaStream_t const s = P.st[k];
+        u64* const h = P.hD[k], * const d = P.dD[k];
+        for (size_t b = 0, a = 0; b < cb; b++) { h[L.ptr + b] = reinterpret_cast<u64>(P.dA[k] + a); h[L.size + b] = hDstSizes[c.b0 + b]; a += hDstSizes[c.b0 + b]; }
+        for (size_t b = 0; b <= cb; b++) h[L.offset + b] = hOffsets[c.b0 + b] - in0;
+        std::memcpy(h + L.kind, hKinds + c.b0, cb);
+        cc[ci].local_starts(hChainStarts, c, h + L.start);
+        std::fill(h + L.hdr, h + L.hdrBytes, (u64)0);
+        for (size_t j = 0; j < entries[ci].size(); j++) {
+            const EntryHeader& x = entries[ci][j];
+            u64 const n = std::min(x.n, HDR_MAX);
+            if (n) std::memcpy((u8*)(h + L.hdrBytes) + j * HDR_MAX, x.p, n);
+            h[L.hdr + x.chain] = reinterpret_cast<u64>((u8*)(d + L.hdrBytes) + j * HDR_MAX); h[L.hdrSize + x.chain] = n;
+        }
+        cudaError_t r;
+        if (in && (r = cudaMemcpyAsync(P.dB[k], (const u8*)hIn + in0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        if ((r = cudaMemcpyAsync(d, h, L.value * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
+        size_t const v = decompress(cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr), (const size_t*)(d + L.size),
+                                    (size_t*)(d + L.value), P.dB[k], (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind),
+                                    (const void* const*)(d + L.hdr), (const size_t*)(d + L.hdrSize), s);
+        if (v) return cudaErrorLaunchFailure;
+        if (bytes && (r = cudaMemcpyAsync((u8*)hDst + c.a0, P.dA[k], bytes, cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
+        return cudaMemcpyAsync(h + L.value, d + L.value, cb * sizeof(u64), cudaMemcpyDeviceToHost, s);
+    };
+    auto finish = [&](size_t ci, int k) -> cudaError_t {
+        const HostChunk& c = chunks[ci];
+        ChainDecompressWords const L(c.b1 - c.b0, cc[ci].n, entries[ci].size());
+        cudaError_t const r = cudaStreamSynchronize(P.st[k]);
+        if (r == cudaSuccess) std::memcpy(hResults + c.b0, P.hD[k] + L.value, (c.b1 - c.b0) * sizeof(u64));
         return r;
     };
     if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS, queue, finish);

@@ -445,6 +445,40 @@ size_t FSEB200_compress_host_packed(int codec, void* hOut, size_t outCapacity, s
 size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size_t* hDstSizes, size_t* hResults,
                                       const void* hIn, const size_t* hOffsets, size_t nBlocks);
 
+/* Tier 1b, packed chains of table reuse (Huff0) -- FSEB200_HUF_compress{4X,1X}_repeat_chains_packed and
+ * FSEB200_HUF_decompress{4X,1X}_repeat_packed on HOST buffers, so that a host program keeps its literal blocks and its streams'
+ * state in host memory and gets the stream it writes out (bytes, nBlocks + 1 offsets, nBlocks kinds) in one call.
+ * codec: 1 = Huff0 4X, 3 = Huff0 1X (the host packed numbering).  Synchronous.  All pointers are host pointers, pinned or pageable,
+ * with no alignment required: hChainStarts (nChains + 1 entries), the per-block arrays, the per-chain state -- hCTables[c] (256
+ * HUF_CElt cells), hRepeats[c], hChainHeaders[c] / hChainHeaderSizes[c] -- and every header.  Blocks lie back to back: block b of
+ * the source starts at hSrc + n_0 + ... + n_{b-1}, and decompress writes block b at the same place in hDst.
+ *   compress:   hCSizes, hKinds, hOffsets and hOut[0, min(total, outCapacity)) are byte for byte what the matching device call
+ *               gives for the same chains, the same entry state and the same outCapacity, and so is every table (all 256 cells),
+ *               flag and chain header on return; a header the device call would point at dOut + dOffsets[j] is hOut +
+ *               hOffsets[j] here.  Its rules carry over unchanged: the capacity rule, the state left as it came in when the total
+ *               does not fit, and for malformed chain geometry only srcSize_wrong values and kind 4, with no offset written.
+ *               Nothing outside the stored blocks is written to hOut; outCapacity = sum(n) always holds them all.
+ *   decompress: hResults equals the device call's for the same stream and entry headers; [0, result) of each block holds its
+ *               bytes.  Exactly [hIn + hOffsets[0], hIn + hOffsets[nBlocks]) of the stream is read, and of an entry header (one
+ *               that a kind-3 block of its chain needs) at most its first 128 bytes -- all a tree header can take.  Offsets that
+ *               decrease anywhere give srcSize_wrong; malformed chain geometry makes every result srcSize_wrong.
+ * The batch is cut into chunks by the packed host calls' byte budget (FSEB200_HOST_PACKED_CHUNK_BYTES), chain boundaries ignored,
+ * and each chunk runs the device call on its own part of the chains.  At most one chain crosses each chunk boundary: compress
+ * carries its state on the device from one chunk's call to the next, which waits for it while its copies still overlap, and
+ * decompress gives a chunk the crossing chain's last tree header from the stream before it.  The calls share the packed host
+ * calls' streams and are serialised per device with them and with the frame calls.
+ * Return value: 0 (also for nBlocks == 0, which writes nothing); srcSize_wrong, before any device work, for a bad codec, nBlocks or
+ * nChains above 0xFFFFFFFF, or a NULL pointer while nBlocks > 0; generic if a CUDA call fails. */
+size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                  void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds,
+                                                  const void* hSrc, const size_t* hSrcSizes, const int* hPreferRepeat,
+                                                  unsigned* const* hCTables, int* hRepeats, const void** hChainHeaders, size_t* hChainHeaderSizes,
+                                                  unsigned maxSymbolValue, unsigned tableLog);
+size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                             void* hDst, const size_t* hDstSizes, size_t* hResults,
+                                             const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
+                                             const void* const* hChainHeaders, const size_t* hChainHeaderSizes);
+
 /* Tier 1b, frames -- the self-describing .fse format of the reference's file tool (programs/fileio.c:266-626) on HOST buffers:
  *   frame   = LE32 magic (0x183E2309 FSE, 0x183E3309 Huff0), 1 byte block-size id (block = 1 KB << id, id <= 6),
  *             { block header, payload }*, 3-byte trailer
