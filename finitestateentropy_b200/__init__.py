@@ -76,6 +76,13 @@ def _declare(L):
         sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     for name in ("FSEB200_HUF_decompress4X_repeat_blocks", "FSEB200_HUF_decompress1X_repeat_blocks"):
         sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_HUF_compress_mixed_repeat_chains", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
+    sig("FSEB200_HUF_decompress_mixed_repeat_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_HUF_compress_mixed_repeat_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+        c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
+    sig("FSEB200_HUF_decompress_mixed_repeat_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+        c_vp)
     for name in ("FSEB200_HUF_compress_packed", "FSEB200_HUF_compress1X_packed"):
         sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     for codec in ("FSE", "FSEU16"):
@@ -91,6 +98,9 @@ def _declare(L):
     sig("FSEB200_compress_host_repeat_chains_packed", c_sz, C.c_int, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
         c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint)
     sig("FSEB200_decompress_host_repeat_packed", c_sz, C.c_int, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_compress_host_mixed_repeat_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint)
+    sig("FSEB200_decompress_host_mixed_repeat_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
     sig("FSEB200_frame_compressBound", c_sz, c_sz, C.c_uint)
     sig("FSEB200_frame_compress_host", c_sz, C.c_int, C.c_uint, c_vp, c_sz, c_vp, c_sz)
     sig("FSEB200_frame_decompress_bound", c_sz, c_vp, c_sz)
@@ -119,10 +129,13 @@ from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch
                     huf_compress_repeat_chains, huf_compress1x_repeat_chains,
                     huf_compress_repeat_chains_packed, huf_compress1x_repeat_chains_packed,
                     huf_decompress_repeat_packed, huf_decompress1x_repeat_packed,
+                    huf_compress_mixed_repeat_chains, huf_decompress_mixed_repeat_blocks,
+                    huf_compress_mixed_repeat_chains_packed, huf_decompress_mixed_repeat_packed,
                     huf_compress_packed, huf_compress1x_packed, packed_pointers,
                     fse_compress_blocks, fse_decompress_blocks, fseu16_compress_blocks, fseu16_decompress_blocks,
                     fse_compress_packed, fseu16_compress_packed, fse_decompress_packed, fseu16_decompress_packed,
                     fse_packed_workspace, huf_decompress_packed, huf_decompress1x_packed,
                     host_compress_packed, host_decompress_packed,
-                    host_compress_repeat_chains_packed, host_decompress_repeat_packed, frame_compress, frame_decompress,
+                    host_compress_repeat_chains_packed, host_decompress_repeat_packed,
+                    host_compress_mixed_repeat_chains_packed, host_decompress_mixed_repeat_packed, frame_compress, frame_decompress,
                     frame_compress_batch, frame_decompress_batch, frame_compress_device, frame_decompress_device)

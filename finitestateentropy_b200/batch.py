@@ -343,6 +343,110 @@ def _header_blocks(fn_name, csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs
     return results
 
 
+def _single_arg(single_stream, n, dev):
+    _check(single_stream, torch.uint8)
+    assert single_stream.numel() == n and single_stream.device == dev, (single_stream.numel(), n, single_stream.device)
+    return single_stream.data_ptr()
+
+
+def huf_compress_mixed_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, single_stream, ctables, repeats,
+                                     chain_hdr_ptrs, chain_hdr_sizes, csizes=None, hdr_ptrs=None, hdr_sizes=None, max_symbol_value=255,
+                                     table_log=12):
+    """huf_compress_repeat_chains with each block's form chosen by single_stream[b] (uint8): 0 HUF_compress4X_repeat, anything
+    else HUF_compress1X_repeat.  Both forms share the stream's table, flag and header.  Returns (csizes, hdr_ptrs, hdr_sizes),
+    as huf_decompress_mixed_repeat_blocks takes them with the same single_stream."""
+    from . import lib
+    n = src_ptrs.numel()
+    dev = src_ptrs.device
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    if hdr_ptrs is None:
+        hdr_ptrs = torch.empty(n, dtype=torch.int64, device=dev)
+    if hdr_sizes is None:
+        hdr_sizes = torch.empty(n, dtype=torch.int64, device=dev)
+    _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, hdr_ptrs, hdr_sizes)
+    _check(prefer, torch.int32)
+    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
+    single = _single_arg(single_stream, n, dev)
+    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
+                                               (chain_hdr_sizes, torch.int64)))
+    fn_name = "FSEB200_HUF_compress_mixed_repeat_chains"
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(),
+                                src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(), single, ctables.data_ptr(),
+                                repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(), hdr_ptrs.data_ptr(),
+                                hdr_sizes.data_ptr(), max_symbol_value, table_log, _stream_ptr())
+    _ret(r, fn_name)
+    return csizes, hdr_ptrs, hdr_sizes
+
+
+def huf_decompress_mixed_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, single_stream, results=None):
+    """huf_decompress_repeat_blocks (single_stream[b] == 0) or huf_decompress1x_repeat_blocks (otherwise) on every block b, in
+    one call on the current stream.  Returns results (int64)."""
+    from . import lib
+    if results is None:
+        results = torch.empty(csrc_ptrs.numel(), dtype=torch.int64, device=csrc_ptrs.device)
+    n = _blocks_args(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results, hdr_ptrs, hdr_sizes)
+    single = _single_arg(single_stream, n, csrc_ptrs.device)
+    fn_name = "FSEB200_HUF_decompress_mixed_repeat_blocks"
+    r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), csrc_ptrs.data_ptr(),
+                                csrc_sizes.data_ptr(), hdr_ptrs.data_ptr(), hdr_sizes.data_ptr(), single, _stream_ptr())
+    _ret(r, fn_name)
+    return results
+
+
+def huf_compress_mixed_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, single_stream, ctables, repeats, chain_hdr_ptrs,
+                                            chain_hdr_sizes, out=None, offsets=None, csizes=None, kinds=None, max_symbol_value=255,
+                                            table_log=12):
+    """huf_compress_repeat_chains_packed with each block's form chosen by single_stream[b] (uint8, 0 = 4X).  Kinds keep their
+    numbering whatever the form, so the stream is (out, offsets, kinds) plus single_stream.  Returns (out, offsets, csizes, kinds)."""
+    from . import lib
+    n = _blocks_args(src_ptrs, src_sizes)
+    dev = src_ptrs.device
+    _check(prefer, torch.int32)
+    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
+    single = _single_arg(single_stream, n, dev)
+    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
+                                               (chain_hdr_sizes, torch.int64)))
+    if out is None:
+        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
+    if offsets is None:
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    if kinds is None:
+        kinds = torch.empty(n, dtype=torch.uint8, device=dev)
+    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64); _check(kinds, torch.uint8)
+    assert offsets.numel() == n + 1 and csizes.numel() == n and kinds.numel() == n and out.device == dev, (offsets.numel(), n)
+    fn_name = "FSEB200_HUF_compress_mixed_repeat_chains_packed"
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, out.data_ptr(), out.numel(), offsets.data_ptr(),
+                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(),
+                                single, ctables.data_ptr(), repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(),
+                                max_symbol_value, table_log, _stream_ptr())
+    _ret(r, fn_name)
+    return out, offsets, csizes, kinds
+
+
+def huf_decompress_mixed_repeat_packed(chain_starts, packed, offsets, kinds, single_stream, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs,
+                                       dst_sizes, results=None):
+    """huf_decompress_repeat_packed over a buffer huf_compress_mixed_repeat_chains_packed wrote, each block in the form
+    single_stream[b] names.  Returns results (int64)."""
+    from . import lib
+    n = _blocks_args(dst_ptrs, dst_sizes)
+    dev = dst_ptrs.device
+    n_chains = _chain_args(chain_starts, dev, ((chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64)))
+    single = _single_arg(single_stream, n, dev)
+    if results is None:
+        results = torch.empty(n, dtype=torch.int64, device=dev)
+    _check(packed, torch.uint8); _check(offsets, torch.int64); _check(kinds, torch.uint8); _check(results, torch.int64)
+    assert offsets.numel() == n + 1 and kinds.numel() == n and results.numel() == n and packed.device == dev, (offsets.numel(), n)
+    fn_name = "FSEB200_HUF_decompress_mixed_repeat_packed"
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(),
+                                packed.data_ptr(), offsets.data_ptr(), kinds.data_ptr(), single, chain_hdr_ptrs.data_ptr(),
+                                chain_hdr_sizes.data_ptr(), _stream_ptr())
+    _ret(r, fn_name)
+    return results
+
+
 def huf_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, max_symbol_value=255, table_log=12):
     """HUF_compress2 on every block b (src_ptrs[b] / src_sizes[b]) at capacity HUF_compressBound, the results stored back to
     back in `out` (capacity out.numel()), on the current stream.  Returns (out, offsets, csizes): offsets (int64, n + 1 entries)
@@ -604,8 +708,23 @@ def host_compress_repeat_chains_packed(src, sizes, chain_starts, prefer, ctables
     allocated at sum(sizes) + 32 bytes if None, always enough), offsets, csizes and kinds are what the device call
     huf_compress_repeat_chains_packed gives.  Synchronous.  Returns (out, offsets, csizes, kinds, (ctables, repeats,
     chain_hdr_ptrs, chain_hdr_sizes))."""
+    return _host_chains_compress(HOST_CHAIN_CODECS[codec], None, src, sizes, chain_starts, prefer, ctables, repeats, chain_hdr_ptrs,
+                                 chain_hdr_sizes, out, max_symbol_value, table_log)
+
+
+def host_compress_mixed_repeat_chains_packed(src, sizes, chain_starts, prefer, single_stream, ctables, repeats, chain_hdr_ptrs,
+                                             chain_hdr_sizes, out=None, max_symbol_value=255, table_log=12):
+    """host_compress_repeat_chains_packed with each block's form chosen by single_stream[b] (a CPU uint8 tensor: 0 4X, else 1X),
+    byte for byte what huf_compress_mixed_repeat_chains_packed gives.  Synchronous.  Returns (out, offsets, csizes, kinds,
+    (ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes))."""
+    return _host_chains_compress(None, single_stream, src, sizes, chain_starts, prefer, ctables, repeats, chain_hdr_ptrs,
+                                 chain_hdr_sizes, out, max_symbol_value, table_log)
+
+
+def _host_chains_compress(cid, single, src, sizes, chain_starts, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, out,
+                          max_symbol_value, table_log):
+    """cid: the C codec of the 4X / 1X call, or None for the mixed call with the per-block forms `single`"""
     from . import lib
-    cid = HOST_CHAIN_CODECS[codec]
     sizes = _host_sizes(sizes)
     n = sizes.numel()
     _host_check(src, torch.uint8)
@@ -621,11 +740,19 @@ def host_compress_repeat_chains_packed(src, sizes, chain_starts, prefer, ctables
     csizes = torch.empty(n, dtype=torch.int64)
     kinds = torch.empty(n, dtype=torch.uint8)
     table_ptrs = torch.tensor([ctables.data_ptr() + 1024 * c for c in range(n_chains)], dtype=torch.int64)
-    r = lib().FSEB200_compress_host_repeat_chains_packed(
-        cid, n_chains, chain_starts.data_ptr(), n, _host_ptr(out), out.numel(), offsets.data_ptr(), _host_ptr(csizes), _host_ptr(kinds),
-        _host_ptr(src), _host_ptr(sizes), _host_ptr(prefer), _host_ptr(table_ptrs), _host_ptr(repeats), _host_ptr(chain_hdr_ptrs),
-        _host_ptr(chain_hdr_sizes), max_symbol_value, table_log)
-    _ret(r, "FSEB200_compress_host_repeat_chains_packed")
+    head = (n_chains, chain_starts.data_ptr(), n, _host_ptr(out), out.numel(), offsets.data_ptr(), _host_ptr(csizes), _host_ptr(kinds),
+            _host_ptr(src), _host_ptr(sizes), _host_ptr(prefer))
+    state = (_host_ptr(table_ptrs), _host_ptr(repeats), _host_ptr(chain_hdr_ptrs), _host_ptr(chain_hdr_sizes), max_symbol_value,
+             table_log)
+    if cid is None:
+        _host_check(single, torch.uint8)
+        assert single.numel() == n, (single.numel(), n)
+        fn_name = "FSEB200_compress_host_mixed_repeat_chains_packed"
+        r = getattr(lib(), fn_name)(*head, _host_ptr(single), *state)
+    else:
+        fn_name = "FSEB200_compress_host_repeat_chains_packed"
+        r = getattr(lib(), fn_name)(cid, *head, *state)
+    _ret(r, fn_name)
     return out, offsets, csizes, kinds, (ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes)
 
 
@@ -636,8 +763,20 @@ def host_decompress_repeat_packed(packed, offsets, kinds, chain_starts, dst_size
     `out` right after block b - 1.  chain_hdr_ptrs / chain_hdr_sizes (int64 CPU tensors, host addresses) are the headers the chains
     entered the compress with.  With out=None it is allocated at sum(dst_sizes) bytes.  results (int64) equals the device call
     huf_decompress_repeat_packed's.  Synchronous.  Returns (out, results)."""
+    return _host_chains_decompress(HOST_CHAIN_CODECS[codec], None, packed, offsets, kinds, chain_starts, dst_sizes, chain_hdr_ptrs,
+                                   chain_hdr_sizes, out, results)
+
+
+def host_decompress_mixed_repeat_packed(packed, offsets, kinds, single_stream, chain_starts, dst_sizes, chain_hdr_ptrs, chain_hdr_sizes,
+                                        out=None, results=None):
+    """host_decompress_repeat_packed over host_compress_mixed_repeat_chains_packed's stream, each block in the form single_stream[b]
+    (a CPU uint8 tensor) names; results equals huf_decompress_mixed_repeat_packed's.  Synchronous.  Returns (out, results)."""
+    return _host_chains_decompress(None, single_stream, packed, offsets, kinds, chain_starts, dst_sizes, chain_hdr_ptrs,
+                                   chain_hdr_sizes, out, results)
+
+
+def _host_chains_decompress(cid, single, packed, offsets, kinds, chain_starts, dst_sizes, chain_hdr_ptrs, chain_hdr_sizes, out, results):
     from . import lib
-    cid = HOST_CHAIN_CODECS[codec]
     dst_sizes = _host_sizes(dst_sizes)
     n = dst_sizes.numel()
     total = int(dst_sizes.sum())
@@ -650,10 +789,18 @@ def host_decompress_repeat_packed(packed, offsets, kinds, chain_starts, dst_size
         results = torch.empty(n, dtype=torch.int64)
     _host_check(out, torch.uint8); _host_check(results, torch.int64)
     assert out.numel() >= total and results.numel() == n, (out.numel(), total, results.numel(), n)
-    r = lib().FSEB200_decompress_host_repeat_packed(
-        cid, n_chains, chain_starts.data_ptr(), n, _host_ptr(out), _host_ptr(dst_sizes), _host_ptr(results), _host_ptr(packed),
-        offsets.data_ptr(), _host_ptr(kinds), _host_ptr(chain_hdr_ptrs), _host_ptr(chain_hdr_sizes))
-    _ret(r, "FSEB200_decompress_host_repeat_packed")
+    head = (n_chains, chain_starts.data_ptr(), n, _host_ptr(out), _host_ptr(dst_sizes), _host_ptr(results), _host_ptr(packed),
+            offsets.data_ptr(), _host_ptr(kinds))
+    tail = (_host_ptr(chain_hdr_ptrs), _host_ptr(chain_hdr_sizes))
+    if cid is None:
+        _host_check(single, torch.uint8)
+        assert single.numel() == n, (single.numel(), n)
+        fn_name = "FSEB200_decompress_host_mixed_repeat_packed"
+        r = getattr(lib(), fn_name)(*head, _host_ptr(single), *tail)
+    else:
+        fn_name = "FSEB200_decompress_host_repeat_packed"
+        r = getattr(lib(), fn_name)(cid, *head, *tail)
+    _ret(r, fn_name)
     return out, results
 
 

@@ -221,6 +221,19 @@ size_t huf_header_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstS
     });
 }
 }
+// Mixed forms: per block, the 4X or the 1X header decoder, as dSingleStream[b] names (0: 4X).
+FSEB_API size_t FSEB200_HUF_decompress_mixed_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                                          const void* const* dCSrcs, const size_t* dCSrcSizes, const void* const* dHeaders,
+                                                          const size_t* dHeaderSizes, const unsigned char* dSingleStream, void* stream)
+{
+    if (nBlocks && (!dHeaders || !dHeaderSizes || !dSingleStream)) return (size_t)err(E_SRC_WRONG);
+    return blocks_call(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, [&](const BlockDescs& d) {
+        HeaderDescs g;
+        static_cast<BlockDescs&>(g) = d;
+        g.hdr = (const u8* const*)dHeaders; g.hdrSize = (const u64*)dHeaderSizes;
+        return launch_huf_decode_headers_mixed(g, dSingleStream, (cudaStream_t)stream);
+    });
+}
 FSEB_API size_t FSEB200_HUF_compress4X_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
                                                      const void* const* dSrcs, const size_t* dSrcSizes, unsigned* const* dCTables, int* dRepeats,
                                                      const int* dPreferRepeat, unsigned maxSymbolValue, unsigned tableLog, void* stream)
@@ -240,17 +253,19 @@ namespace {
 size_t huf_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities,
                          size_t* dCSizes, const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
                          unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
-                         const void** dHeaders, size_t* dHeaderSizes, int nStreams, unsigned msv, unsigned tlog, void* stream)
+                         const void** dHeaders, size_t* dHeaderSizes, int nStreams, unsigned msv, unsigned tlog, void* stream,
+                         const unsigned char* dSingleStream = nullptr)           // nStreams 0: mixed, the form per block
 {
     if (nBlocks && (nChains > 0xFFFFFFFFull || !dChainStarts || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders ||
-                    !dChainHeaderSizes || !dHeaders || !dHeaderSizes)) return (size_t)err(E_SRC_WRONG);
+                    !dChainHeaderSizes || !dHeaders || !dHeaderSizes || (!nStreams && !dSingleStream))) return (size_t)err(E_SRC_WRONG);
     return blocks_call(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, [&](const BlockDescs& d) {
-        ChainDescs g;
+        ChainMixedDescs g;
         static_cast<BlockDescs&>(g) = d;
         g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
         g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.hdr = (const u8**)dChainHeaders; g.hdrSize = (u64*)dChainHeaderSizes;
-        g.blkHdr = (const u8**)dHeaders; g.blkHdrSize = (u64*)dHeaderSizes; g.fact = nullptr;
-        return launch_huf_encode_chains(g, nStreams, msv, tlog, (cudaStream_t)stream);
+        g.blkHdr = (const u8**)dHeaders; g.blkHdrSize = (u64*)dHeaderSizes; g.fact = nullptr; g.single = dSingleStream;
+        return nStreams ? launch_huf_encode_chains(g, nStreams, msv, tlog, (cudaStream_t)stream)
+                        : launch_huf_encode_chains_mixed(g, msv, tlog, (cudaStream_t)stream);
     });
 }
 }
@@ -274,6 +289,18 @@ FSEB_API size_t FSEB200_HUF_compress1X_repeat_chains(size_t nChains, const size_
     return huf_repeat_chains(nChains, dChainStarts, nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, dPreferRepeat, dCTables,
                              dRepeats, dChainHeaders, dChainHeaderSizes, dHeaders, dHeaderSizes, 1, maxSymbolValue, tableLog, stream);
 }
+FSEB_API size_t FSEB200_HUF_compress_mixed_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
+                                                         const size_t* dDstCapacities, size_t* dCSizes, const void* const* dSrcs,
+                                                         const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                         const unsigned char* dSingleStream, unsigned* const* dCTables,
+                                                         int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                         const void** dHeaders, size_t* dHeaderSizes, unsigned maxSymbolValue,
+                                                         unsigned tableLog, void* stream)
+{
+    return huf_repeat_chains(nChains, dChainStarts, nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, dPreferRepeat, dCTables,
+                             dRepeats, dChainHeaders, dChainHeaderSizes, dHeaders, dHeaderSizes, 0, maxSymbolValue, tableLog, stream,
+                             dSingleStream);
+}
 // Packed chains: the chain calls with every block stored back to back in one buffer and a kind byte per block
 // (common.cuh ChainPackedDescs), and the decoders of that buffer.
 namespace {
@@ -281,12 +308,13 @@ size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size
                                 size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs,
                                 const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats,
                                 const void** dChainHeaders, size_t* dChainHeaderSizes, int nStreams, unsigned msv, unsigned tlog,
-                                void* stream)
+                                void* stream, const unsigned char* dSingleStream = nullptr)   // nStreams 0: mixed, the form per block
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dOut || !dOffsets || !dCSizes || !dKinds || !dSrcs ||
-        !dSrcSizes || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes) return (size_t)err(E_SRC_WRONG);
-    ChainPackedDescs g;
+        !dSrcSizes || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes || (!nStreams && !dSingleStream))
+        return (size_t)err(E_SRC_WRONG);
+    ChainPackedMixedDescs g;
     g.dst = nullptr; g.dstCap = nullptr; g.result = (u64*)dCSizes; g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes;
     g.nBlocks = (u32)nBlocks;
     g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
@@ -294,20 +322,23 @@ size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size
     g.blkHdr = nullptr; g.blkHdrSize = nullptr; g.fact = nullptr;
     g.pk.out = (u8*)dOut; g.pk.outCap = outCapacity; g.pk.offset = (u64*)dOffsets; g.pk.result = g.result;
     g.pk.src = g.src; g.pk.srcSize = g.srcSize; g.pk.nBlocks = g.nBlocks;
-    g.kind = dKinds; g.end = nullptr; g.malformed = nullptr;
-    return ok_or_generic(launch_huf_encode_chains_packed(g, nStreams, msv, tlog, (cudaStream_t)stream));
+    g.kind = dKinds; g.end = nullptr; g.malformed = nullptr; g.single = dSingleStream;
+    return ok_or_generic(nStreams ? launch_huf_encode_chains_packed(g, nStreams, msv, tlog, (cudaStream_t)stream)
+                                  : launch_huf_encode_chains_packed_mixed(g, msv, tlog, (cudaStream_t)stream));
 }
 size_t huf_repeat_unpack(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstSizes,
                          size_t* dResults, const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
-                         const void* const* dChainHeaders, const size_t* dChainHeaderSizes, int nStreams, void* stream)
+                         const void* const* dChainHeaders, const size_t* dChainHeaderSizes, int nStreams, void* stream,
+                         const unsigned char* dSingleStream = nullptr)           // nStreams 0: mixed, the form per block
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dDsts || !dDstSizes || !dResults || !dIn ||
-        !dOffsets || !dKinds || !dChainHeaders || !dChainHeaderSizes) return (size_t)err(E_SRC_WRONG);
+        !dOffsets || !dKinds || !dChainHeaders || !dChainHeaderSizes || (!nStreams && !dSingleStream)) return (size_t)err(E_SRC_WRONG);
     return ok_or_generic(launch_huf_decompress_repeat_packed((const u64*)dChainStarts, (u32)nChains, (u8* const*)dDsts,
                                                              (const u64*)dDstSizes, (u64*)dResults, (const u8*)dIn,
                                                              (const u64*)dOffsets, dKinds, (const u8* const*)dChainHeaders,
-                                                             (const u64*)dChainHeaderSizes, (u32)nBlocks, nStreams, (cudaStream_t)stream));
+                                                             (const u64*)dChainHeaderSizes, (u32)nBlocks, nStreams, (cudaStream_t)stream,
+                                                             dSingleStream));
 }
 }
 FSEB_API size_t FSEB200_HUF_compress4X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
@@ -343,6 +374,25 @@ FSEB_API size_t FSEB200_HUF_decompress1X_repeat_packed(size_t nChains, const siz
 {
     return huf_repeat_unpack(nChains, dChainStarts, nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, dKinds, dChainHeaders,
                              dChainHeaderSizes, 1, stream);
+}
+FSEB_API size_t FSEB200_HUF_compress_mixed_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
+                                                                size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                                const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                                const unsigned char* dSingleStream, unsigned* const* dCTables, int* dRepeats,
+                                                                const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                                unsigned maxSymbolValue, unsigned tableLog, void* stream)
+{
+    return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 0, maxSymbolValue, tableLog, stream,
+                                    dSingleStream);
+}
+FSEB_API size_t FSEB200_HUF_decompress_mixed_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
+                                                           const size_t* dDstSizes, size_t* dResults, const void* dIn, const size_t* dOffsets,
+                                                           const unsigned char* dKinds, const unsigned char* dSingleStream,
+                                                           const void* const* dChainHeaders, const size_t* dChainHeaderSizes, void* stream)
+{
+    return huf_repeat_unpack(nChains, dChainStarts, nBlocks, dDsts, dDstSizes, dResults, dIn, dOffsets, dKinds, dChainHeaders,
+                             dChainHeaderSizes, 0, stream, dSingleStream);
 }
 FSEB_API size_t FSEB200_HUF_decompress4X_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                                        const void* const* dCSrcs, const size_t* dCSrcSizes, const void* const* dHeaders,

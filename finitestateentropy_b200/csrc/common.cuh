@@ -182,6 +182,18 @@ struct ChainPackedDescs : ChainDescs {
 __device__ __forceinline__ u64 enc_cap(const ChainPackedDescs& g, u32 b) { return huf_bound(enc_len(g, b)); }
 __device__ __forceinline__ u8* enc_dst(const ChainPackedDescs& g, u8*, u32 b) { return g.pk.out + g.pk.offset[b]; }   // after placement
 
+// Mixed chains: ChainDescs or ChainPackedDescs whose blocks each choose their form -- single[b] == 0: HUF_compress4X_repeat,
+// anything else: HUF_compress1X_repeat.  The kernels run them as stream mode 0 (huf_encode.cu); every other rule is the base's.
+template <class Base>
+struct Mixed : Base {
+    const u8* single;              // per block
+};
+using ChainMixedDescs = Mixed<ChainDescs>;
+using ChainPackedMixedDescs = Mixed<ChainPackedDescs>;
+// block b's form: true for one stream.  Only mixed geometry has a choice.
+template <class Geo> __device__ __forceinline__ bool enc_single(const Geo&, u32) { return false; }
+template <class Base> __device__ __forceinline__ bool enc_single(const Mixed<Base>& g, u32 b) { return g.single[b] != 0; }
+
 // decoder: compressed source, its size, the output, the regenerated size, the result; `orig` (stored blocks) is uniform-only
 __device__ __forceinline__ const u8* dec_src(const BatchGeom& g, const u8* cbuf, u32 b) { return cbuf + (u64)b * g.slot; }
 __device__ __forceinline__ u64 dec_csize(const BatchGeom&, const u64* csizes, u32 b) { return csizes[b]; }

@@ -393,7 +393,7 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
 // chunk runs the device call unchanged on chunk-local geometry.  Chains are contiguous ranges of blocks, so the chains that meet
 // a chunk are a contiguous range of which only the first can have started in an earlier chunk: at most one chain crosses each
 // chunk boundary, and its state (compress) or its last tree header (decompress) is all that passes from chunk to chunk.
-// codec: 1 = Huff0 4X, 3 = Huff0 1X.
+// codec: 1 = Huff0 4X, 3 = Huff0 1X; the mixed pair (a form per block, hSingleStream) runs the same code as codec 0.
 // ================================================================================================
 namespace {
 // The most of a tree header a Huff0 decoder reads (HUF_readStats: 1 + 127 bytes in the FSE form, 1 + 64 raw); a header's size
@@ -425,21 +425,22 @@ struct ChunkChains {
     }
 };
 
-// The chain compress, for cb blocks and nc chunk-local chains: source pointers, sizes, prefer flags (two per word) and chain starts
-// (nc + 1) go up; offsets (cb + 1), values and kinds (eight per word) come down.  The per-chain state views are ChainPool's at the
-// chunk's first chain.
+// The chain compress, for cb blocks and nc chunk-local chains: source pointers, sizes, prefer flags (two per word), chain starts
+// (nc + 1) and, for the mixed call, the blocks' forms (eight per word) go up; offsets (cb + 1), values and kinds (eight per word)
+// come down.  The per-chain state views are ChainPool's at the chunk's first chain.
 struct ChainCompressWords {
-    size_t ptr = 0, size, prefer, start, offset, value, kind, end;
-    ChainCompressWords(size_t cb, size_t nc) : size(cb), prefer(2 * cb), start(prefer + (cb + 1) / 2), offset(start + nc + 1),
-        value(offset + cb + 1), kind(value + cb), end(kind + (cb + 7) / 8) {}
+    size_t ptr = 0, size, prefer, start, single, offset, value, kind, end;
+    ChainCompressWords(size_t cb, size_t nc, bool mixed) : size(cb), prefer(2 * cb), start(prefer + (cb + 1) / 2), single(start + nc + 1),
+        offset(single + (mixed ? (cb + 7) / 8 : 0)), value(offset + cb + 1), kind(value + cb), end(kind + (cb + 7) / 8) {}
 };
 // The chain decompress, for cb blocks, nc chunk-local chains and ne entry headers: destination pointers, sizes, offsets (cb + 1),
-// kinds, chain starts, the chains' entry header pointers and sizes, and ne header images of HDR_MAX bytes with a 32-byte sector
-// of slack behind them (the decoder reads whole sectors) go up; values come down.
+// kinds, chain starts, the chains' entry header pointers and sizes, ne header images of HDR_MAX bytes with a 32-byte sector of
+// slack behind them (the decoder reads whole sectors) and, for the mixed call, the blocks' forms go up; values come down.
 struct ChainDecompressWords {
-    size_t ptr = 0, size, offset, kind, start, hdr, hdrSize, hdrBytes, value, end;
-    ChainDecompressWords(size_t cb, size_t nc, size_t ne) : size(cb), offset(2 * cb), kind(3 * cb + 1), start(kind + (cb + 7) / 8),
-        hdr(start + nc + 1), hdrSize(hdr + nc), hdrBytes(hdrSize + nc), value(hdrBytes + ne * (HDR_MAX / 8) + 4), end(value + cb) {}
+    size_t ptr = 0, size, offset, kind, start, hdr, hdrSize, hdrBytes, single, value, end;
+    ChainDecompressWords(size_t cb, size_t nc, size_t ne, bool mixed) : size(cb), offset(2 * cb), kind(3 * cb + 1), start(kind + (cb + 7) / 8),
+        hdr(start + nc + 1), hdrSize(hdr + nc), hdrBytes(hdrSize + nc), single(hdrBytes + ne * (HDR_MAX / 8) + 4),
+        value(single + (mixed ? (cb + 7) / 8 : 0)), end(value + cb) {}
 };
 
 // A compress call's per-chain state on the device, in u64 words for nChains chains: the tables (256 cells, 1 KiB each), pointers
@@ -487,17 +488,18 @@ struct ChunkEvents {
 struct EntryHeader { size_t chain; const u8* p; u64 n; };
 }
 
-FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
-                                                           void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
-                                                           unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
-                                                           const int* hPreferRepeat, unsigned* const* hCTables, int* hRepeats,
-                                                           const void** hChainHeaders, size_t* hChainHeaderSizes,
-                                                           unsigned maxSymbolValue, unsigned tableLog)
+namespace {
+// codec 1 (4X), 3 (1X) or 0 (mixed: the form of block b from hSingle[b])
+size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hOut, size_t outCapacity,
+                            size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
+                            const int* hPreferRepeat, const unsigned char* hSingle, unsigned* const* hCTables, int* hRepeats,
+                            const void** hChainHeaders, size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog)
 {
-    if ((codec != 1 && codec != 3) || nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    bool const mixed = codec == 0;
+    if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
     if (nBlocks == 0) return 0;
     if (!hChainStarts || !hOut || !hOffsets || !hCSizes || !hKinds || !hSrc || !hSrcSizes || !hPreferRepeat || !hCTables ||
-        !hRepeats || !hChainHeaders || !hChainHeaderSizes) return (size_t)err(E_SRC_WRONG);
+        !hRepeats || !hChainHeaders || !hChainHeaderSizes || (mixed && !hSingle)) return (size_t)err(E_SRC_WRONG);
     if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
         for (size_t b = 0; b < nBlocks; b++) { hCSizes[b] = (size_t)err(E_SRC_WRONG); hKinds[b] = 4; }
         return 0;
@@ -509,7 +511,7 @@ FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nCh
     size_t words = 0;
     for (const HostChunk& c : chunks) {
         cc.emplace_back(hChainStarts, nChains, c);
-        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n).end);
+        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n, mixed).end);
     }
     auto& P = packed_ring();
     std::lock_guard<std::mutex> lock(P.mu);
@@ -537,28 +539,35 @@ FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nCh
     auto queue = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
         size_t const cb = c.b1 - c.b0, c0 = cc[ci].c0;
-        ChainCompressWords const L(cb, cc[ci].n);
+        ChainCompressWords const L(cb, cc[ci].n, mixed);
         u64 const bytes = c.a1 - c.a0;
         cudaStream_t const s = P.st[k];
         u64* const h = P.hD[k], * const d = P.dD[k];
         for (size_t b = 0, a = 0; b < cb; b++) { h[L.ptr + b] = reinterpret_cast<u64>(P.dA[k] + a); h[L.size + b] = hSrcSizes[c.b0 + b]; a += hSrcSizes[c.b0 + b]; }
         std::memcpy(h + L.prefer, hPreferRepeat + c.b0, cb * sizeof(int));
         cc[ci].local_starts(hChainStarts, c, h + L.start);
+        if (mixed) std::memcpy(h + L.single, hSingle + c.b0, cb);
         cudaError_t r;
         if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if ((r = cudaMemcpyAsync(d, h, L.offset * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if (ci && (r = cudaStreamWaitEvent(s, ev.ev[(ci - 1) % P.NS], 0)) != cudaSuccess) return r;
-        size_t const v = compress(cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
-                                  (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size),
-                                  (const int*)(d + L.prefer), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
-                                  (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, s);
+        size_t const v = mixed
+            ? FSEB200_HUF_compress_mixed_repeat_chains_packed(
+                  cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
+                  (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size), (const int*)(d + L.prefer),
+                  (const unsigned char*)(d + L.single), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
+                  (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, s)
+            : compress(cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
+                       (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size),
+                       (const int*)(d + L.prefer), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
+                       (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, s);
         if (v) return cudaErrorLaunchFailure;
         if ((r = cudaEventRecord(ev.ev[k], s)) != cudaSuccess) return r;
         return cudaMemcpyAsync(h + L.offset, d + L.offset, (L.end - L.offset) * sizeof(u64), cudaMemcpyDeviceToHost, s);
     };
     u64 total = 0;
     auto finish = [&](size_t ci, int k) -> cudaError_t {
-        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n);
+        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n, mixed);
         cudaError_t const r = cudaStreamSynchronize(P.st[k]);
         if (r != cudaSuccess) return r;
         return finish_packed(chunks[ci], P.hD[k] + L.offset, P.hD[k] + L.value, (const u8*)(P.hD[k] + L.kind), P.dB[k], P.st[k],
@@ -581,15 +590,16 @@ FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nCh
     return 0;
 }
 
-FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
-                                                      void* hDst, const size_t* hDstSizes, size_t* hResults,
-                                                      const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
-                                                      const void* const* hChainHeaders, const size_t* hChainHeaderSizes)
+// codec 1 (4X), 3 (1X) or 0 (mixed: the form of block b from hSingle[b])
+size_t host_chains_decompress(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hDst, const size_t* hDstSizes,
+                              size_t* hResults, const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
+                              const unsigned char* hSingle, const void* const* hChainHeaders, const size_t* hChainHeaderSizes)
 {
-    if ((codec != 1 && codec != 3) || nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
+    bool const mixed = codec == 0;
+    if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
     if (nBlocks == 0) return 0;
-    if (!hChainStarts || !hDst || !hDstSizes || !hResults || !hIn || !hOffsets || !hKinds || !hChainHeaders || !hChainHeaderSizes)
-        return (size_t)err(E_SRC_WRONG);
+    if (!hChainStarts || !hDst || !hDstSizes || !hResults || !hIn || !hOffsets || !hKinds || !hChainHeaders || !hChainHeaderSizes ||
+        (mixed && !hSingle)) return (size_t)err(E_SRC_WRONG);
     for (size_t b = 0; b < nBlocks; b++) if (hOffsets[b + 1] < hOffsets[b]) return (size_t)err(E_SRC_WRONG);
     if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
         for (size_t b = 0; b < nBlocks; b++) hResults[b] = (size_t)err(E_SRC_WRONG);
@@ -617,7 +627,7 @@ FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains,
             seen |= k == 2 || k == 3;
             if (k == 2) last2 = b;
         }
-        words = std::max(words, ChainDecompressWords(c.b1 - c.b0, cc[ci].n, entries[ci].size()).end);
+        words = std::max(words, ChainDecompressWords(c.b1 - c.b0, cc[ci].n, entries[ci].size(), mixed).end);
     }
     auto& P = packed_ring();
     std::lock_guard<std::mutex> lock(P.mu);
@@ -627,7 +637,7 @@ FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains,
     auto queue = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
         size_t const cb = c.b1 - c.b0;
-        ChainDecompressWords const L(cb, cc[ci].n, entries[ci].size());
+        ChainDecompressWords const L(cb, cc[ci].n, entries[ci].size(), mixed);
         u64 const in0 = hOffsets[c.b0], in = hOffsets[c.b1] - in0, bytes = c.a1 - c.a0;
         cudaStream_t const s = P.st[k];
         u64* const h = P.hD[k], * const d = P.dD[k];
@@ -642,25 +652,74 @@ FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains,
             if (n) std::memcpy((u8*)(h + L.hdrBytes) + j * HDR_MAX, x.p, n);
             h[L.hdr + x.chain] = reinterpret_cast<u64>((u8*)(d + L.hdrBytes) + j * HDR_MAX); h[L.hdrSize + x.chain] = n;
         }
+        if (mixed) std::memcpy(h + L.single, hSingle + c.b0, cb);
         cudaError_t r;
         if (in && (r = cudaMemcpyAsync(P.dB[k], (const u8*)hIn + in0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if ((r = cudaMemcpyAsync(d, h, L.value * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-        size_t const v = decompress(cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr), (const size_t*)(d + L.size),
-                                    (size_t*)(d + L.value), P.dB[k], (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind),
-                                    (const void* const*)(d + L.hdr), (const size_t*)(d + L.hdrSize), s);
+        size_t const v = mixed
+            ? FSEB200_HUF_decompress_mixed_repeat_packed(cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr),
+                                                         (const size_t*)(d + L.size), (size_t*)(d + L.value), P.dB[k],
+                                                         (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind),
+                                                         (const unsigned char*)(d + L.single), (const void* const*)(d + L.hdr),
+                                                         (const size_t*)(d + L.hdrSize), s)
+            : decompress(cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr), (const size_t*)(d + L.size),
+                         (size_t*)(d + L.value), P.dB[k], (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind),
+                         (const void* const*)(d + L.hdr), (const size_t*)(d + L.hdrSize), s);
         if (v) return cudaErrorLaunchFailure;
         if (bytes && (r = cudaMemcpyAsync((u8*)hDst + c.a0, P.dA[k], bytes, cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
         return cudaMemcpyAsync(h + L.value, d + L.value, cb * sizeof(u64), cudaMemcpyDeviceToHost, s);
     };
     auto finish = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
-        ChainDecompressWords const L(c.b1 - c.b0, cc[ci].n, entries[ci].size());
+        ChainDecompressWords const L(c.b1 - c.b0, cc[ci].n, entries[ci].size(), mixed);
         cudaError_t const r = cudaStreamSynchronize(P.st[k]);
         if (r == cudaSuccess) std::memcpy(hResults + c.b0, P.hD[k] + L.value, (c.b1 - c.b0) * sizeof(u64));
         return r;
     };
     if (e == cudaSuccess) e = run_chunks(P, chunks.size(), P.NS, queue, finish);
     return e == cudaSuccess ? 0 : (size_t)err(E_GENERIC);
+}
+}  // namespace
+
+FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                           void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
+                                                           unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
+                                                           const int* hPreferRepeat, unsigned* const* hCTables, int* hRepeats,
+                                                           const void** hChainHeaders, size_t* hChainHeaderSizes,
+                                                           unsigned maxSymbolValue, unsigned tableLog)
+{
+    if (codec != 1 && codec != 3) return (size_t)err(E_SRC_WRONG);
+    return host_chains_compress(codec, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
+                                hPreferRepeat, nullptr, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue, tableLog);
+}
+FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                      void* hDst, const size_t* hDstSizes, size_t* hResults,
+                                                      const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
+                                                      const void* const* hChainHeaders, const size_t* hChainHeaderSizes)
+{
+    if (codec != 1 && codec != 3) return (size_t)err(E_SRC_WRONG);
+    return host_chains_decompress(codec, nChains, hChainStarts, nBlocks, hDst, hDstSizes, hResults, hIn, hOffsets, hKinds, nullptr,
+                                  hChainHeaders, hChainHeaderSizes);
+}
+FSEB_API size_t FSEB200_compress_host_mixed_repeat_chains_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                                 void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
+                                                                 unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
+                                                                 const int* hPreferRepeat, const unsigned char* hSingleStream,
+                                                                 unsigned* const* hCTables, int* hRepeats, const void** hChainHeaders,
+                                                                 size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog)
+{
+    return host_chains_compress(0, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
+                                hPreferRepeat, hSingleStream, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue,
+                                tableLog);
+}
+FSEB_API size_t FSEB200_decompress_host_mixed_repeat_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hDst,
+                                                            const size_t* hDstSizes, size_t* hResults, const void* hIn,
+                                                            const size_t* hOffsets, const unsigned char* hKinds,
+                                                            const unsigned char* hSingleStream, const void* const* hChainHeaders,
+                                                            const size_t* hChainHeaderSizes)
+{
+    return host_chains_decompress(0, nChains, hChainStarts, nBlocks, hDst, hDstSizes, hResults, hIn, hOffsets, hKinds, hSingleStream,
+                                  hChainHeaders, hChainHeaderSizes);
 }
 
 // ================================================================================================

@@ -48,12 +48,15 @@ struct __align__(16) Plan {        // per block, in global scratch
     u32 ctable[256];               // val | nbBits << 16
     u8  header[136];
     u32 hSize;
-    u32 state;                     // 0 = emit, 1 = verdict is final (nothing to emit)
+    u32 state;                     // PLAN_EMIT, PLAN_FINAL (the verdict is final: nothing to emit) or PLAN_EMIT_1X
     u32 total;                     // compressed size when state == 0
     u32 streamOff[4];              // byte offset of each stream from the start of the block
     u32 streamBytes[4];
     u16 segCount[4][256];          // plan kernel only: per-segment histograms (a segment count is <= HUF_BLOCK_MAX / 4 = 32768)
 };
+// Plan::state.  A mixed chain call runs two emit launches, 4X and 1X; a 1X block of such a call is PLAN_EMIT_1X, so the 4X launch
+// passes it by as it passes a final verdict, and the 1X launch (the Emit1X view) passes by everything else.
+enum : u32 { PLAN_EMIT = 0, PLAN_FINAL = 1, PLAN_EMIT_1X = 2 };
 
 // ---------------------------------------------------------------------------------------------
 // kernel 1: statistics, code table, tree header, stream sizes, verdict -- one CTA per group of 32 blocks
@@ -144,6 +147,17 @@ __device__ __forceinline__ bool plan_streams(Plan& P, const u32 (&cell)[8], Coun
     return true;
 }
 
+// Stream mode NS: 4 or 1 streams per block, or 0 (mixed chains): per block, the form enc_single names.  by_form calls f with the
+// block's stream count as a Form; under mode 0 that is a warp-uniform branch, since one warp owns one block at a time in both
+// kernels that call it.
+template <int S> using Form = std::integral_constant<int, S>;
+template <int NS, class F>
+__device__ __forceinline__ auto by_form(bool single, F f)
+{
+    if constexpr (NS == 0) return single ? f(Form<1>{}) : f(Form<4>{});
+    else return f(Form<NS>{});
+}
+
 // HUF_estimateCompressedSize (huf_compress.c:422-430) of the table whose cells the lane holds as above, in bits before its >> 3,
 // from the block's counts cnt[i] of symbols i * 32 + lane
 __device__ __forceinline__ u32 estimate_bits(const u32 (&cell)[8], const u32 (&cnt)[8])
@@ -232,18 +246,19 @@ __device__ __forceinline__ void warp_hist4_pipelined(u32 (*count4)[256], const u
 // the argument verdict or the histogram exit that would apply (and keeps the counts either way: prefer + valid skips the exits),
 // phase 2 builds every tree the exits leave, phase 3 plans the block with its new table.  huf_chain_kernel then decides.
 // Geo = ChainPackedDescs: the same, at capacities HUF_compressBound(srcSize).
+// Mixed chains (common.cuh Mixed): NS = 0, and phase 3 plans each block in the form its flag names.
 template <class Geo, int NS>
 __global__ void __launch_bounds__(32 * PLAN_WARPS, 3)
 huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8* __restrict__ src,
                 unsigned msvReq, unsigned tlogReq, Plan* __restrict__ plans)
 {
-    static_assert(NS == 4 || NS == 1, "4X or 1X");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PlanCta& S = *reinterpret_cast<PlanCta*>(smem_raw);
     unsigned const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     u32 const b0 = blockIdx.x * GROUP;
     constexpr bool REP = std::is_same_v<Geo, RepeatDescs>;
-    constexpr bool CHAIN = std::is_base_of_v<ChainDescs, Geo>;                              // ChainDescs or ChainPackedDescs
+    constexpr bool CHAIN = std::is_base_of_v<ChainDescs, Geo>;                              // ChainDescs or ChainPackedDescs, or mixed
+    static_assert(NS == 4 || NS == 1 || (NS == 0 && CHAIN), "4X, 1X, or mixed chains");
 #define FSEB_FINAL(v) { if (lane == 0) {                                                                            \
         if constexpr (CHAIN) { g.fact[b].kind = CF_ARGS; g.fact[b].exitValue = (v); }                                  \
         else { P.state = 1; enc_out(g, csizes, b) = (v); }                                                             \
@@ -418,9 +433,9 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         u64 const cap = enc_cap(g, b);
         Plan& P = plans[b];
         u64 hs = S.res[c];
-        auto const count = [&](int k, u32 i) {
+        auto const count = [&](auto form, int k, u32 i) {
             u32 const sy = i * 32 + lane;                                    // 1X: the four segment counts of a symbol add up to its block count
-            return (NS == 4) ? (u32)P.segCount[k][sy] : (u32)P.segCount[0][sy] + P.segCount[1][sy] + P.segCount[2][sy] + P.segCount[3][sy];
+            return (decltype(form)::value == 4) ? (u32)P.segCount[k][sy] : (u32)P.segCount[0][sy] + P.segCount[1][sy] + P.segCount[2][sy] + P.segCount[3][sy];
         };
         auto const new_cells = [&](u32 (&cell)[8]) {
             u32 const msv = S.msv[c];
@@ -434,6 +449,9 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
         const u8* const hdr = reinterpret_cast<const u8*>(&S.nd[0][0] + c * HDR_STRIDE);
         u32 cell[8];
         u64 total;
+        auto const plan = [&](auto form) {                                   // plan_streams in the block's form
+            return plan_streams<decltype(form)::value>(P, cell, [&](int k, u32 i) { return count(form, k, i); }, hdr, hs, cap, n, lane, total);
+        };
         if constexpr (CHAIN) {                   // the plan with the new table (its cells also for saving it), its verdict and estimate
             ChainFact& F = g.fact[b];
             if (lane == 0) F.hSize = hs;
@@ -441,7 +459,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
             u32 sum[8];
             new_cells(cell);
             block_counts(sum);
-            bool const ok = plan_streams<NS>(P, cell, count, hdr, hs, cap, n, lane, total);
+            bool const ok = by_form<NS>(enc_single(g, b), plan);
             if (!ok) {
                 #pragma unroll
                 for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = cell[i];
@@ -478,7 +496,7 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
                 for (u32 i = 0; i < 8; i++) cell[i] = g.ctable[b][i * 32 + lane] & 0xFFFFFFu;      // byte 3 is padding
             }
         } else new_cells(cell);
-        if (!plan_streams<NS>(P, cell, count, hdr, hs, cap, n, lane, total)) FSEB_FINAL(0);
+        if (!by_form<NS>(enc_single(g, b), plan)) FSEB_FINAL(0);
         if (lane == 0) { P.state = 0; enc_out(g, csizes, b) = total; }
     }
 #undef FSEB_FINAL
@@ -511,8 +529,11 @@ struct ChainBlock {                // what the decision for one block reads
     u32 n;
     int prefer;
 };
-template <class Geo>
-__device__ __forceinline__ void chain_load(const Geo& g, const Plan* plans, u32 b, ChainBlock& x, unsigned lane)
+struct ChainBlockMixed : ChainBlock {
+    bool single;                   // the block's form (mixed chains)
+};
+template <class Geo, class Blk>
+__device__ __forceinline__ void chain_load(const Geo& g, const Plan* plans, u32 b, Blk& x, unsigned lane)
 {
     x.f = g.fact[b];
     const Plan& P = plans[b];      // read whatever the kind: a plan the block did not fill is never used
@@ -522,20 +543,48 @@ __device__ __forceinline__ void chain_load(const Geo& g, const Plan* plans, u32 
         for (u32 i = 0; i < 8; i++) x.cnt[k][i] = P.segCount[k][i * 32 + lane];
     #pragma unroll
     for (u32 i = 0; i < 8; i++) x.cell[i] = P.ctable[i * 32 + lane];
-    if constexpr (std::is_same_v<Geo, ChainDescs>) x.dst = enc_dst(g, nullptr, b);
+    if constexpr (std::is_same_v<Geo, ChainDescs> || std::is_same_v<Geo, ChainMixedDescs>) x.dst = enc_dst(g, nullptr, b);
     else x.dst = nullptr;                                                                   // packed: no place yet, and none needed
     x.cap = enc_cap(g, b); x.n = enc_len(g, b); x.prefer = g.prefer[b];
+    if constexpr (std::is_same_v<Blk, ChainBlockMixed>) x.single = enc_single(g, b);
+}
+
+// HUF_compressCTable_internal with the chain's table T (cells, byte 3 cleared) in the S-stream form: the 4X size tests
+// (huf_compress.c:564-565), the capacity rule and the final test (:625).  The block's value, 0 or the size, goes to r; a size comes
+// with its plan (the cells, hSize 0, the streams' places), and then the block is emitted (returns true).  Mixed chains only: the
+// 4X and 1X kernels keep this step inline; a build that ran it through this helper for them too changed their SASS, and one chain
+// of 32,768 blocks took 35 instead of 28 ms per GiB on an H100.
+template <int S>
+__device__ __forceinline__ bool chain_old_plan(Plan& P, const u32 (&T)[8], const ChainBlock& x, const u32 (&sum)[8], unsigned lane, u64& r)
+{
+    u32 const n = x.n;
+    auto const count = [&](int k, u32 i) { return S == 4 ? x.cnt[k][i] : sum[i]; };
+    u32 bits[S], offs[S], lens[S];
+    u64 total;
+    stream_bits<S>(T, count, bits);
+    bool const fits = place_streams<S>(bits, 0, x.cap, offs, lens, total);
+    bool const ok = !(S == 4 && (x.cap < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;
+    if (ok) {
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = T[i];
+        #pragma unroll
+        for (int k = 0; k < S; k++) if (lane == (unsigned)k) { P.streamOff[k] = offs[k]; P.streamBytes[k] = lens[k]; }
+        if (lane == 0) { P.hSize = 0; P.total = (u32)total; }
+    }
+    r = ok ? total : 0;
+    return ok;
 }
 
 // The decisions restate the repeat plan's rules and plan_streams inline: this loop is serial and latency-bound, and built on shared
 // helpers ptxas scheduled the next block's loads later (1 chain of 32,768 blocks: 5 % slower on an H100).
 // Geo = ChainDescs: the state goes back to the chain's entries, the RLE byte to the block, its header to blkHdr / blkHdrSize.
 // Geo = ChainPackedDescs: none of these (the placement writes the RLE byte and the kinds); end[c] records what chainState needs.
+// NS = 0 (mixed chains): the old-table sizing in each block's form, and the 1X blocks to the 1X emit launch.
 template <int NS, class Geo>
 __global__ void __launch_bounds__(32 * CHAIN_WARPS)
 huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malformed)
 {
-    constexpr bool PACKED = std::is_same_v<Geo, ChainPackedDescs>;
+    constexpr bool PACKED = std::is_base_of_v<ChainPackedDescs, Geo>;
     unsigned const lane = threadIdx.x & 31u;
     if (*malformed) {              // every verdict srcSize_wrong, nothing else written and nothing emitted
         for (u64 b = blockIdx.x * (u64)blockDim.x + threadIdx.x; b < g.nBlocks; b += (u64)gridDim.x * blockDim.x) {
@@ -557,18 +606,18 @@ huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malfor
     u64 HS = g.hdrSize[c];
     bool saved = false;
     u32 lastNew = CHAIN_NONE, lastSaved = CHAIN_NONE;                                             // packed only
-    ChainBlock nx;
+    using Blk = std::conditional_t<NS == 0, ChainBlockMixed, ChainBlock>;
+    Blk nx;
     chain_load(g, plans, b0, nx, lane);
     #pragma unroll 1
     for (u32 b = b0; b < b1; b++) {
-        ChainBlock const x = nx;
+        Blk const x = nx;
         if (b + 1 < b1) chain_load(g, plans, b + 1, nx, lane);
         ChainFact const& f = x.f;
         u32 const n = x.n;
         u32 sum[8];                                                                               // block counts
         #pragma unroll
         for (u32 i = 0; i < 8; i++) sum[i] = x.cnt[0][i] + x.cnt[1][i] + x.cnt[2][i] + x.cnt[3][i];
-        auto const count = [&](int k, u32 i) { return NS == 4 ? x.cnt[k][i] : sum[i]; };
         u64 r = 0;
         bool useOld = false, emit = false;
         if (f.kind == CF_ARGS) r = f.exitValue;                                                   // huf_compress.c:656-664
@@ -603,23 +652,28 @@ huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malfor
         }
         Plan& P = plans[b];
         if (useOld) {                                                                             // HUF_compressCTable_internal with the old table
-            u32 bits[NS], offs[NS], lens[NS];
-            u64 total;
-            stream_bits<NS>(T, count, bits);
-            bool const fits = place_streams<NS>(bits, 0, x.cap, offs, lens, total);
-            bool const ok = !(NS == 4 && (x.cap < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;   // :564-565, :625
-            r = ok ? total : 0; emit = ok;
-            if (ok) {
-                #pragma unroll
-                for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = T[i];
-                #pragma unroll
-                for (int k = 0; k < NS; k++) if (lane == (unsigned)k) { P.streamOff[k] = offs[k]; P.streamBytes[k] = lens[k]; }
-                if (lane == 0) { P.hSize = 0; P.total = (u32)total; }
+            if constexpr (NS == 0) emit = x.single ? chain_old_plan<1>(P, T, x, sum, lane, r) : chain_old_plan<4>(P, T, x, sum, lane, r);
+            else {                                                                                // chain_old_plan<NS>, inline
+                auto const count = [&](int k, u32 i) { return NS == 4 ? x.cnt[k][i] : sum[i]; };
+                u32 bits[NS], offs[NS], lens[NS];
+                u64 total;
+                stream_bits<NS>(T, count, bits);
+                bool const fits = place_streams<NS>(bits, 0, x.cap, offs, lens, total);
+                bool const ok = !(NS == 4 && (x.cap < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;   // :564-565, :625
+                r = ok ? total : 0; emit = ok;
+                if (ok) {
+                    #pragma unroll
+                    for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = T[i];
+                    #pragma unroll
+                    for (int k = 0; k < NS; k++) if (lane == (unsigned)k) { P.streamOff[k] = offs[k]; P.streamBytes[k] = lens[k]; }
+                    if (lane == 0) { P.hSize = 0; P.total = (u32)total; }
+                }
             }
         }
         bool const coded = !is_err(r) && r >= 2;                                                  // 1X: a 1-byte stream is emitted, not coded
         if (lane == 0) {
-            P.state = emit ? 0 : 1;
+            if constexpr (NS == 0) P.state = emit ? (x.single ? PLAN_EMIT_1X : PLAN_EMIT) : PLAN_FINAL;
+            else P.state = emit ? PLAN_EMIT : PLAN_FINAL;
             g.result[b] = r;
             if constexpr (!PACKED) {
                 g.blkHdr[b] = coded && F != 0 ? H : nullptr;
@@ -663,6 +717,11 @@ static __device__ __noinline__ void store_piece_exact(u32* gw, u32 j, uint4 v, u
     for (u32 t = 0; t < 16; t++) { u32 const at = 4 * j + t; if (at >= a0 && at < endByte) pb[t] = (u8)(wd[t >> 2] >> (8 * (t & 3))); }
 }
 
+// The 1X emit launch of a mixed chain call: the blocks of geometry G whose plan is PLAN_EMIT_1X
+template <class G> struct Emit1X : G {};
+template <class G> struct EmitState { static constexpr u32 value = PLAN_EMIT; };
+template <class G> struct EmitState<Emit1X<G>> { static constexpr u32 value = PLAN_EMIT_1X; };
+
 // NS = streams per block.  4X: a CTA of 4 warps, one per stream.  1X (descriptor batches only): a CTA of ONE warp whose
 // segment is the whole block, and no jump table -- the same warp loop, 3 KB of shared memory per CTA (DESIGN.md 4.2).
 template <class Geo, int NS>
@@ -680,7 +739,7 @@ huf_emit_kernel(Geo g, u8* __restrict__ cbuf, const u8* __restrict__ src, const 
     unsigned const lane = tid & 31u; int const k = tid >> 5;
     u32 const b = blockIdx.x;
     const Plan& P = plans[b];
-    if (P.state != 0) return;                                       // verdict already delivered by the plan kernel
+    if (P.state != EmitState<Geo>::value) return;                          // verdict already delivered by the plan kernel (or the other launch's block)
     u32 const n = enc_len(g, b);
     const u8* const s = enc_src(g, src, b);
     u8* const d = enc_dst(g, cbuf, b);
@@ -1054,7 +1113,7 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
     e = optin.ensure(hufe::huf_plan_kernel<Geo, NS>, current_device(), (int)smem);
     if (e != cudaSuccess) return e;
     constexpr bool chain = std::is_base_of_v<ChainDescs, Geo>;
-    constexpr bool chainPacked = std::is_same_v<Geo, ChainPackedDescs>;
+    constexpr bool chainPacked = std::is_base_of_v<ChainPackedDescs, Geo>;
     constexpr bool packed = std::is_same_v<Geo, PackedDescs>;
     using EmitGeo = std::conditional_t<chainPacked, PackedDescs,    // the plan holds the chosen table
                                        std::conditional_t<std::is_same_v<Geo, RepeatDescs> || chain, BlockDescs, Geo>>;
@@ -1089,7 +1148,14 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
         pack::launch_pack<hufe::HufChainPlace>(gx, tileSum, tileSum + pack::tiles_of(gx.nBlocks), plans, stream);
         hufe::huf_pack_raw_kernel<<<gx.nBlocks, pack::COPY_THREADS, 0, stream>>>(gx.pk);
     }
-    hufe::huf_emit_kernel<EmitGeo, NS><<<gx.nBlocks, 32 * NS, 0, stream>>>(emit_view(gx), (u8*)cbuf, (const u8*)src, plans, nullptr);
+    if constexpr (NS == 0) {                                        // mixed: a 4X launch and a 1X launch, each passing the other's blocks by
+        hufe::Emit1X<EmitGeo> v1;
+        if constexpr (chainPacked) static_cast<PackedDescs&>(v1) = gx.pk;
+        else static_cast<BlockDescs&>(v1) = gx;
+        EmitGeo const& v4 = v1;
+        hufe::huf_emit_kernel<EmitGeo, 4><<<gx.nBlocks, 32 * 4, 0, stream>>>(v4, (u8*)cbuf, (const u8*)src, plans, nullptr);
+        hufe::huf_emit_kernel<hufe::Emit1X<EmitGeo>, 1><<<gx.nBlocks, 32, 0, stream>>>(v1, (u8*)cbuf, (const u8*)src, plans, nullptr);
+    } else hufe::huf_emit_kernel<EmitGeo, NS><<<gx.nBlocks, 32 * NS, 0, stream>>>(emit_view(gx), (u8*)cbuf, (const u8*)src, plans, nullptr);
     if constexpr (chainPacked) {                                    // the streams' state, if the total fits
         u64 const cgrid = ((u64)gx.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
         hufe::huf_chain_state_kernel<<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(
@@ -1111,6 +1177,7 @@ cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const
 //   RepeatDescs       HUF_compress4X_repeat / HUF_compress1X_repeat per block (table reuse)
 //   ChainDescs        chains of table reuse: plan, the chains' decisions, emit -- the repeat call block after block per chain
 //   ChainPackedDescs  packed chains: plan, the chains' decisions, the placement scan and raw copies, emit, the streams' state
+//   Mixed<...>        either chain geometry with a form per block: the same steps, and two emit launches (4X, 1X)
 template <class Geo>
 static cudaError_t huf_encode_descs(const Geo& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
@@ -1136,6 +1203,15 @@ cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned
 cudaError_t launch_huf_encode_chains_packed(const ChainPackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
     return huf_encode_descs(g, nStreams, msv, tlog, stream);
+}
+// mixed chains (common.cuh Mixed): each block in the form its flag names -- stream mode 0
+cudaError_t launch_huf_encode_chains_mixed(const ChainMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return huf_encode<ChainMixedDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+}
+cudaError_t launch_huf_encode_chains_packed_mixed(const ChainPackedMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return huf_encode<ChainPackedMixedDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
 }
 
 // the chain geometry's verdict (start[0] == 0, start[nChains] == nBlocks, never decreasing) to *malformed, for the decoders

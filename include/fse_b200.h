@@ -315,6 +315,47 @@ size_t FSEB200_HUF_decompress1X_repeat_packed(size_t nChains, const size_t* dCha
                                               const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
                                               const void* const* dChainHeaders, const size_t* dChainHeaderSizes, void* stream);
 
+/* Tier 1, chains of table reuse whose blocks each choose one or four streams (Huff0): the chain and packed-chain calls above, with
+ * one more per-block array, dSingleStream (unsigned char).  dSingleStream[b] == 0 codes step b of the loop with HUF_compress4X_repeat,
+ * any other value with HUF_compress1X_repeat -- the value is taken literally, as dPreferRepeat is.  zstd's literal coder makes
+ * that choice per section (one stream below 256 bytes) and both forms share the stream's table, flag and tree header: a header
+ * written by a 4X block is read by HUF_readDTableX1 exactly as one written by a 1X block.  Every other rule is that of the 4X / 1X
+ * call the mixed call stands for:
+ *   FSEB200_HUF_compress_mixed_repeat_chains          FSEB200_HUF_compress{4X,1X}_repeat_chains, the form per block;
+ *   FSEB200_HUF_decompress_mixed_repeat_blocks        per block exactly FSEB200_HUF_decompress{4X,1X}_repeat_blocks in its form,
+ *                                                     so the chain call's output decodes in one call;
+ *   FSEB200_HUF_compress_mixed_repeat_chains_packed   FSEB200_HUF_compress{4X,1X}_repeat_chains_packed: capacity HUF_compressBound(n)
+ *                                                     for both forms, the same kinds (2 own header, 3 treeless, whatever the form),
+ *                                                     offsets, capacity rule and state write-back;
+ *   FSEB200_HUF_decompress_mixed_repeat_packed        FSEB200_HUF_decompress{4X,1X}_repeat_packed, the form from the flag; a kind-3
+ *                                                     block's header is the last kind-2 block of its chain before it, whatever that
+ *                                                     block's form, else the chain's entry header.
+ * The form is not part of the kind byte: zstd carries it in the literal section header, apart from the block type, and the kinds
+ * keep zstd's numbering.  A mixed packed stream is therefore its bytes, offsets, kinds and the per-block dSingleStream flags.
+ * Argument verdicts are those of the 4X / 1X calls; a NULL dSingleStream while nBlocks > 0 is srcSize_wrong, the device untouched. */
+size_t FSEB200_HUF_compress_mixed_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                                void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
+                                                const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                const unsigned char* dSingleStream,
+                                                unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                const void** dHeaders, size_t* dHeaderSizes,
+                                                unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_decompress_mixed_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                                  const void* const* dCSrcs, const size_t* dCSrcSizes,
+                                                  const void* const* dHeaders, const size_t* dHeaderSizes,
+                                                  const unsigned char* dSingleStream, void* stream);
+size_t FSEB200_HUF_compress_mixed_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                                       void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                       const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                       const unsigned char* dSingleStream,
+                                                       unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                       unsigned maxSymbolValue, unsigned tableLog, void* stream);
+size_t FSEB200_HUF_decompress_mixed_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                                  void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
+                                                  const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
+                                                  const unsigned char* dSingleStream,
+                                                  const void* const* dChainHeaders, const size_t* dChainHeaderSizes, void* stream);
+
 /* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
  * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
  * DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).
@@ -478,6 +519,21 @@ size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains, const si
                                              void* hDst, const size_t* hDstSizes, size_t* hResults,
                                              const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
                                              const void* const* hChainHeaders, const size_t* hChainHeaderSizes);
+/* The same pair for chains whose blocks each choose their form (FSEB200_HUF_compress_mixed_repeat_chains_packed /
+ * FSEB200_HUF_decompress_mixed_repeat_packed): hSingleStream[b] (0 4X, else 1X, per block) in place of the codec, and every rule
+ * above unchanged -- chunking, the crossing chain's state, the entry headers (a tree header does not depend on the form of the
+ * block that wrote it) and the capacity rule.  A NULL hSingleStream while nBlocks > 0 gives srcSize_wrong before any device work. */
+size_t FSEB200_compress_host_mixed_repeat_chains_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                        void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds,
+                                                        const void* hSrc, const size_t* hSrcSizes, const int* hPreferRepeat,
+                                                        const unsigned char* hSingleStream,
+                                                        unsigned* const* hCTables, int* hRepeats, const void** hChainHeaders, size_t* hChainHeaderSizes,
+                                                        unsigned maxSymbolValue, unsigned tableLog);
+size_t FSEB200_decompress_host_mixed_repeat_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                   void* hDst, const size_t* hDstSizes, size_t* hResults,
+                                                   const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
+                                                   const unsigned char* hSingleStream,
+                                                   const void* const* hChainHeaders, const size_t* hChainHeaderSizes);
 
 /* Tier 1b, frames -- the self-describing .fse format of the reference's file tool (programs/fileio.c:266-626) on HOST buffers:
  *   frame   = LE32 magic (0x183E2309 FSE, 0x183E3309 Huff0), 1 byte block-size id (block = 1 KB << id, id <= 6),
