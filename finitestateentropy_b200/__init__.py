@@ -83,6 +83,8 @@ def _declare(L):
         c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     sig("FSEB200_HUF_decompress_mixed_repeat_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
         c_vp)
+    sig("FSEB200_HUF_compress_literals_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+        c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint, c_vp)
     for name in ("FSEB200_HUF_compress_packed", "FSEB200_HUF_compress1X_packed"):
         sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
     for codec in ("FSE", "FSEU16"):
@@ -101,6 +103,8 @@ def _declare(L):
     sig("FSEB200_compress_host_mixed_repeat_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
         c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint)
     sig("FSEB200_decompress_host_mixed_repeat_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
+    sig("FSEB200_compress_host_literals_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint)
     sig("FSEB200_frame_compressBound", c_sz, c_sz, C.c_uint)
     sig("FSEB200_frame_compress_host", c_sz, C.c_int, C.c_uint, c_vp, c_sz, c_vp, c_sz)
     sig("FSEB200_frame_decompress_bound", c_sz, c_vp, c_sz)
@@ -131,6 +135,7 @@ from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch
                     huf_decompress_repeat_packed, huf_decompress1x_repeat_packed,
                     huf_compress_mixed_repeat_chains, huf_decompress_mixed_repeat_blocks,
                     huf_compress_mixed_repeat_chains_packed, huf_decompress_mixed_repeat_packed,
+                    huf_compress_literals_chains_packed, host_compress_literals_chains_packed,
                     huf_compress_packed, huf_compress1x_packed, packed_pointers,
                     fse_compress_blocks, fse_decompress_blocks, fseu16_compress_blocks, fseu16_decompress_blocks,
                     fse_compress_packed, fseu16_compress_packed, fse_decompress_packed, fseu16_decompress_packed,

@@ -426,6 +426,44 @@ def huf_compress_mixed_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, p
     return out, offsets, csizes, kinds
 
 
+def huf_compress_literals_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
+                                        out=None, offsets=None, csizes=None, kinds=None, single_stream=None, max_symbol_value=255,
+                                        table_log=11, min_literals=64, min_gain_log=6):
+    """huf_compress_mixed_repeat_chains_packed under zstd's literal-coding policy (FSEB200_HUF_compress_literals_chains_packed): the
+    device chooses each block's form from the stream's flag, skips blocks below the size threshold (min_literals, or 6 bytes with
+    a valid table), stores a block raw when it fails the minimum gain (n >> min_gain_log) + 2 and RLE only when its bytes are
+    equal, and keeps a step's table and flag only for a block stored with its own header.  The other arguments are the mixed
+    call's.  Returns (out, offsets, csizes, kinds, single_stream): single_stream (uint8) holds the forms it chose, so the stream
+    decodes with huf_decompress_mixed_repeat_packed."""
+    from . import lib
+    n = _blocks_args(src_ptrs, src_sizes)
+    dev = src_ptrs.device
+    _check(prefer, torch.int32)
+    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
+    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
+                                               (chain_hdr_sizes, torch.int64)))
+    if out is None:
+        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
+    if offsets is None:
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    if kinds is None:
+        kinds = torch.empty(n, dtype=torch.uint8, device=dev)
+    if single_stream is None:
+        single_stream = torch.empty(n, dtype=torch.uint8, device=dev)
+    single = _single_arg(single_stream, n, dev)
+    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64); _check(kinds, torch.uint8)
+    assert offsets.numel() == n + 1 and csizes.numel() == n and kinds.numel() == n and out.device == dev, (offsets.numel(), n)
+    fn_name = "FSEB200_HUF_compress_literals_chains_packed"
+    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, out.data_ptr(), out.numel(), offsets.data_ptr(),
+                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(),
+                                single, ctables.data_ptr(), repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(),
+                                max_symbol_value, table_log, min_literals, min_gain_log, _stream_ptr())
+    _ret(r, fn_name)
+    return out, offsets, csizes, kinds, single_stream
+
+
 def huf_decompress_mixed_repeat_packed(chain_starts, packed, offsets, kinds, single_stream, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs,
                                        dst_sizes, results=None):
     """huf_decompress_repeat_packed over a buffer huf_compress_mixed_repeat_chains_packed wrote, each block in the form
@@ -721,9 +759,23 @@ def host_compress_mixed_repeat_chains_packed(src, sizes, chain_starts, prefer, s
                                  chain_hdr_sizes, out, max_symbol_value, table_log)
 
 
+def host_compress_literals_chains_packed(src, sizes, chain_starts, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, out=None,
+                                         max_symbol_value=255, table_log=11, min_literals=64, min_gain_log=6):
+    """huf_compress_literals_chains_packed on HOST memory (FSEB200_compress_host_literals_chains_packed), with the arguments and
+    state of host_compress_mixed_repeat_chains_packed but no forms in: byte for byte what the device call gives.  Synchronous.
+    Returns (out, offsets, csizes, kinds, single_stream, (ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes)); the stream decodes
+    with host_decompress_mixed_repeat_packed and that single_stream."""
+    single = torch.empty(_host_sizes(sizes).numel(), dtype=torch.uint8)
+    out, offsets, csizes, kinds, state = _host_chains_compress(None, single, src, sizes, chain_starts, prefer, ctables, repeats,
+                                                               chain_hdr_ptrs, chain_hdr_sizes, out, max_symbol_value, table_log,
+                                                               (min_literals, min_gain_log))
+    return out, offsets, csizes, kinds, single, state
+
+
 def _host_chains_compress(cid, single, src, sizes, chain_starts, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, out,
-                          max_symbol_value, table_log):
-    """cid: the C codec of the 4X / 1X call, or None for the mixed call with the per-block forms `single`"""
+                          max_symbol_value, table_log, literals=None):
+    """cid: the C codec of the 4X / 1X call, or None for the mixed call with the per-block forms `single`, or for the literal-policy
+    call with literals = (min_literals, min_gain_log), which writes the forms into `single`"""
     from . import lib
     sizes = _host_sizes(sizes)
     n = sizes.numel()
@@ -744,7 +796,10 @@ def _host_chains_compress(cid, single, src, sizes, chain_starts, prefer, ctables
             _host_ptr(src), _host_ptr(sizes), _host_ptr(prefer))
     state = (_host_ptr(table_ptrs), _host_ptr(repeats), _host_ptr(chain_hdr_ptrs), _host_ptr(chain_hdr_sizes), max_symbol_value,
              table_log)
-    if cid is None:
+    if literals is not None:
+        fn_name = "FSEB200_compress_host_literals_chains_packed"
+        r = getattr(lib(), fn_name)(*head, _host_ptr(single), *state, *literals)
+    elif cid is None:
         _host_check(single, torch.uint8)
         assert single.numel() == n, (single.numel(), n)
         fn_name = "FSEB200_compress_host_mixed_repeat_chains_packed"

@@ -304,6 +304,21 @@ FSEB_API size_t FSEB200_HUF_compress_mixed_repeat_chains(size_t nChains, const s
 // Packed chains: the chain calls with every block stored back to back in one buffer and a kind byte per block
 // (common.cuh ChainPackedDescs), and the decoders of that buffer.
 namespace {
+// the packed-chain geometry of a call's arguments, checked by the caller
+void chain_packed_descs(ChainPackedDescs& g, size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut, size_t outCapacity,
+                        size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs, const size_t* dSrcSizes,
+                        const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders,
+                        size_t* dChainHeaderSizes)
+{
+    g.dst = nullptr; g.dstCap = nullptr; g.result = (u64*)dCSizes; g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes;
+    g.nBlocks = (u32)nBlocks;
+    g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
+    g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.hdr = (const u8**)dChainHeaders; g.hdrSize = (u64*)dChainHeaderSizes;
+    g.blkHdr = nullptr; g.blkHdrSize = nullptr; g.fact = nullptr;
+    g.pk.out = (u8*)dOut; g.pk.outCap = outCapacity; g.pk.offset = (u64*)dOffsets; g.pk.result = g.result;
+    g.pk.src = g.src; g.pk.srcSize = g.srcSize; g.pk.nBlocks = g.nBlocks;
+    g.kind = dKinds; g.end = nullptr; g.malformed = nullptr;
+}
 size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut, size_t outCapacity,
                                 size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs,
                                 const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats,
@@ -315,14 +330,9 @@ size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size
         !dSrcSizes || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes || (!nStreams && !dSingleStream))
         return (size_t)err(E_SRC_WRONG);
     ChainPackedMixedDescs g;
-    g.dst = nullptr; g.dstCap = nullptr; g.result = (u64*)dCSizes; g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes;
-    g.nBlocks = (u32)nBlocks;
-    g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
-    g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.hdr = (const u8**)dChainHeaders; g.hdrSize = (u64*)dChainHeaderSizes;
-    g.blkHdr = nullptr; g.blkHdrSize = nullptr; g.fact = nullptr;
-    g.pk.out = (u8*)dOut; g.pk.outCap = outCapacity; g.pk.offset = (u64*)dOffsets; g.pk.result = g.result;
-    g.pk.src = g.src; g.pk.srcSize = g.srcSize; g.pk.nBlocks = g.nBlocks;
-    g.kind = dKinds; g.end = nullptr; g.malformed = nullptr; g.single = dSingleStream;
+    chain_packed_descs(g, nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes, dPreferRepeat,
+                       dCTables, dRepeats, dChainHeaders, dChainHeaderSizes);
+    g.single = dSingleStream;
     return ok_or_generic(nStreams ? launch_huf_encode_chains_packed(g, nStreams, msv, tlog, (cudaStream_t)stream)
                                   : launch_huf_encode_chains_packed_mixed(g, msv, tlog, (cudaStream_t)stream));
 }
@@ -385,6 +395,23 @@ FSEB_API size_t FSEB200_HUF_compress_mixed_repeat_chains_packed(size_t nChains, 
     return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
                                     dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 0, maxSymbolValue, tableLog, stream,
                                     dSingleStream);
+}
+FSEB_API size_t FSEB200_HUF_compress_literals_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
+                                                            size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                            const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                            unsigned char* dSingleStream, unsigned* const* dCTables, int* dRepeats,
+                                                            const void** dChainHeaders, size_t* dChainHeaderSizes, unsigned maxSymbolValue,
+                                                            unsigned tableLog, unsigned minLiterals, unsigned minGainLog, void* stream)
+{
+    if (nBlocks == 0) return 0;
+    if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dOut || !dOffsets || !dCSizes || !dKinds || !dSrcs ||
+        !dSrcSizes || !dPreferRepeat || !dSingleStream || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes ||
+        minGainLog < 1 || minGainLog > 31) return (size_t)err(E_SRC_WRONG);
+    ChainPackedLiteralsDescs g;
+    chain_packed_descs(g, nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes, dPreferRepeat,
+                       dCTables, dRepeats, dChainHeaders, dChainHeaderSizes);
+    g.single = dSingleStream; g.minLiterals = minLiterals; g.minGainLog = minGainLog;
+    return ok_or_generic(launch_huf_encode_literals_chains_packed(g, maxSymbolValue, tableLog, (cudaStream_t)stream));
 }
 FSEB_API size_t FSEB200_HUF_decompress_mixed_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
                                                            const size_t* dDstSizes, size_t* dResults, const void* dIn, const size_t* dOffsets,

@@ -190,9 +190,20 @@ struct Mixed : Base {
 };
 using ChainMixedDescs = Mixed<ChainDescs>;
 using ChainPackedMixedDescs = Mixed<ChainPackedDescs>;
-// block b's form: true for one stream.  Only mixed geometry has a choice.
+// Packed chains under zstd's literal-coding policy (include/fse_b200.h, FSEB200_HUF_compress_literals_chains_packed): the chain
+// kernel chooses each block's form from the stream's flag and writes it to single[b], applies the size threshold minLiterals and
+// the minimum gain (n >> minGainLog) + 2, and keeps a step's (table, flag) only when the block is stored with its own header.  The
+// plan kernel plans the form n alone decides (1X below 256 bytes, else 4X); the chain kernel re-plans 256 <= n < 1024 as 1X when
+// the flag is 2.  The chain kernel also writes each block's kind, which the placement (HufLiteralsPlace) stores by.
+struct ChainPackedLiteralsDescs : ChainPackedDescs {
+    u8* single;                    // per block, out
+    u32 minLiterals;
+    u32 minGainLog;                // 1 .. 31
+};
+// block b's form: true for one stream.  Only mixed geometry has a choice; the literal policy's plan takes the form n decides.
 template <class Geo> __device__ __forceinline__ bool enc_single(const Geo&, u32) { return false; }
 template <class Base> __device__ __forceinline__ bool enc_single(const Mixed<Base>& g, u32 b) { return g.single[b] != 0; }
+__device__ __forceinline__ bool enc_single(const ChainPackedLiteralsDescs& g, u32 b) { return enc_len(g, b) < 256; }
 
 // decoder: compressed source, its size, the output, the regenerated size, the result; `orig` (stored blocks) is uniform-only
 __device__ __forceinline__ const u8* dec_src(const BatchGeom& g, const u8* cbuf, u32 b) { return cbuf + (u64)b * g.slot; }

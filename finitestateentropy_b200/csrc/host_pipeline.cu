@@ -276,7 +276,8 @@ cudaError_t queue_packed_compress(Ring<3>& P, int k, const HostChunk& c, int cod
 // The finish of a packed compress chunk c whose offsets `lo` (chunk-local, cb + 1) and values have landed in the pinned image:
 // global offsets, the capacity rule of one call over the whole batch (a block that does not fit gets dstSize_tooSmall and, where
 // there are kinds, kind 4), and the stored bytes -- a prefix of the chunk's packed bytes at dOut, since the blocks that fit come
-// first -- copied down on s.  `total` is the global offset of the chunk's first block and moves past the chunk.
+// first -- copied down on s.  `total` is the global offset of the chunk's first block and moves past the chunk.  Where there are
+// kinds, a block stores bytes unless its kind is 4 (under the literal policy a raw block's value may be an error).
 cudaError_t finish_packed(const HostChunk& c, const u64* lo, const u64* vals, const u8* kinds, const u8* dOut, cudaStream_t s,
                           u8* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds, u64& total)
 {
@@ -285,9 +286,10 @@ cudaError_t finish_packed(const HostChunk& c, const u64* lo, const u64* vals, co
     for (size_t b = 0; b < cb; b++) {
         u64 const off = total + lo[b], len = lo[b + 1] - lo[b];
         u64 v = vals[b];
-        bool const over = !is_err(v) && off + len > outCapacity;
+        bool const stores = kinds ? kinds[b] != 4 : !is_err(v);
+        bool const over = stores && off + len > outCapacity;
         if (over) v = err(E_DST_TOO_SMALL);
-        else if (!is_err(v) && len) end = lo[b + 1];
+        else if (stores && len) end = lo[b + 1];
         hOffsets[c.b0 + b] = (size_t)off; hCSizes[c.b0 + b] = (size_t)v;
         if (hKinds) hKinds[c.b0 + b] = over ? 4 : kinds[b];
     }
@@ -393,7 +395,8 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
 // chunk runs the device call unchanged on chunk-local geometry.  Chains are contiguous ranges of blocks, so the chains that meet
 // a chunk are a contiguous range of which only the first can have started in an earlier chunk: at most one chain crosses each
 // chunk boundary, and its state (compress) or its last tree header (decompress) is all that passes from chunk to chunk.
-// codec: 1 = Huff0 4X, 3 = Huff0 1X; the mixed pair (a form per block, hSingleStream) runs the same code as codec 0.
+// codec: 1 = Huff0 4X, 3 = Huff0 1X; the mixed pair (a form per block, hSingleStream) runs the same code as codec 0, and the
+// literal-policy compress (the forms an output) as codec 0 with its own device call.
 // ================================================================================================
 namespace {
 // The most of a tree header a Huff0 decoder reads (HUF_readStats: 1 + 127 bytes in the FSE form, 1 + 64 raw); a header's size
@@ -426,12 +429,13 @@ struct ChunkChains {
 };
 
 // The chain compress, for cb blocks and nc chunk-local chains: source pointers, sizes, prefer flags (two per word), chain starts
-// (nc + 1) and, for the mixed call, the blocks' forms (eight per word) go up; offsets (cb + 1), values and kinds (eight per word)
-// come down.  The per-chain state views are ChainPool's at the chunk's first chain.
+// (nc + 1) and, for the mixed call, the blocks' forms (eight per word) go up; offsets (cb + 1), values, kinds (eight per word) and,
+// for the literal-policy call, the forms it chose come down.  The per-chain state views are ChainPool's at the chunk's first chain.
 struct ChainCompressWords {
-    size_t ptr = 0, size, prefer, start, single, offset, value, kind, end;
-    ChainCompressWords(size_t cb, size_t nc, bool mixed) : size(cb), prefer(2 * cb), start(prefer + (cb + 1) / 2), single(start + nc + 1),
-        offset(single + (mixed ? (cb + 7) / 8 : 0)), value(offset + cb + 1), kind(value + cb), end(kind + (cb + 7) / 8) {}
+    size_t ptr = 0, size, prefer, start, single, offset, value, kind, singleOut, end;
+    ChainCompressWords(size_t cb, size_t nc, bool mixed, bool lit) : size(cb), prefer(2 * cb), start(prefer + (cb + 1) / 2),
+        single(start + nc + 1), offset(single + (mixed ? (cb + 7) / 8 : 0)), value(offset + cb + 1), kind(value + cb),
+        singleOut(kind + (cb + 7) / 8), end(singleOut + (lit ? (cb + 7) / 8 : 0)) {}
 };
 // The chain decompress, for cb blocks, nc chunk-local chains and ne entry headers: destination pointers, sizes, offsets (cb + 1),
 // kinds, chain starts, the chains' entry header pointers and sizes, ne header images of HDR_MAX bytes with a 32-byte sector of
@@ -489,17 +493,22 @@ struct EntryHeader { size_t chain; const u8* p; u64 n; };
 }
 
 namespace {
-// codec 1 (4X), 3 (1X) or 0 (mixed: the form of block b from hSingle[b])
+// The literal-policy compress: the forms come back in `single`, and its two thresholds
+struct LiteralsOut { unsigned char* single; unsigned minLiterals, minGainLog; };
+
+// codec 1 (4X), 3 (1X) or 0 (mixed: the form of block b from hSingle[b]; with lit, the literal policy, which writes the forms)
 size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hOut, size_t outCapacity,
                             size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
                             const int* hPreferRepeat, const unsigned char* hSingle, unsigned* const* hCTables, int* hRepeats,
-                            const void** hChainHeaders, size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog)
+                            const void** hChainHeaders, size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog,
+                            const LiteralsOut* lit = nullptr)
 {
-    bool const mixed = codec == 0;
+    bool const mixed = codec == 0 && !lit;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
     if (nBlocks == 0) return 0;
     if (!hChainStarts || !hOut || !hOffsets || !hCSizes || !hKinds || !hSrc || !hSrcSizes || !hPreferRepeat || !hCTables ||
-        !hRepeats || !hChainHeaders || !hChainHeaderSizes || (mixed && !hSingle)) return (size_t)err(E_SRC_WRONG);
+        !hRepeats || !hChainHeaders || !hChainHeaderSizes || (mixed && !hSingle) ||
+        (lit && (!lit->single || lit->minGainLog < 1 || lit->minGainLog > 31))) return (size_t)err(E_SRC_WRONG);
     if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
         for (size_t b = 0; b < nBlocks; b++) { hCSizes[b] = (size_t)err(E_SRC_WRONG); hKinds[b] = 4; }
         return 0;
@@ -511,7 +520,7 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
     size_t words = 0;
     for (const HostChunk& c : chunks) {
         cc.emplace_back(hChainStarts, nChains, c);
-        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n, mixed).end);
+        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n, mixed, lit != nullptr).end);
     }
     auto& P = packed_ring();
     std::lock_guard<std::mutex> lock(P.mu);
@@ -539,7 +548,7 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
     auto queue = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
         size_t const cb = c.b1 - c.b0, c0 = cc[ci].c0;
-        ChainCompressWords const L(cb, cc[ci].n, mixed);
+        ChainCompressWords const L(cb, cc[ci].n, mixed, lit != nullptr);
         u64 const bytes = c.a1 - c.a0;
         cudaStream_t const s = P.st[k];
         u64* const h = P.hD[k], * const d = P.dD[k];
@@ -551,7 +560,14 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
         if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if ((r = cudaMemcpyAsync(d, h, L.offset * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if (ci && (r = cudaStreamWaitEvent(s, ev.ev[(ci - 1) % P.NS], 0)) != cudaSuccess) return r;
-        size_t const v = mixed
+        size_t const v = lit
+            ? FSEB200_HUF_compress_literals_chains_packed(
+                  cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
+                  (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size), (const int*)(d + L.prefer),
+                  (unsigned char*)(d + L.singleOut), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
+                  (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, lit->minLiterals,
+                  lit->minGainLog, s)
+            : mixed
             ? FSEB200_HUF_compress_mixed_repeat_chains_packed(
                   cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
                   (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size), (const int*)(d + L.prefer),
@@ -567,9 +583,10 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
     };
     u64 total = 0;
     auto finish = [&](size_t ci, int k) -> cudaError_t {
-        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n, mixed);
+        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n, mixed, lit != nullptr);
         cudaError_t const r = cudaStreamSynchronize(P.st[k]);
         if (r != cudaSuccess) return r;
+        if (lit) std::memcpy(lit->single + chunks[ci].b0, P.hD[k] + L.singleOut, chunks[ci].b1 - chunks[ci].b0);
         return finish_packed(chunks[ci], P.hD[k] + L.offset, P.hD[k] + L.value, (const u8*)(P.hD[k] + L.kind), P.dB[k], P.st[k],
                              (u8*)hOut, outCapacity, hOffsets, hCSizes, hKinds, total);
     };
@@ -711,6 +728,19 @@ FSEB_API size_t FSEB200_compress_host_mixed_repeat_chains_packed(size_t nChains,
     return host_chains_compress(0, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
                                 hPreferRepeat, hSingleStream, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue,
                                 tableLog);
+}
+FSEB_API size_t FSEB200_compress_host_literals_chains_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                             void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
+                                                             unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
+                                                             const int* hPreferRepeat, unsigned char* hSingleStream,
+                                                             unsigned* const* hCTables, int* hRepeats, const void** hChainHeaders,
+                                                             size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog,
+                                                             unsigned minLiterals, unsigned minGainLog)
+{
+    LiteralsOut const lit = { hSingleStream, minLiterals, minGainLog };
+    return host_chains_compress(0, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
+                                hPreferRepeat, nullptr, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue,
+                                tableLog, &lit);
 }
 FSEB_API size_t FSEB200_decompress_host_mixed_repeat_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hDst,
                                                             const size_t* hDstSizes, size_t* hResults, const void* hIn,

@@ -463,6 +463,8 @@ huf_plan_kernel(Geo g, u8* __restrict__ cbuf, u64* __restrict__ csizes, const u8
             if (!ok) {
                 #pragma unroll
                 for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = cell[i];
+                if constexpr (std::is_same_v<Geo, ChainPackedLiteralsDescs>)                    // for a 1X re-plan in the chain kernel
+                    for (u32 i = lane; i < (u32)hs; i += 32) P.header[i] = hdr[i];
             }
             u32 const newBits = estimate_bits(cell, sum);
             if (lane == 0) { F.newBits = newBits; F.newValue = ok ? total : 0; }
@@ -549,30 +551,93 @@ __device__ __forceinline__ void chain_load(const Geo& g, const Plan* plans, u32 
     if constexpr (std::is_same_v<Blk, ChainBlockMixed>) x.single = enc_single(g, b);
 }
 
-// HUF_compressCTable_internal with the chain's table T (cells, byte 3 cleared) in the S-stream form: the 4X size tests
-// (huf_compress.c:564-565), the capacity rule and the final test (:625).  The block's value, 0 or the size, goes to r; a size comes
-// with its plan (the cells, hSize 0, the streams' places), and then the block is emitted (returns true).  Mixed chains only: the
-// 4X and 1X kernels keep this step inline; a build that ran it through this helper for them too changed their SASS, and one chain
-// of 32,768 blocks took 35 instead of 28 ms per GiB on an H100.
+// HUF_compressCTable_internal with the table T (cells, byte 3 cleared) after a header of hs bytes in the S-stream form: the 4X
+// size tests (huf_compress.c:564-565), the capacity rule and the final test (:625).  The block's value, 0 or the size, goes to r;
+// a size comes with its plan (the cells, hSize, the streams' places; the header bytes must be in the plan already), and then the
+// block is emitted (returns true).  The chain's table has hs 0; the literal policy also re-plans a new table as 1X with its header.
+// Mixed and literal chains only: the 4X and 1X kernels keep this step inline; a build that ran it through this helper for them too
+// changed their SASS, and one chain of 32,768 blocks took 35 instead of 28 ms per GiB on an H100.
 template <int S>
-__device__ __forceinline__ bool chain_old_plan(Plan& P, const u32 (&T)[8], const ChainBlock& x, const u32 (&sum)[8], unsigned lane, u64& r)
+__device__ __forceinline__ bool chain_plan(Plan& P, const u32 (&T)[8], u64 hs, const ChainBlock& x, const u32 (&sum)[8], unsigned lane,
+                                           u64& r)
 {
     u32 const n = x.n;
     auto const count = [&](int k, u32 i) { return S == 4 ? x.cnt[k][i] : sum[i]; };
     u32 bits[S], offs[S], lens[S];
     u64 total;
     stream_bits<S>(T, count, bits);
-    bool const fits = place_streams<S>(bits, 0, x.cap, offs, lens, total);
-    bool const ok = !(S == 4 && (x.cap < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;
+    bool const fits = place_streams<S>(bits, hs, x.cap - hs, offs, lens, total);
+    bool const ok = !(S == 4 && (x.cap - hs < 6 + 1 + 1 + 1 + 8 || n < 12)) && fits && total < (u64)n - 1;
     if (ok) {
         #pragma unroll
         for (u32 i = 0; i < 8; i++) P.ctable[i * 32 + lane] = T[i];
         #pragma unroll
         for (int k = 0; k < S; k++) if (lane == (unsigned)k) { P.streamOff[k] = offs[k]; P.streamBytes[k] = lens[k]; }
-        if (lane == 0) { P.hSize = 0; P.total = (u32)total; }
+        if (lane == 0) { P.hSize = (u32)hs; P.total = (u32)total; }
     }
     r = ok ? total : 0;
     return ok;
+}
+
+// One step of zstd's literal coder (ZSTD_compressLiterals; the rule is stated once, in include/fse_b200.h) on block b of a chain
+// whose state is (T, F): the form from F, the size threshold, HUF_compress{1X,4X}_repeat on the step's flag Fs (its candidate
+// table is the block's new cells x.cell), then the block's kind.  The plan kernel planned the form n decides; a block F makes 1X
+// (F == 2, 256 <= n < 1024) is re-planned here, from its new cells and header or from T.  Writes the block's value, kind, form and
+// plan state; commits the candidate (T := x.cell, F := 1) and returns true only for kind 2.
+__device__ __forceinline__ bool literals_step(const ChainPackedLiteralsDescs& g, Plan& P, u32 b, const ChainBlockMixed& x,
+                                              const u32 (&sum)[8], u32 (&T)[8], int& F, unsigned lane)
+{
+    ChainFact const& f = x.f;
+    u32 const n = x.n;
+    bool const single = n < 256 || (F == 2 && n < 1024);
+    u64 r = 0;
+    u8 kind = 0;
+    if (n > HUF_BLOCK_MAX) { r = err(E_SRC_WRONG); kind = 4; }
+    else if (n >= (F == 2 ? 6u : g.minLiterals)) {
+        int Fs = F;
+        bool useOld = false, fresh = false;
+        if (f.kind == CF_ARGS) r = f.exitValue;                                                   // huf_compress.c:656-664
+        else if (x.prefer && Fs == 2) useOld = true;                                              // :665-669
+        else if (f.kind == CF_HIST) r = f.exitValue;                                              // hist.c:128, :673-674
+        else {
+            if (Fs == 1) {                                                                        // :679-683 HUF_validateCTable
+                bool bad = false;
+                #pragma unroll
+                for (u32 i = 0; i < 8; i++) bad |= sum[i] && (T[i] >> 16) == 0;
+                if (__any_sync(FULL, bad)) Fs = 0;
+            }
+            if (x.prefer && Fs != 0) useOld = true;                                               // :685-689
+            else if (is_err(f.hSize)) r = f.hSize;
+            else {
+                if (Fs != 0) {                                                                    // :703-713 the estimates, old and new
+                    u32 oldBits = 0;
+                    #pragma unroll
+                    for (u32 i = 0; i < 8; i++) oldBits += sum[i] * (T[i] >> 16);
+                    oldBits = __reduce_add_sync(FULL, oldBits);
+                    useOld = (oldBits >> 3) <= f.hSize + (f.newBits >> 3) || f.hSize + 12 >= n;
+                }
+                if (!useOld && f.hSize + 12 < n) { fresh = true; Fs = 0; r = f.newValue; }        // :716-719 the candidate table
+            }
+        }
+        if (useOld) single ? chain_plan<1>(P, T, 0, x, sum, lane, r) : chain_plan<4>(P, T, 0, x, sum, lane, r);
+        else if (fresh && single && !x.single) chain_plan<1>(P, x.cell, f.hSize, x, sum, lane, r);   // planned 4X, coded 1X
+        if (is_err(r) || r == 0 || r >= (u64)n - ((n >> g.minGainLog) + 2)) kind = 0;             // size_t: n < minGain rejects nothing
+        else if (r == 1) {                                      // RLE, unless a 1X stream of < 8 symbols fit in one byte
+            const u8* const s = g.src[b];
+            kind = (n >= 8 || __all_sync(FULL, lane >= n || s[lane] == s[0])) ? 1 : 0;
+        } else kind = Fs != 0 ? 3 : 2;
+    }
+    bool const commit = kind == 2;
+    if (commit) {
+        #pragma unroll
+        for (u32 i = 0; i < 8; i++) T[i] = x.cell[i];
+        F = 1;                                                                                    // the block carries the new table
+    }
+    if (lane == 0) {
+        P.state = kind == 2 || kind == 3 ? (single ? PLAN_EMIT_1X : PLAN_EMIT) : PLAN_FINAL;
+        g.result[b] = r; g.kind[b] = kind; g.single[b] = single;
+    }
+    return commit;
 }
 
 // The decisions restate the repeat plan's rules and plan_streams inline: this loop is serial and latency-bound, and built on shared
@@ -580,6 +645,7 @@ __device__ __forceinline__ bool chain_old_plan(Plan& P, const u32 (&T)[8], const
 // Geo = ChainDescs: the state goes back to the chain's entries, the RLE byte to the block, its header to blkHdr / blkHdrSize.
 // Geo = ChainPackedDescs: none of these (the placement writes the RLE byte and the kinds); end[c] records what chainState needs.
 // NS = 0 (mixed chains): the old-table sizing in each block's form, and the 1X blocks to the 1X emit launch.
+// Geo = ChainPackedLiteralsDescs (NS = 0): zstd's literal policy, each step on copies of the state; see literals_step.
 template <int NS, class Geo>
 __global__ void __launch_bounds__(32 * CHAIN_WARPS)
 huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malformed)
@@ -618,6 +684,10 @@ huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malfor
         u32 sum[8];                                                                               // block counts
         #pragma unroll
         for (u32 i = 0; i < 8; i++) sum[i] = x.cnt[0][i] + x.cnt[1][i] + x.cnt[2][i] + x.cnt[3][i];
+        if constexpr (std::is_same_v<Geo, ChainPackedLiteralsDescs>) {
+            if (literals_step(g, plans[b], b, x, sum, T, F, lane)) lastNew = lastSaved = b;
+            continue;
+        }
         u64 r = 0;
         bool useOld = false, emit = false;
         if (f.kind == CF_ARGS) r = f.exitValue;                                                   // huf_compress.c:656-664
@@ -652,8 +722,8 @@ huf_chain_kernel(Geo g, Plan* __restrict__ plans, const u32* __restrict__ malfor
         }
         Plan& P = plans[b];
         if (useOld) {                                                                             // HUF_compressCTable_internal with the old table
-            if constexpr (NS == 0) emit = x.single ? chain_old_plan<1>(P, T, x, sum, lane, r) : chain_old_plan<4>(P, T, x, sum, lane, r);
-            else {                                                                                // chain_old_plan<NS>, inline
+            if constexpr (NS == 0) emit = x.single ? chain_plan<1>(P, T, 0, x, sum, lane, r) : chain_plan<4>(P, T, 0, x, sum, lane, r);
+            else {                                                                                // chain_plan<NS> with hs 0, inline
                 auto const count = [&](int k, u32 i) { return NS == 4 ? x.cnt[k][i] : sum[i]; };
                 u32 bits[NS], offs[NS], lens[NS];
                 u64 total;
@@ -1012,6 +1082,41 @@ struct HufChainPlace {
     }
 };
 
+// Packed chains under the literal policy: the chain kernel has written every kind, and a raw block's value may be anything (an
+// error, a size the minimum gain rejected), so the stored length follows the kind: n raw, 1 RLE, the value for kinds 2 and 3.
+// The capacity verdict makes a block kind 4; the RLE byte is the source's first.  Malformed geometry (the chain kernel wrote only
+// the values): kinds 4, nothing placed.
+struct HufLiteralsPlace {
+    typedef ChainPackedLiteralsDescs Geo;
+    typedef Plan* Aux;
+    static __device__ __forceinline__ u64 value(const Geo& g, u64 b) { return g.result[b]; }
+    static __device__ __forceinline__ u64 len(const Geo& g, u64 b, u64 v)
+    {
+        if (*g.malformed) return 0;
+        u8 const k = g.kind[b];
+        return k == 0 ? g.srcSize[b] : k == 1 ? 1 : k == 4 ? 0 : v;
+    }
+    static __device__ __forceinline__ void place(const Geo& g, Plan* plans, u64 b, u64, u64 off, u64 len)
+    {
+        if (*g.malformed) { g.kind[b] = 4; return; }
+        g.pk.offset[b] = off;
+        u8 const k = g.kind[b];
+        if (k != 4 && off + len > g.pk.outCap) { g.result[b] = err(E_DST_TOO_SMALL); plans[b].state = PLAN_FINAL; g.kind[b] = 4; }
+        else if (k == 1) g.pk.out[off] = g.src[b][0];
+    }
+};
+
+// raw copy of every block of kind 0 (the literal policy's placement), one CTA per block
+__global__ void __launch_bounds__(pack::COPY_THREADS)
+huf_pack_raw_kinds_kernel(PackedDescs g, const u8* __restrict__ kind)
+{
+    u32 const b = blockIdx.x;
+    if (kind[b] != 0) return;
+    u32 const n = (u32)g.srcSize[b];                                // kind 0 means srcSize <= HUF_BLOCK_MAX
+    if (n == 0) return;
+    pack::cta_copy<pack::COPY_THREADS, pack::COPY_UNROLL>(g.out + g.offset[b], g.src[b], n);
+}
+
 // The streams' state, one warp per chain, once every block's place is known: nothing unless the geometry is sound and the total
 // (*total, which also becomes offset[nBlocks]) fits.  Then the chain's flag, the table of its last block that saved one (that
 // block's plan holds it, whatever its value), and the header of its last kind-2 block, at its place in out.
@@ -1144,7 +1249,10 @@ cudaError_t huf_encode(const Geo& g, void* cbuf, u64* csizes, const void* src, u
         u64 const cgrid = ((u64)gx.nChains + hufe::CHAIN_WARPS - 1) / hufe::CHAIN_WARPS;
         hufe::huf_chain_kernel<NS, Geo><<<(unsigned)(cgrid ? cgrid : 1), 32 * hufe::CHAIN_WARPS, 0, stream>>>(gx, plans, malformed);
     }
-    if constexpr (chainPacked) {                                    // offsets, kinds, capacity verdicts, RLE bytes, raw copies; then emit
+    if constexpr (std::is_same_v<Geo, ChainPackedLiteralsDescs>) {  // offsets by the decided kinds, capacity verdicts, RLE bytes, raw copies
+        pack::launch_pack<hufe::HufLiteralsPlace>(gx, tileSum, tileSum + pack::tiles_of(gx.nBlocks), plans, stream);
+        hufe::huf_pack_raw_kinds_kernel<<<gx.nBlocks, pack::COPY_THREADS, 0, stream>>>(gx.pk, gx.kind);
+    } else if constexpr (chainPacked) {                             // offsets, kinds, capacity verdicts, RLE bytes, raw copies; then emit
         pack::launch_pack<hufe::HufChainPlace>(gx, tileSum, tileSum + pack::tiles_of(gx.nBlocks), plans, stream);
         hufe::huf_pack_raw_kernel<<<gx.nBlocks, pack::COPY_THREADS, 0, stream>>>(gx.pk);
     }
@@ -1178,6 +1286,8 @@ cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const
 //   ChainDescs        chains of table reuse: plan, the chains' decisions, emit -- the repeat call block after block per chain
 //   ChainPackedDescs  packed chains: plan, the chains' decisions, the placement scan and raw copies, emit, the streams' state
 //   Mixed<...>        either chain geometry with a form per block: the same steps, and two emit launches (4X, 1X)
+//   ChainPackedLiteralsDescs  packed chains under zstd's literal policy: as Mixed<ChainPackedDescs>, the forms and kinds decided by
+//                     the chain kernel, the placement and raw copies by kind
 template <class Geo>
 static cudaError_t huf_encode_descs(const Geo& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
@@ -1212,6 +1322,11 @@ cudaError_t launch_huf_encode_chains_mixed(const ChainMixedDescs& g, unsigned ms
 cudaError_t launch_huf_encode_chains_packed_mixed(const ChainPackedMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
     return huf_encode<ChainPackedMixedDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+}
+// packed chains under the literal policy (common.cuh ChainPackedLiteralsDescs): stream mode 0, the forms decided by the chain kernel
+cudaError_t launch_huf_encode_literals_chains_packed(const ChainPackedLiteralsDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
+{
+    return huf_encode<ChainPackedLiteralsDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
 }
 
 // the chain geometry's verdict (start[0] == 0, start[nChains] == nBlocks, never decreasing) to *malformed, for the decoders

@@ -25,6 +25,7 @@ cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned
 cudaError_t launch_huf_encode_chains_packed(const ChainPackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_encode_chains_mixed(const ChainMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_encode_chains_packed_mixed(const ChainPackedMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream);
+cudaError_t launch_huf_encode_literals_chains_packed(const ChainPackedLiteralsDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_chain_check(const u64* start, u32 nChains, u32 nBlocks, u32* malformed, cudaStream_t stream);
 cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream);
 // the same per block in the form single[b] names (0: 4X, else 1X), huf_packed.cu

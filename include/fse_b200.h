@@ -356,6 +356,50 @@ size_t FSEB200_HUF_decompress_mixed_repeat_packed(size_t nChains, const size_t* 
                                                   const unsigned char* dSingleStream,
                                                   const void* const* dChainHeaders, const size_t* dChainHeaderSizes, void* stream);
 
+/* Tier 1, packed chains under zstd's literal-coding policy (Huff0): FSEB200_HUF_compress_mixed_repeat_chains_packed with the
+ * decisions zstd's literal coder (ZSTD_compressLiterals, zstd 1.5) takes around each HUF_compress{4X,1X}_repeat call made on the
+ * device from the state the chain carries: the form, the size below which no coding is attempted, the raw and RLE fallbacks,
+ * and the rollback of the stream's state when a block is not stored coded.  The arguments are the mixed call's, except that
+ * dSingleStream is an output (one form flag per block, written for every block) and minLiterals, minGainLog follow tableLog.
+ * The rule, per chain, block after block, with the state (T, F, H) read from the per-chain entries at the start, n = dSrcSizes[b]
+ * and minGain(n) = (n >> minGainLog) + 2:
+ *   single[b] = n < 256 || (F == 2 && n < 1024)                              -> dSingleStream[b]
+ *   n > 128 KB:                           value srcSize_wrong, kind 4, state unchanged   (the decoders' limit, zstd's block limit)
+ *   else n < (F == 2 ? 6 : minLiterals):  value 0, kind 0 (raw), state unchanged          (not attempted)
+ *   else: on copies T', F' of T, F
+ *     v = HUF_compress{1X if single[b] else 4X}_repeat(dst, HUF_compressBound(n), src, n, maxSymbolValue, tableLog, wksp,
+ *                                                     sizeof wksp, T', &F', dPreferRepeat[b], 0);  the value is v, and
+ *     isError(v) || v == 0 || v >= n - minGain(n)  (size_t: when n < minGain(n) the difference wraps and rejects nothing):
+ *                                             kind 0 (raw), state unchanged;
+ *     else v == 1:                            kind 1 (RLE) if n >= 8 or all n bytes are equal, else kind 0 (raw: a 1X block of
+ *                                             at most 7 symbols coded with the old table can fit in one byte); state unchanged;
+ *     else F' != 0:                           kind 3 (coded with the stream's table T, no header), state unchanged;
+ *     else:                                   kind 2 (its own tree header), state := (T', 1, this block's stored bytes).
+ * HUF_compress_internal saves a new table and sets the flag to none before its last compressibility test, so without the rollback a
+ * block that ends up raw or RLE would still have replaced the stream's table; zstd restores the previous table and flag in that
+ * case, as this rule does.  zstd 1.5 sets (minLiterals, minGainLog) by strategy (ZSTD_minLiteralsToCompress, ZSTD_minGain): (64, 6)
+ * below btopt, (16, 7) for btultra, (8, 8) for btultra2; minLiterals may be any value, 0 included, and minGainLog must be 1 .. 31.
+ * zstd derives dPreferRepeat from its strategy and n; here it stays a per-block input.  Byte equality with libzstd is not claimed:
+ * later zstd versions also change how the table is built (optimal depth, sampling of incompressible input), and the reference this
+ * library follows has no counterpart for that; the bytes of a coded block are those of the reference's HUF_compress{4X,1X}_repeat.
+ * Stored length: n for kind 0, 1 for kind 1 (src[0]), v for kinds 2 and 3, 0 for kind 4 -- so at most n, and sum(n) + 32 bytes of
+ * slack always fits.  Offsets, the capacity rule (a block that does not fit outCapacity gets dstSize_tooSmall and kind 4) and the
+ * state write-back (only if dOffsets[nBlocks] <= outCapacity; otherwise every per-chain entry as it came in) are those of the packed
+ * chain calls; a table is written only if a kind-2 block committed one, and the chain header is that of the chain's last kind-2
+ * block.  Malformed chain geometry gives every value srcSize_wrong and every kind 4, and nothing else is written (dSingleStream
+ * included).  The stream is what the mixed packed calls read: FSEB200_HUF_decompress_mixed_repeat_packed decodes (dOut, dOffsets,
+ * dKinds, dSingleStream) with the headers the chains entered with.
+ * Contract: that of FSEB200_HUF_compress_mixed_repeat_chains_packed; dSingleStream overlaps no other array.
+ * Return value: 0 (also for nBlocks == 0, which launches nothing and writes nothing); srcSize_wrong, the device untouched, for
+ * nBlocks or nChains above 0xFFFFFFFF, a NULL array or minGainLog outside 1 .. 31 while nBlocks > 0; generic if a launch fails. */
+size_t FSEB200_HUF_compress_literals_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks,
+                                                   void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
+                                                   const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
+                                                   unsigned char* dSingleStream,
+                                                   unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
+                                                   unsigned maxSymbolValue, unsigned tableLog, unsigned minLiterals, unsigned minGainLog,
+                                                   void* stream);
+
 /* Tier 1, per-block descriptors (FSE, FSE-U16): the same argument shape for the two FSE codecs -- e.g. the FSE-coded blocks of
  * an .fse frame body, packed back to back behind their block headers.  All six arrays and every buffer they point to are in
  * DEVICE memory; the call is asynchronous on `stream` and the host never reads the arrays (no copy, no synchronize).
@@ -534,6 +578,17 @@ size_t FSEB200_decompress_host_mixed_repeat_packed(size_t nChains, const size_t*
                                                    const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
                                                    const unsigned char* hSingleStream,
                                                    const void* const* hChainHeaders, const size_t* hChainHeaderSizes);
+/* FSEB200_HUF_compress_literals_chains_packed on host buffers, through the same pipeline: hSingleStream is an output (written for
+ * every block, as the device call writes it) and every other rule is the mixed compress's above.  The rolled-back state of the
+ * chain that crosses a chunk boundary stays on the device between the chunks' calls, so the output, the forms and the state are
+ * byte for byte what one device call over the whole batch gives.  The stream decodes with FSEB200_decompress_host_mixed_repeat_packed.
+ * Argument verdicts (NULL pointers, sizes, minGainLog outside 1 .. 31) come before any device work. */
+size_t FSEB200_compress_host_literals_chains_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
+                                                    void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds,
+                                                    const void* hSrc, const size_t* hSrcSizes, const int* hPreferRepeat,
+                                                    unsigned char* hSingleStream,
+                                                    unsigned* const* hCTables, int* hRepeats, const void** hChainHeaders, size_t* hChainHeaderSizes,
+                                                    unsigned maxSymbolValue, unsigned tableLog, unsigned minLiterals, unsigned minGainLog);
 
 /* Tier 1b, frames -- the self-describing .fse format of the reference's file tool (programs/fileio.c:266-626) on HOST buffers:
  *   frame   = LE32 magic (0x183E2309 FSE, 0x183E3309 Huff0), 1 byte block-size id (block = 1 KB << id, id <= 6),
