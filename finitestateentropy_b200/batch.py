@@ -173,9 +173,7 @@ def _repeat_blocks(fn_name, src_ptrs, src_sizes, dst_ptrs, dst_caps, ctables, re
     if csizes is None:
         csizes = torch.empty(src_ptrs.numel(), dtype=torch.int64, device=src_ptrs.device)
     n = _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, ctables)
-    for a in (repeats, prefer):
-        _check(a, torch.int32)
-        assert a.numel() == n and a.device == src_ptrs.device, (a.numel(), n, a.device)
+    _arrays(n, src_ptrs.device, (repeats, torch.int32), (prefer, torch.int32))
     r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
                                 src_sizes.data_ptr(), ctables.data_ptr(), repeats.data_ptr(), prefer.data_ptr(), msv, tlog,
                                 _stream_ptr())
@@ -191,39 +189,59 @@ def huf_compress_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_
     and its header chain_hdr_ptrs[c] / chain_hdr_sizes[c] (int64), read at the start and updated at the end of the chain.
     Returns (csizes, hdr_ptrs, hdr_sizes) (int64): block b's value and the header it was coded with (0 / 0: its own, or none),
     as FSEB200_HUF_decompress4X_repeat_blocks takes them."""
-    return _repeat_chains("FSEB200_HUF_compress4X_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer,
+    return _repeat_chains("FSEB200_HUF_compress4X_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, None,
                           ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, max_symbol_value, table_log)
 
 
 def huf_compress1x_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, ctables, repeats, chain_hdr_ptrs,
                                  chain_hdr_sizes, csizes=None, hdr_ptrs=None, hdr_sizes=None, max_symbol_value=255, table_log=12):
     """huf_compress_repeat_chains in the single-stream format (HUF_compress1X_repeat per block)"""
-    return _repeat_chains("FSEB200_HUF_compress1X_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer,
+    return _repeat_chains("FSEB200_HUF_compress1X_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, None,
                           ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, max_symbol_value, table_log)
 
 
-def _repeat_chains(fn_name, chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, ctables, repeats, chain_hdr_ptrs,
-                   chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, msv, tlog):
-    from . import lib
-    n = src_ptrs.numel()
-    if csizes is None:
-        csizes = torch.empty(n, dtype=torch.int64, device=src_ptrs.device)
-    if hdr_ptrs is None:
-        hdr_ptrs = torch.empty(n, dtype=torch.int64, device=src_ptrs.device)
-    if hdr_sizes is None:
-        hdr_sizes = torch.empty(n, dtype=torch.int64, device=src_ptrs.device)
-    _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, hdr_ptrs, hdr_sizes)
-    _check(prefer, torch.int32)
-    assert prefer.numel() == n and prefer.device == src_ptrs.device, (prefer.numel(), n, prefer.device)
+def _arrays(n, dev, *arrays):
+    """the device addresses of (tensor, dtype) pairs, each checked to be a contiguous CUDA tensor of that dtype with n entries on
+    `dev`; a None tensor (the form flags of a call that has none) is left out"""
+    ptrs = []
+    for a, dtype in arrays:
+        if a is not None:
+            _check(a, dtype)
+            assert a.numel() == n and a.device == dev, (a.numel(), n, a.device)
+            ptrs.append(a.data_ptr())
+    return ptrs
+
+
+def _chain_args(chain_starts, dev, *per_chain):
+    """(n_chains, addresses of the per-chain arrays) after checking chain_starts (int64, n_chains + 1) and each array"""
     _check(chain_starts, torch.int64)
     n_chains = chain_starts.numel() - 1
-    assert n_chains >= 0 and chain_starts.device == src_ptrs.device, (chain_starts.numel(), chain_starts.device)
-    for a, dtype in ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64)):
-        _check(a, dtype)
-        assert a.numel() == n_chains and a.device == src_ptrs.device, (a.numel(), n_chains, a.device)
+    assert n_chains >= 0 and chain_starts.device == dev, (chain_starts.numel(), chain_starts.device)
+    return n_chains, _arrays(n_chains, dev, *per_chain)
+
+
+def _state_args(chain_starts, dev, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes):
+    return _chain_args(chain_starts, dev, (ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
+                       (chain_hdr_sizes, torch.int64))
+
+
+def _repeat_chains(fn_name, chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, single, ctables, repeats, chain_hdr_ptrs,
+                   chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes, msv, tlog):
+    """the pointer-form chain compress; `single` the per-block forms of the mixed call, None for the 4X and 1X calls"""
+    from . import lib
+    n = src_ptrs.numel()
+    dev = src_ptrs.device
+    if csizes is None:
+        csizes = torch.empty(n, dtype=torch.int64, device=dev)
+    if hdr_ptrs is None:
+        hdr_ptrs = torch.empty(n, dtype=torch.int64, device=dev)
+    if hdr_sizes is None:
+        hdr_sizes = torch.empty(n, dtype=torch.int64, device=dev)
+    _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, hdr_ptrs, hdr_sizes)
+    per_block = _arrays(n, dev, (prefer, torch.int32), (single, torch.uint8))
+    n_chains, state = _state_args(chain_starts, dev, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes)
     r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(),
-                                src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(), ctables.data_ptr(),
-                                repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(), hdr_ptrs.data_ptr(),
+                                src_ptrs.data_ptr(), src_sizes.data_ptr(), *per_block, *state, hdr_ptrs.data_ptr(),
                                 hdr_sizes.data_ptr(), msv, tlog, _stream_ptr())
     _ret(r, fn_name)
     return csizes, hdr_ptrs, hdr_sizes
@@ -237,36 +255,28 @@ def huf_compress_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, prefer,
     stored lengths, csizes the loop's value per block (dstSize_tooSmall for a block that does not fit `out`), kinds (uint8) 0 raw,
     1 RLE, 2 own tree header, 3 the previous table's header, 4 nothing stored.  With out=None, `out` is allocated at
     sum(src_sizes) + 32 bytes, always enough: reading that sum costs one host synchronisation."""
-    return _repeat_chains_packed("FSEB200_HUF_compress4X_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer, ctables,
-                                 repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds, max_symbol_value, table_log)
+    return _repeat_chains_packed("FSEB200_HUF_compress4X_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer, None, ctables,
+                                 repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds, (max_symbol_value, table_log))
 
 
 def huf_compress1x_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
                                         out=None, offsets=None, csizes=None, kinds=None, max_symbol_value=255, table_log=12):
     """huf_compress_repeat_chains_packed in the single-stream format (HUF_compress1X_repeat per block)"""
-    return _repeat_chains_packed("FSEB200_HUF_compress1X_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer, ctables,
-                                 repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds, max_symbol_value, table_log)
+    return _repeat_chains_packed("FSEB200_HUF_compress1X_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer, None, ctables,
+                                 repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds, (max_symbol_value, table_log))
 
 
-def _chain_args(chain_starts, dev, per_chain):
-    _check(chain_starts, torch.int64)
-    n_chains = chain_starts.numel() - 1
-    assert n_chains >= 0 and chain_starts.device == dev, (chain_starts.numel(), chain_starts.device)
-    for a, dtype in per_chain:
-        _check(a, dtype)
-        assert a.numel() == n_chains and a.device == dev, (a.numel(), n_chains, a.device)
-    return n_chains
-
-
-def _repeat_chains_packed(fn_name, chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
-                          out, offsets, csizes, kinds, msv, tlog):
+def _repeat_chains_packed(fn_name, chain_starts, src_ptrs, src_sizes, prefer, single, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
+                          out, offsets, csizes, kinds, scalars, forms_out=False):
+    """the packed chain compress; `single` the per-block forms (None for the 4X and 1X calls), which with forms_out the call
+    writes, allocated here when None and returned last; `scalars` the C call's arguments between the chain headers and the stream"""
     from . import lib
     n = _blocks_args(src_ptrs, src_sizes)
     dev = src_ptrs.device
-    _check(prefer, torch.int32)
-    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
-    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
-                                               (chain_hdr_sizes, torch.int64)))
+    if forms_out and single is None:
+        single = torch.empty(n, dtype=torch.uint8, device=dev)
+    per_block = _arrays(n, dev, (prefer, torch.int32), (single, torch.uint8))
+    n_chains, state = _state_args(chain_starts, dev, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes)
     if out is None:
         out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
     if offsets is None:
@@ -278,11 +288,10 @@ def _repeat_chains_packed(fn_name, chain_starts, src_ptrs, src_sizes, prefer, ct
     _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64); _check(kinds, torch.uint8)
     assert offsets.numel() == n + 1 and csizes.numel() == n and kinds.numel() == n and out.device == dev, (offsets.numel(), n)
     r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, out.data_ptr(), out.numel(), offsets.data_ptr(),
-                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(),
-                                ctables.data_ptr(), repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(),
-                                msv, tlog, _stream_ptr())
+                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), *per_block, *state,
+                                *scalars, _stream_ptr())
     _ret(r, fn_name)
-    return out, offsets, csizes, kinds
+    return (out, offsets, csizes, kinds) + ((single,) if forms_out else ())
 
 
 def huf_decompress_repeat_packed(chain_starts, packed, offsets, kinds, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes,
@@ -291,29 +300,31 @@ def huf_decompress_repeat_packed(chain_starts, packed, offsets, kinds, chain_hdr
     regenerating dst_sizes[b] bytes, on the current stream: a kind-3 block takes the header of the last kind-2 block before it
     in its chain, or chain_hdr_ptrs[c] / chain_hdr_sizes[c] (int64, the headers the chains entered the compress call with).
     Returns results (int64; the regenerated size or an error code per block)."""
-    return _repeat_unpack("FSEB200_HUF_decompress4X_repeat_packed", chain_starts, packed, offsets, kinds, chain_hdr_ptrs,
+    return _repeat_unpack("FSEB200_HUF_decompress4X_repeat_packed", chain_starts, packed, offsets, kinds, None, chain_hdr_ptrs,
                           chain_hdr_sizes, dst_ptrs, dst_sizes, results)
 
 
 def huf_decompress1x_repeat_packed(chain_starts, packed, offsets, kinds, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes,
                                    results=None):
     """huf_decompress_repeat_packed in the single-stream format (huf_compress1x_repeat_chains_packed's buffers)"""
-    return _repeat_unpack("FSEB200_HUF_decompress1X_repeat_packed", chain_starts, packed, offsets, kinds, chain_hdr_ptrs,
+    return _repeat_unpack("FSEB200_HUF_decompress1X_repeat_packed", chain_starts, packed, offsets, kinds, None, chain_hdr_ptrs,
                           chain_hdr_sizes, dst_ptrs, dst_sizes, results)
 
 
-def _repeat_unpack(fn_name, chain_starts, packed, offsets, kinds, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes, results):
+def _repeat_unpack(fn_name, chain_starts, packed, offsets, kinds, single, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes,
+                   results):
+    """the packed chain decompress; `single` the per-block forms of the mixed call, None for the 4X and 1X calls"""
     from . import lib
     n = _blocks_args(dst_ptrs, dst_sizes)
     dev = dst_ptrs.device
-    n_chains = _chain_args(chain_starts, dev, ((chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64)))
+    n_chains, headers = _chain_args(chain_starts, dev, (chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64))
+    forms = _arrays(n, dev, (single, torch.uint8))
     if results is None:
         results = torch.empty(n, dtype=torch.int64, device=dev)
     _check(packed, torch.uint8); _check(offsets, torch.int64); _check(kinds, torch.uint8); _check(results, torch.int64)
     assert offsets.numel() == n + 1 and kinds.numel() == n and results.numel() == n and packed.device == dev, (offsets.numel(), n)
     r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(),
-                                packed.data_ptr(), offsets.data_ptr(), kinds.data_ptr(), chain_hdr_ptrs.data_ptr(),
-                                chain_hdr_sizes.data_ptr(), _stream_ptr())
+                                packed.data_ptr(), offsets.data_ptr(), kinds.data_ptr(), *forms, *headers, _stream_ptr())
     _ret(r, fn_name)
     return results
 
@@ -332,21 +343,17 @@ def huf_decompress1x_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, h
                           hdr_sizes, results)
 
 
-def _header_blocks(fn_name, csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results):
+def _header_blocks(fn_name, csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, results, single=None):
+    """the header-taking blocks decompress; `single` the per-block forms of the mixed call, None for the 4X and 1X calls"""
     from . import lib
     if results is None:
         results = torch.empty(csrc_ptrs.numel(), dtype=torch.int64, device=csrc_ptrs.device)
     n = _blocks_args(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results, hdr_ptrs, hdr_sizes)
+    forms = _arrays(n, csrc_ptrs.device, (single, torch.uint8))
     r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), csrc_ptrs.data_ptr(),
-                                csrc_sizes.data_ptr(), hdr_ptrs.data_ptr(), hdr_sizes.data_ptr(), _stream_ptr())
+                                csrc_sizes.data_ptr(), hdr_ptrs.data_ptr(), hdr_sizes.data_ptr(), *forms, _stream_ptr())
     _ret(r, fn_name)
     return results
-
-
-def _single_arg(single_stream, n, dev):
-    _check(single_stream, torch.uint8)
-    assert single_stream.numel() == n and single_stream.device == dev, (single_stream.numel(), n, single_stream.device)
-    return single_stream.data_ptr()
 
 
 def huf_compress_mixed_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer, single_stream, ctables, repeats,
@@ -355,43 +362,16 @@ def huf_compress_mixed_repeat_chains(chain_starts, src_ptrs, src_sizes, dst_ptrs
     """huf_compress_repeat_chains with each block's form chosen by single_stream[b] (uint8): 0 HUF_compress4X_repeat, anything
     else HUF_compress1X_repeat.  Both forms share the stream's table, flag and header.  Returns (csizes, hdr_ptrs, hdr_sizes),
     as huf_decompress_mixed_repeat_blocks takes them with the same single_stream."""
-    from . import lib
-    n = src_ptrs.numel()
-    dev = src_ptrs.device
-    if csizes is None:
-        csizes = torch.empty(n, dtype=torch.int64, device=dev)
-    if hdr_ptrs is None:
-        hdr_ptrs = torch.empty(n, dtype=torch.int64, device=dev)
-    if hdr_sizes is None:
-        hdr_sizes = torch.empty(n, dtype=torch.int64, device=dev)
-    _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes, hdr_ptrs, hdr_sizes)
-    _check(prefer, torch.int32)
-    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
-    single = _single_arg(single_stream, n, dev)
-    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
-                                               (chain_hdr_sizes, torch.int64)))
-    fn_name = "FSEB200_HUF_compress_mixed_repeat_chains"
-    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(),
-                                src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(), single, ctables.data_ptr(),
-                                repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(), hdr_ptrs.data_ptr(),
-                                hdr_sizes.data_ptr(), max_symbol_value, table_log, _stream_ptr())
-    _ret(r, fn_name)
-    return csizes, hdr_ptrs, hdr_sizes
+    return _repeat_chains("FSEB200_HUF_compress_mixed_repeat_chains", chain_starts, src_ptrs, src_sizes, dst_ptrs, dst_caps, prefer,
+                          single_stream, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, csizes, hdr_ptrs, hdr_sizes,
+                          max_symbol_value, table_log)
 
 
 def huf_decompress_mixed_repeat_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs, hdr_sizes, single_stream, results=None):
     """huf_decompress_repeat_blocks (single_stream[b] == 0) or huf_decompress1x_repeat_blocks (otherwise) on every block b, in
     one call on the current stream.  Returns results (int64)."""
-    from . import lib
-    if results is None:
-        results = torch.empty(csrc_ptrs.numel(), dtype=torch.int64, device=csrc_ptrs.device)
-    n = _blocks_args(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results, hdr_ptrs, hdr_sizes)
-    single = _single_arg(single_stream, n, csrc_ptrs.device)
-    fn_name = "FSEB200_HUF_decompress_mixed_repeat_blocks"
-    r = getattr(lib(), fn_name)(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), csrc_ptrs.data_ptr(),
-                                csrc_sizes.data_ptr(), hdr_ptrs.data_ptr(), hdr_sizes.data_ptr(), single, _stream_ptr())
-    _ret(r, fn_name)
-    return results
+    return _header_blocks("FSEB200_HUF_decompress_mixed_repeat_blocks", csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, hdr_ptrs,
+                          hdr_sizes, results, single_stream)
 
 
 def huf_compress_mixed_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, single_stream, ctables, repeats, chain_hdr_ptrs,
@@ -399,31 +379,9 @@ def huf_compress_mixed_repeat_chains_packed(chain_starts, src_ptrs, src_sizes, p
                                             table_log=12):
     """huf_compress_repeat_chains_packed with each block's form chosen by single_stream[b] (uint8, 0 = 4X).  Kinds keep their
     numbering whatever the form, so the stream is (out, offsets, kinds) plus single_stream.  Returns (out, offsets, csizes, kinds)."""
-    from . import lib
-    n = _blocks_args(src_ptrs, src_sizes)
-    dev = src_ptrs.device
-    _check(prefer, torch.int32)
-    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
-    single = _single_arg(single_stream, n, dev)
-    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
-                                               (chain_hdr_sizes, torch.int64)))
-    if out is None:
-        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
-    if offsets is None:
-        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    if csizes is None:
-        csizes = torch.empty(n, dtype=torch.int64, device=dev)
-    if kinds is None:
-        kinds = torch.empty(n, dtype=torch.uint8, device=dev)
-    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64); _check(kinds, torch.uint8)
-    assert offsets.numel() == n + 1 and csizes.numel() == n and kinds.numel() == n and out.device == dev, (offsets.numel(), n)
-    fn_name = "FSEB200_HUF_compress_mixed_repeat_chains_packed"
-    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, out.data_ptr(), out.numel(), offsets.data_ptr(),
-                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(),
-                                single, ctables.data_ptr(), repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(),
-                                max_symbol_value, table_log, _stream_ptr())
-    _ret(r, fn_name)
-    return out, offsets, csizes, kinds
+    return _repeat_chains_packed("FSEB200_HUF_compress_mixed_repeat_chains_packed", chain_starts, src_ptrs, src_sizes, prefer,
+                                 single_stream, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds,
+                                 (max_symbol_value, table_log))
 
 
 def huf_compress_literals_chains_packed(chain_starts, src_ptrs, src_sizes, prefer, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes,
@@ -435,54 +393,17 @@ def huf_compress_literals_chains_packed(chain_starts, src_ptrs, src_sizes, prefe
     equal, and keeps a step's table and flag only for a block stored with its own header.  The other arguments are the mixed
     call's.  Returns (out, offsets, csizes, kinds, single_stream): single_stream (uint8) holds the forms it chose, so the stream
     decodes with huf_decompress_mixed_repeat_packed."""
-    from . import lib
-    n = _blocks_args(src_ptrs, src_sizes)
-    dev = src_ptrs.device
-    _check(prefer, torch.int32)
-    assert prefer.numel() == n and prefer.device == dev, (prefer.numel(), n, prefer.device)
-    n_chains = _chain_args(chain_starts, dev, ((ctables, torch.int64), (repeats, torch.int32), (chain_hdr_ptrs, torch.int64),
-                                               (chain_hdr_sizes, torch.int64)))
-    if out is None:
-        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
-    if offsets is None:
-        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    if csizes is None:
-        csizes = torch.empty(n, dtype=torch.int64, device=dev)
-    if kinds is None:
-        kinds = torch.empty(n, dtype=torch.uint8, device=dev)
-    if single_stream is None:
-        single_stream = torch.empty(n, dtype=torch.uint8, device=dev)
-    single = _single_arg(single_stream, n, dev)
-    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64); _check(kinds, torch.uint8)
-    assert offsets.numel() == n + 1 and csizes.numel() == n and kinds.numel() == n and out.device == dev, (offsets.numel(), n)
-    fn_name = "FSEB200_HUF_compress_literals_chains_packed"
-    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, out.data_ptr(), out.numel(), offsets.data_ptr(),
-                                csizes.data_ptr(), kinds.data_ptr(), src_ptrs.data_ptr(), src_sizes.data_ptr(), prefer.data_ptr(),
-                                single, ctables.data_ptr(), repeats.data_ptr(), chain_hdr_ptrs.data_ptr(), chain_hdr_sizes.data_ptr(),
-                                max_symbol_value, table_log, min_literals, min_gain_log, _stream_ptr())
-    _ret(r, fn_name)
-    return out, offsets, csizes, kinds, single_stream
+    return _repeat_chains_packed("FSEB200_HUF_compress_literals_chains_packed", chain_starts, src_ptrs, src_sizes, prefer,
+                                 single_stream, ctables, repeats, chain_hdr_ptrs, chain_hdr_sizes, out, offsets, csizes, kinds,
+                                 (max_symbol_value, table_log, min_literals, min_gain_log), forms_out=True)
 
 
 def huf_decompress_mixed_repeat_packed(chain_starts, packed, offsets, kinds, single_stream, chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs,
                                        dst_sizes, results=None):
     """huf_decompress_repeat_packed over a buffer huf_compress_mixed_repeat_chains_packed wrote, each block in the form
     single_stream[b] names.  Returns results (int64)."""
-    from . import lib
-    n = _blocks_args(dst_ptrs, dst_sizes)
-    dev = dst_ptrs.device
-    n_chains = _chain_args(chain_starts, dev, ((chain_hdr_ptrs, torch.int64), (chain_hdr_sizes, torch.int64)))
-    single = _single_arg(single_stream, n, dev)
-    if results is None:
-        results = torch.empty(n, dtype=torch.int64, device=dev)
-    _check(packed, torch.uint8); _check(offsets, torch.int64); _check(kinds, torch.uint8); _check(results, torch.int64)
-    assert offsets.numel() == n + 1 and kinds.numel() == n and results.numel() == n and packed.device == dev, (offsets.numel(), n)
-    fn_name = "FSEB200_HUF_decompress_mixed_repeat_packed"
-    r = getattr(lib(), fn_name)(n_chains, chain_starts.data_ptr(), n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(),
-                                packed.data_ptr(), offsets.data_ptr(), kinds.data_ptr(), single, chain_hdr_ptrs.data_ptr(),
-                                chain_hdr_sizes.data_ptr(), _stream_ptr())
-    _ret(r, fn_name)
-    return results
+    return _repeat_unpack("FSEB200_HUF_decompress_mixed_repeat_packed", chain_starts, packed, offsets, kinds, single_stream,
+                          chain_hdr_ptrs, chain_hdr_sizes, dst_ptrs, dst_sizes, results)
 
 
 def huf_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, max_symbol_value=255, table_log=12):

@@ -250,14 +250,16 @@ FSEB_API size_t FSEB200_HUF_compress1X_repeat_blocks(size_t nBlocks, void* const
 }
 // Chains: blocks of one stream in one call, the stream's state carried from block to block on the device (common.cuh ChainDescs).
 namespace {
+// nStreams 4 or 1: every block in that form; 0: mixed, each block's form in dSingleStream, which must then be given
+bool forms_given(int nStreams, const void* dSingleStream) { return nStreams || dSingleStream; }
 size_t huf_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities,
                          size_t* dCSizes, const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
                          unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
                          const void** dHeaders, size_t* dHeaderSizes, int nStreams, unsigned msv, unsigned tlog, void* stream,
-                         const unsigned char* dSingleStream = nullptr)           // nStreams 0: mixed, the form per block
+                         const unsigned char* dSingleStream = nullptr)
 {
     if (nBlocks && (nChains > 0xFFFFFFFFull || !dChainStarts || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders ||
-                    !dChainHeaderSizes || !dHeaders || !dHeaderSizes || (!nStreams && !dSingleStream))) return (size_t)err(E_SRC_WRONG);
+                    !dChainHeaderSizes || !dHeaders || !dHeaderSizes || !forms_given(nStreams, dSingleStream))) return (size_t)err(E_SRC_WRONG);
     return blocks_call(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes, [&](const BlockDescs& d) {
         ChainMixedDescs g;
         static_cast<BlockDescs&>(g) = d;
@@ -319,31 +321,49 @@ void chain_packed_descs(ChainPackedDescs& g, size_t nChains, const size_t* dChai
     g.pk.src = g.src; g.pk.srcSize = g.srcSize; g.pk.nBlocks = g.nBlocks;
     g.kind = dKinds; g.end = nullptr; g.malformed = nullptr;
 }
+// The form of a packed chain compress: every block in nStreams streams (4 or 1), or (0) each block's form in dSingleStream --
+// read, or under zstd's literal policy (`literals`, with minLiterals and minGainLog) chosen by the device and written there.
+struct ChainForm {
+    int nStreams;
+    unsigned char* dSingleStream;
+    bool literals;
+    unsigned minLiterals, minGainLog;
+};
 size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut, size_t outCapacity,
                                 size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs,
                                 const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats,
-                                const void** dChainHeaders, size_t* dChainHeaderSizes, int nStreams, unsigned msv, unsigned tlog,
-                                void* stream, const unsigned char* dSingleStream = nullptr)   // nStreams 0: mixed, the form per block
+                                const void** dChainHeaders, size_t* dChainHeaderSizes, const ChainForm& f, unsigned msv, unsigned tlog,
+                                void* stream)
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dOut || !dOffsets || !dCSizes || !dKinds || !dSrcs ||
-        !dSrcSizes || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes || (!nStreams && !dSingleStream))
+        !dSrcSizes || !dPreferRepeat || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes ||
+        !forms_given(f.nStreams, f.dSingleStream) || (f.literals && (f.minGainLog < 1 || f.minGainLog > 31)))
         return (size_t)err(E_SRC_WRONG);
-    ChainPackedMixedDescs g;
-    chain_packed_descs(g, nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes, dPreferRepeat,
+    ChainPackedDescs d;
+    chain_packed_descs(d, nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes, dPreferRepeat,
                        dCTables, dRepeats, dChainHeaders, dChainHeaderSizes);
-    g.single = dSingleStream;
-    return ok_or_generic(nStreams ? launch_huf_encode_chains_packed(g, nStreams, msv, tlog, (cudaStream_t)stream)
-                                  : launch_huf_encode_chains_packed_mixed(g, msv, tlog, (cudaStream_t)stream));
+    if (f.literals) {
+        ChainPackedLiteralsDescs g;
+        static_cast<ChainPackedDescs&>(g) = d;
+        g.single = f.dSingleStream; g.minLiterals = f.minLiterals; g.minGainLog = f.minGainLog;
+        return ok_or_generic(launch_huf_encode_literals_chains_packed(g, msv, tlog, (cudaStream_t)stream));
+    }
+    ChainPackedMixedDescs g;
+    static_cast<ChainPackedDescs&>(g) = d;
+    g.single = f.dSingleStream;
+    return ok_or_generic(f.nStreams ? launch_huf_encode_chains_packed(g, f.nStreams, msv, tlog, (cudaStream_t)stream)
+                                    : launch_huf_encode_chains_packed_mixed(g, msv, tlog, (cudaStream_t)stream));
 }
 size_t huf_repeat_unpack(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstSizes,
                          size_t* dResults, const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
                          const void* const* dChainHeaders, const size_t* dChainHeaderSizes, int nStreams, void* stream,
-                         const unsigned char* dSingleStream = nullptr)           // nStreams 0: mixed, the form per block
+                         const unsigned char* dSingleStream = nullptr)
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dDsts || !dDstSizes || !dResults || !dIn ||
-        !dOffsets || !dKinds || !dChainHeaders || !dChainHeaderSizes || (!nStreams && !dSingleStream)) return (size_t)err(E_SRC_WRONG);
+        !dOffsets || !dKinds || !dChainHeaders || !dChainHeaderSizes || !forms_given(nStreams, dSingleStream))
+        return (size_t)err(E_SRC_WRONG);
     return ok_or_generic(launch_huf_decompress_repeat_packed((const u64*)dChainStarts, (u32)nChains, (u8* const*)dDsts,
                                                              (const u64*)dDstSizes, (u64*)dResults, (const u8*)dIn,
                                                              (const u64*)dOffsets, dKinds, (const u8* const*)dChainHeaders,
@@ -358,7 +378,8 @@ FSEB_API size_t FSEB200_HUF_compress4X_repeat_chains_packed(size_t nChains, cons
                                                             size_t* dChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
     return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
-                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 4, maxSymbolValue, tableLog, stream);
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, ChainForm{4}, maxSymbolValue,
+                                    tableLog, stream);
 }
 FSEB_API size_t FSEB200_HUF_compress1X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
                                                             size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
@@ -367,7 +388,8 @@ FSEB_API size_t FSEB200_HUF_compress1X_repeat_chains_packed(size_t nChains, cons
                                                             size_t* dChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
     return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
-                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 1, maxSymbolValue, tableLog, stream);
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, ChainForm{1}, maxSymbolValue,
+                                    tableLog, stream);
 }
 FSEB_API size_t FSEB200_HUF_decompress4X_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
                                                        const size_t* dDstSizes, size_t* dResults, const void* dIn, const size_t* dOffsets,
@@ -393,8 +415,8 @@ FSEB_API size_t FSEB200_HUF_compress_mixed_repeat_chains_packed(size_t nChains, 
                                                                 unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
     return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
-                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes, 0, maxSymbolValue, tableLog, stream,
-                                    dSingleStream);
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes,
+                                    ChainForm{0, const_cast<unsigned char*>(dSingleStream)}, maxSymbolValue, tableLog, stream);
 }
 FSEB_API size_t FSEB200_HUF_compress_literals_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
                                                             size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
@@ -403,15 +425,9 @@ FSEB_API size_t FSEB200_HUF_compress_literals_chains_packed(size_t nChains, cons
                                                             const void** dChainHeaders, size_t* dChainHeaderSizes, unsigned maxSymbolValue,
                                                             unsigned tableLog, unsigned minLiterals, unsigned minGainLog, void* stream)
 {
-    if (nBlocks == 0) return 0;
-    if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dOut || !dOffsets || !dCSizes || !dKinds || !dSrcs ||
-        !dSrcSizes || !dPreferRepeat || !dSingleStream || !dCTables || !dRepeats || !dChainHeaders || !dChainHeaderSizes ||
-        minGainLog < 1 || minGainLog > 31) return (size_t)err(E_SRC_WRONG);
-    ChainPackedLiteralsDescs g;
-    chain_packed_descs(g, nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes, dPreferRepeat,
-                       dCTables, dRepeats, dChainHeaders, dChainHeaderSizes);
-    g.single = dSingleStream; g.minLiterals = minLiterals; g.minGainLog = minGainLog;
-    return ok_or_generic(launch_huf_encode_literals_chains_packed(g, maxSymbolValue, tableLog, (cudaStream_t)stream));
+    return huf_repeat_chains_packed(nChains, dChainStarts, nBlocks, dOut, outCapacity, dOffsets, dCSizes, dKinds, dSrcs, dSrcSizes,
+                                    dPreferRepeat, dCTables, dRepeats, dChainHeaders, dChainHeaderSizes,
+                                    ChainForm{0, dSingleStream, true, minLiterals, minGainLog}, maxSymbolValue, tableLog, stream);
 }
 FSEB_API size_t FSEB200_HUF_decompress_mixed_repeat_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts,
                                                            const size_t* dDstSizes, size_t* dResults, const void* dIn, const size_t* dOffsets,

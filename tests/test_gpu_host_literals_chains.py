@@ -21,13 +21,10 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import torch                                                                       # noqa: E402
 
-from test_gpu_blocks import CANARY                                                 # noqa: E402
 from huf_chain_packed_cases import at_bound, resolve_headers                       # noqa: E402
 from huf_literals_chain_cases import literal_chains, built_chains, long_literal_chain   # noqa: E402
-from test_gpu_huf_repeat_packed import _ref, FILL                                  # noqa: E402
-from test_gpu_huf_literals_chains import Literals, regenerable                    # noqa: E402
-from test_gpu_host_packed import host_buffer                                       # noqa: E402
-from test_gpu_host_chains import HostState, _sources, _first_blocks, BLOCK_OVERHEAD   # noqa: E402
+from huf_chain_harness import (PackedChains, literals, compare_compress, regenerable, host_buffer, _sources,  # noqa: E402
+                               _first_blocks, _ref, BLOCK_OVERHEAD, CANARY, FILL)
 import finitestateentropy_b200 as fb                                               # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -35,45 +32,6 @@ pytestmark = pytest.mark.gpu
 
 def _chains(ref, step=9):
     return literal_chains(ref, 255, 11)[::step] + built_chains(ref) + at_bound([long_literal_chain(ref, 96)])
-
-
-def host_compress(run, cap, pinned, off):
-    srcs = _sources(run)
-    data = np.concatenate(srcs + [np.zeros(0, np.uint8)])
-    _, src = host_buffer(len(data), pinned, off + 2)
-    src.copy_(torch.from_numpy(data))
-    oarena, out = host_buffer(cap, pinned, off, fill=FILL)
-    st = HostState(run)
-    prefer = torch.tensor([run.chains[c]["blocks"][i]["prefer"] for c, i in run.blocks], dtype=torch.int32)
-    _, offs, cs, kinds, forms, _ = fb.host_compress_literals_chains_packed(src, [len(s) for s in srcs], run.starts, prefer, st.tables,
-                                                                           st.flags, st.hp, st.hs, out=out, max_symbol_value=run.msv,
-                                                                           table_log=run.tlog, min_literals=run.ml,
-                                                                           min_gain_log=run.mgl)
-    assert np.array_equal(src.numpy(), data)
-    return (oarena, out, offs.numpy().view(np.uint64).copy(), cs.numpy().view(np.uint64).copy(), kinds.numpy().copy(),
-            forms.numpy().copy(), st)
-
-
-def compare_compress(run, cap, pinned=True, off=1):
-    run.reset()
-    _, dout, doff, dcs, dkinds, dforms, _ = run.call(cap=cap)
-    dstate = run.state()
-    oarena, out, offs, cs, kinds, forms, st = host_compress(run, cap, pinned, off)
-    assert np.array_equal(cs, dcs) and np.array_equal(kinds, dkinds) and np.array_equal(offs, doff)
-    assert np.array_equal(forms, dforms)
-    assert np.array_equal(out.numpy(), dout.cpu().numpy()), cap
-    o = oarena.numpy()
-    assert (o[:CANARY + off] == FILL).all() and (o[CANARY + off + cap:] == FILL).all(), "sentinels around hOut"
-    tabs = st.tables.numpy().view(np.uint32)
-    for c in range(len(run.chains)):
-        assert np.array_equal(tabs[c], dstate["tabs"][run.toff[c]:run.toff[c] + 256]), c
-    assert np.array_equal(st.flags.numpy(), dstate["rep"])
-    hp, hs = st.hp.numpy().view(np.uint64), st.hs.numpy().view(np.uint64)
-    for c in range(len(run.chains)):
-        dp = int(dstate["chp"][c])
-        want = st.entry[c] if dp == run.hdrs.ptr(c) else out.data_ptr() + (dp - dout.data_ptr())
-        assert (int(hp[c]), int(hs[c])) == (want, int(dstate["chs"][c])), c
-    return out, offs, cs, kinds, forms
 
 
 def host_round_trip(run, out, offs, kinds, forms, pinned=False, off=3):
@@ -105,7 +63,8 @@ def host_round_trip(run, out, offs, kinds, forms, pinned=False, off=3):
 @pytest.mark.parametrize("pinned", [True, False], ids=["pinned", "pageable"])
 def test_matches_the_device_call(pinned):
     ref = _ref()
-    run = Literals(ref, _chains(ref, 5 if pinned else 7), 255 if pinned else 200, 11, *((64, 6) if pinned else (8, 8)))
+    run = PackedChains(literals(*((64, 6) if pinned else (8, 8))), ref, _chains(ref, 5 if pinned else 7), 255 if pinned else 200,
+                       11)
     total = sum(len(s) for s in _sources(run))
     out, offs, cs, kinds, forms = compare_compress(run, total + 32, pinned=pinned, off=1 if pinned else 5)
     assert list(kinds) == run.kinds and list(forms) == run.flags
@@ -121,7 +80,7 @@ def _rolled_back_crossings(run, budget):
     seen = 0
     for b0 in firsts[1:]:
         c, i = run.blocks[b0]
-        if i > 0 and run.kinds[b0 - 1] in (0, 1) and len(srcs[b0 - 1]) >= run.ml and run.kinds[b0] in (2, 3):
+        if i > 0 and run.kinds[b0 - 1] in (0, 1) and len(srcs[b0 - 1]) >= run.form.kw["min_literals"] and run.kinds[b0] in (2, 3):
             seen += 1
     return seen
 
@@ -142,7 +101,7 @@ def test_chunk_budgets():
 def _child():
     ref = _ref()
     budget = int(os.environ["FSEB200_HOST_PACKED_CHUNK_BYTES"])
-    run = Literals(ref, _chains(ref, 11), 255, 11, 8, 8)
+    run = PackedChains(literals(8, 8), ref, _chains(ref, 11), 255, 11)
     total = sum(len(s) for s in _sources(run))
     out, offs, cs, kinds, forms = compare_compress(run, total + 32, pinned=True, off=1)
     host_round_trip(run, out, offs, kinds, forms, pinned=False, off=5)

@@ -23,16 +23,11 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import torch                                                                       # noqa: E402
 
-from test_gpu_blocks import CANARY                                                 # noqa: E402
 from huf_chain_cases import drift_chains                                           # noqa: E402
 from huf_chain_packed_cases import at_bound, resolve_headers                       # noqa: E402
 from huf_mixed_chain_cases import with_flags, ragged_chains, long_mixed_chain, built_chains   # noqa: E402
-from test_gpu_huf_repeat import Arena                                              # noqa: E402
-from test_gpu_huf_repeat_packed import regenerable, _t, _ref, FILL                 # noqa: E402
-from test_gpu_huf_mixed_chains import Mixed, decode_mixed                          # noqa: E402
-from test_gpu_host_packed import host_buffer                                       # noqa: E402
-from test_gpu_host_chains import HostState, _sources, _first_blocks, BLOCK_OVERHEAD   # noqa: E402
-import finitestateentropy_b200 as fb                                               # noqa: E402
+from huf_chain_harness import (MIXED, PackedChains, host_compress, compare_compress, compare_decompress, _sources,  # noqa: E402
+                               _first_blocks, _ref, BLOCK_OVERHEAD)
 
 pytestmark = pytest.mark.gpu
 
@@ -42,83 +37,11 @@ def _chains(ref, n_drift=6, seed=0):
             + built_chains(ref)[:2] + at_bound([long_mixed_chain(ref, 64)]))
 
 
-def host_compress(run, cap, pinned, off):
-    srcs = _sources(run)
-    data = np.concatenate(srcs + [np.zeros(0, np.uint8)])
-    _, src = host_buffer(len(data), pinned, off + 2)
-    src.copy_(torch.from_numpy(data))
-    oarena, out = host_buffer(cap, pinned, off, fill=FILL)
-    st = HostState(run)
-    prefer = torch.tensor([run.chains[c]["blocks"][i]["prefer"] for c, i in run.blocks], dtype=torch.int32)
-    single = torch.tensor(run.flags, dtype=torch.uint8)
-    _, offs, cs, kinds, _ = fb.host_compress_mixed_repeat_chains_packed(src, [len(s) for s in srcs], run.starts, prefer, single,
-                                                                        st.tables, st.flags, st.hp, st.hs, out=out,
-                                                                        max_symbol_value=run.msv, table_log=run.tlog)
-    assert np.array_equal(src.numpy(), data)
-    return oarena, out, offs.numpy().view(np.uint64).copy(), cs.numpy().view(np.uint64).copy(), kinds.numpy().copy(), st
-
-
-def compare_compress(run, cap, pinned=True, off=1):
-    run.reset()
-    _, dout, doff, dcs, dkinds, _ = run.call(cap=cap)
-    dstate = run.state()
-    oarena, out, offs, cs, kinds, st = host_compress(run, cap, pinned, off)
-    assert np.array_equal(cs, dcs) and np.array_equal(kinds, dkinds) and np.array_equal(offs, doff)
-    assert np.array_equal(out.numpy(), dout.cpu().numpy()), cap
-    o = oarena.numpy()
-    assert (o[:CANARY + off] == FILL).all() and (o[CANARY + off + cap:] == FILL).all(), "sentinels around hOut"
-    tabs = st.tables.numpy().view(np.uint32)
-    for c in range(len(run.chains)):
-        assert np.array_equal(tabs[c], dstate["tabs"][run.toff[c]:run.toff[c] + 256]), c
-    assert np.array_equal(st.flags.numpy(), dstate["rep"])
-    hp, hs = st.hp.numpy().view(np.uint64), st.hs.numpy().view(np.uint64)
-    for c in range(len(run.chains)):
-        dp = int(dstate["chp"][c])
-        want = st.entry[c] if dp == run.hdrs.ptr(c) else out.data_ptr() + (dp - dout.data_ptr())
-        assert (int(hp[c]), int(hs[c])) == (want, int(dstate["chs"][c])), c
-    return out, offs, cs, kinds
-
-
-def compare_decompress(run, out, offs, kinds, pinned=True, off=3):
-    srcs = _sources(run)
-    sizes = [len(s) for s in srcs]
-    total = int(offs[-1])
-    packed = out.numpy()[:total].copy()
-    _, inp = host_buffer(total, pinned, off + 4)
-    inp.copy_(torch.from_numpy(packed))
-    hblobs = [np.ascontiguousarray(b, np.uint8) for b, _ in run.hdr_blobs]
-    hp = torch.tensor([b.ctypes.data for b in hblobs], dtype=torch.int64)
-    hs = torch.tensor([len(b) for b in hblobs], dtype=torch.int64)
-    darena, dst = host_buffer(sum(sizes), pinned, off, fill=FILL)
-    single = torch.tensor(run.flags, dtype=torch.uint8)
-    _, res = fb.host_decompress_mixed_repeat_packed(inp, torch.from_numpy(offs.view(np.int64).copy()), torch.from_numpy(kinds.copy()),
-                                                    single, run.starts, sizes, hp, hs, out=dst)
-    r = res.numpy().view(np.uint64)
-    dh = Arena()
-    for b in hblobs:
-        dh.add(b, skew=1)
-    dh.upload()
-    dev_in = torch.from_numpy(np.concatenate([packed, np.zeros(64, np.uint8)])).cuda()
-    want, _ = decode_mixed(_t(run.starts), dev_in, _t(offs), _t(kinds, torch.uint8), run.sg, _t([dh.ptr(c) for c in range(len(hblobs))]),
-                           _t([len(b) for b in hblobs]), sizes)
-    assert np.array_equal(r, want), [(b, int(r[b]), int(want[b])) for b in range(len(r)) if r[b] != want[b]][:8]
-    d = darena.numpy()
-    assert (d[:CANARY + off] == FILL).all() and (d[CANARY + off + sum(sizes):] == FILL).all(), "sentinels around hDst"
-    rh = resolve_headers(kinds, run.starts)
-    start, n_ok = 0, 0
-    for k, s in enumerate(srcs):
-        if regenerable(run, k, rh, lambda c: not run.hdr_blobs[c][1]):
-            assert int(r[k]) == len(s) and np.array_equal(d[CANARY + off + start: CANARY + off + start + len(s)], s), k
-            n_ok += 1
-        start += len(s)
-    return r, n_ok
-
-
 @pytest.mark.parametrize("pinned", [True, False], ids=["pinned", "pageable"])
 def test_matches_the_device_calls(pinned):
     ref = _ref()
     msv, tlog = (255, 11) if pinned else (200, 11)
-    run = Mixed(ref, _chains(ref, 2, seed=1 if pinned else 2), msv, tlog)
+    run = PackedChains(MIXED, ref, _chains(ref, 2, seed=1 if pinned else 2), msv, tlog)
     total = sum(len(s) for s in _sources(run))
     out, offs, cs, kinds = compare_compress(run, total + 32, pinned=pinned, off=1 if pinned else 5)
     assert list(kinds) == run.kinds
@@ -130,7 +53,8 @@ def test_matches_the_device_calls(pinned):
 def test_two_threads():
     """two host threads run the mixed pair on different chains at once: both give what one thread alone gives"""
     ref = _ref()
-    runs = [Mixed(ref, _chains(ref, 3, seed=3), 255, 11), Mixed(ref, at_bound([long_mixed_chain(ref, 200)]), 255, 11)]
+    runs = [PackedChains(MIXED, ref, _chains(ref, 3, seed=3), 255, 11),
+            PackedChains(MIXED, ref, at_bound([long_mixed_chain(ref, 200)]), 255, 11)]
     alone = []
     for run in runs:
         out, offs, cs, kinds, st = host_compress(run, sum(len(s) for s in _sources(run)) + 32, True, 1)[1:]
@@ -191,7 +115,7 @@ def test_chunk_budgets():
 def _child():
     ref = _ref()
     budget = int(os.environ["FSEB200_HOST_PACKED_CHUNK_BYTES"])
-    run = Mixed(ref, _chains(ref, 6, seed=5), 255, 11)
+    run = PackedChains(MIXED, ref, _chains(ref, 6, seed=5), 255, 11)
     total = sum(len(s) for s in _sources(run))
     out, offs, cs, kinds = compare_compress(run, total + 32, pinned=True, off=1)
     compare_decompress(run, out, offs, kinds, pinned=False, off=5)

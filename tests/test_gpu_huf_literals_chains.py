@@ -12,129 +12,19 @@ import torch
 
 from helpers import is_error
 from huf_repeat_cases import main_configs
-from huf_chain_cases import chain_header
 from huf_chain_packed_cases import at_bound, resolve_headers
-from huf_literals_chain_cases import (ref_literals_chain, expected_literals, literal_chains, built_chains, long_literal_chain,
-                                      POLICIES)
-from test_gpu_huf_repeat import Arena
-from test_gpu_huf_repeat_chains import _dev, _view, _guards_ok
-from test_gpu_huf_repeat_packed import Packed, _t, _u64, EDGE, FILL, SRC_WRONG, TOO_SMALL
-from test_gpu_huf_mixed_chains import decode_mixed
+from huf_literals_chain_cases import literal_chains, built_chains, long_literal_chain, POLICIES
+from huf_chain_harness import (MIXED, PackedChains, literals, decode, regenerable, _ref, _t, _u64, _view, FILL, SRC_WRONG,
+                               TOO_SMALL)
 import finitestateentropy_b200 as fb
 
 pytestmark = pytest.mark.gpu
 
 
-def _ref():
-    from huf_repeat_cases import ref_lib
-    ref = ref_lib()
-    if ref is None:
-        pytest.skip("compiled reference not available")
-    return ref
-
-
-class Literals(Packed):
-    """Packed's state handling on the literal-policy call: the policy loop, and calls of huf_compress_literals_chains_packed"""
-
-    def __init__(self, ref, chains, msv, tlog, min_lit, min_gain_log):
-        self.ref, self.four, self.chains, self.msv, self.tlog = ref, None, chains, msv, tlog
-        self.ml, self.mgl = min_lit, min_gain_log
-        self.want = [ref_literals_chain(ref, ch, msv, tlog, min_lit, min_gain_log) for ch in chains]
-        self.vals, self.kinds, self.blobs, self.flags, self.starts = expected_literals(self.want, chains)
-        self.blocks = [(c, i) for c, ch in enumerate(chains) for i in range(len(ch["blocks"]))]
-        self.first = self.starts[:-1]
-        srcs, hdrs = Arena(), Arena()
-        for k, (c, i) in enumerate(self.blocks):
-            srcs.add(chains[c]["blocks"][i]["src"], skew=k % 3)
-        self.hdr_blobs = [chain_header(ref, ch) for ch in chains]
-        for blob, _ in self.hdr_blobs:
-            hdrs.add(blob)
-        self.srcs, self.hdrs = srcs.upload(), hdrs.upload()
-        n = len(self.blocks)
-        self.sizes = [len(chains[c]["blocks"][i]["src"]) for c, i in self.blocks]
-        self.sp = torch.tensor([srcs.ptr(k) for k in range(n)] or [0], dtype=torch.int64, device="cuda")[:n]
-        self.ss = torch.tensor(self.sizes or [0], dtype=torch.int64, device="cuda")[:n]
-        self.pr = torch.tensor([chains[c]["blocks"][i]["prefer"] for c, i in self.blocks] or [0], dtype=torch.int32, device="cuda")[:n]
-        self.reset()
-
-    def call(self, cap=None, parts=None, starts=None, stream=None, skew=3):
-        """one call over blocks parts[c] = (lo, hi) of each chain into `cap` bytes with guards around the output, the kinds and
-        the form flags.  Returns (buf, out, offsets, csizes, kinds, forms, idx)."""
-        parts = parts or [(0, len(ch["blocks"])) for ch in self.chains]
-        idx, st = [], [0]
-        for c, (lo, hi) in enumerate(parts):
-            idx += [self.first[c] + i for i in range(lo, hi)]
-            st.append(len(idx))
-        if starts is not None:
-            st = starts
-        ix = torch.tensor(idx or [0], dtype=torch.int64, device="cuda")[:len(idx)]
-        if cap is None:
-            cap = int(self.ss[ix].sum()) + 32
-        buf = torch.full((cap + 2 * EDGE + skew,), FILL, dtype=torch.uint8, device="cuda")
-        out = buf[EDGE + skew:EDGE + skew + cap]
-        off, cs = _dev([0xCD] * (len(idx) + 1)), _dev([0xCD] * len(idx))
-        kinds = torch.full((len(idx) + 16,), 0xEE, dtype=torch.uint8, device="cuda")
-        forms = torch.full((len(idx) + 16,), 0xEE, dtype=torch.uint8, device="cuda")
-        sv = _dev(st)
-        with torch.cuda.stream(stream or torch.cuda.current_stream()):
-            fb.huf_compress_literals_chains_packed(_view(sv), self.sp[ix], self.ss[ix], self.pr[ix], _view(self.ctp), _view(self.rep),
-                                                   _view(self.chp), _view(self.chs), out=out, offsets=_view(off), csizes=_view(cs),
-                                                   kinds=kinds[8:8 + len(idx)], single_stream=forms[8:8 + len(idx)],
-                                                   max_symbol_value=self.msv, table_log=self.tlog, min_literals=self.ml,
-                                                   min_gain_log=self.mgl)
-        torch.cuda.synchronize()
-        for t in (off, cs, sv, self.ctp, self.rep, self.chp, self.chs):
-            assert _guards_ok(t)
-        kh, fh = kinds.cpu().numpy(), forms.cpu().numpy()
-        for g in (kh, fh):
-            assert (g[:8] == 0xEE).all() and (g[-8:] == 0xEE).all()
-        return buf, out, _u64(_view(off)), _u64(_view(cs)), kh[8:8 + len(idx)], fh[8:8 + len(idx)], idx
-
-    def check_one_call(self, res):
-        """a whole-batch call that fits: values, kinds, forms, offsets, stored bytes, guards, and each chain's final table (written
-        only if a kind-2 block committed one), flag and header"""
-        buf, out, off, cs, kinds, forms, idx = res
-        n = len(idx)
-        bad = [k for k in range(n) if int(cs[k]) != self.vals[k] or kinds[k] != self.kinds[k] or forms[k] != self.flags[k]]
-        assert not bad, [(self.chains[self.blocks[k][0]]["name"], self.blocks[k][1], int(cs[k]), self.vals[k], int(kinds[k]),
-                          self.kinds[k], int(forms[k]), self.flags[k]) for k in bad[:6]]
-        lens = [len(b) for b in self.blobs]
-        assert list(off) == list(np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64)), "offsets"
-        host = buf.cpu().numpy()
-        o0 = out.data_ptr() - buf.data_ptr()
-        for k in range(n):
-            assert (host[o0 + int(off[k]):o0 + int(off[k + 1])] == self.blobs[k]).all(), (k, self.blocks[k])
-        assert (host[:o0] == FILL).all() and (host[o0 + int(off[n]):] == FILL).all()
-        s = self.state()
-        for c, ch in enumerate(self.chains):
-            per, (T, F, H) = self.want[c]
-            t = s["tabs"][self.toff[c]:self.toff[c] + 256]
-            committed = any(x["kind"] == 2 for x in per)
-            assert (t == (T & 0x00FFFFFF if committed else ch["table"])).all(), ch["name"]
-            assert int(s["rep"][c]) == F, ch["name"]
-            if H[0] == "chain":
-                hv = (self.hdrs.ptr(c), len(self.hdr_blobs[c][0]))
-            else:
-                k = self.first[c] + H[1]
-                hv = (out.data_ptr() + int(off[k]), int(cs[k]))
-            assert (int(s["chp"][c]), int(s["chs"][c])) == hv, ch["name"]
-        return s
-
-
-def regenerable(run, k, heads):
-    """whether block k must decode back to its source: stored (kind 0 to 3), not RLE by the n >= 8 rule over unequal bytes, and
-    not a kind-3 block whose entry header is a stand-in"""
-    c, i = run.blocks[k]
-    src, kind = run.chains[c]["blocks"][i]["src"], run.kinds[k]
-    if kind == 4 or (kind == 1 and not (src == src[0]).all()):
-        return False
-    return not (heads[k] is not None and heads[k][0] == "chain" and not run.hdr_blobs[c][1])
-
-
 def round_trip(run, out, off, kinds, forms, stream=None):
     """the mixed packed decoder with the written forms; every regenerable block comes back.  Returns the count."""
-    res, regions = decode_mixed(_t(run.starts), out, _t(off), _t(kinds, torch.uint8), _t(forms, torch.uint8), _view(run.chp),
-                                _view(run.chs), run.sizes, stream=stream)
+    res, regions = decode(MIXED, _t(run.starts), out, _t(off), _t(kinds, torch.uint8), _t(forms, torch.uint8), _view(run.chp),
+                          _view(run.chs), run.sizes, stream=stream)
     heads = resolve_headers(kinds, run.starts)
     ok = 0
     for k, (c, i) in enumerate(run.blocks):
@@ -154,7 +44,7 @@ def round_trip(run, out, off, kinds, forms, stream=None):
 @pytest.mark.parametrize("msv,tlog", main_configs())
 def test_compress_matches_the_policy_loop(msv, tlog, policy):
     ref = _ref()
-    run = Literals(ref, literal_chains(ref, msv, tlog, seed=policy[1]), msv, tlog, *policy)
+    run = PackedChains(literals(*policy), ref, literal_chains(ref, msv, tlog, seed=policy[1]), msv, tlog)
     assert {0, 1, 2, 3, 4} <= set(run.kinds) and set(run.flags) == {0, 1}
     res = run.call(stream=torch.cuda.Stream())
     run.check_one_call(res)
@@ -167,7 +57,7 @@ def test_built_chains_at_every_policy():
     """the built chains alone, so that a rule's block is compared at every policy and not only among many chains"""
     ref = _ref()
     for policy in POLICIES + ((0, 6), (16, 7)):
-        run = Literals(ref, built_chains(ref), 255, 11, *policy)
+        run = PackedChains(literals(*policy), ref, built_chains(ref), 255, 11)
         res = run.call()
         run.check_one_call(res)
         run.reset()
@@ -176,7 +66,7 @@ def test_built_chains_at_every_policy():
 
 def test_capacity_at_block_ends():
     ref = _ref()
-    run = Literals(ref, literal_chains(ref, 255, 11)[::17] + built_chains(ref), 255, 11, 8, 8)
+    run = PackedChains(literals(8, 8), ref, literal_chains(ref, 255, 11)[::17] + built_chains(ref), 255, 11)
     whole = run.call()
     run.check_one_call(whole)
     ends = whole[2]
@@ -211,9 +101,9 @@ def test_split_calls_carry_the_state():
     """each chain cut into two calls right after a block the policy rolled back: the second call's results equal one call's"""
     ref = _ref()
     chains = built_chains(ref)
-    one = Literals(ref, chains, 255, 11, 8, 8)
+    one = PackedChains(literals(8, 8), ref, chains, 255, 11)
     one.check_one_call(one.call())
-    two = Literals(ref, chains, 255, 11, 8, 8)
+    two = PackedChains(literals(8, 8), ref, chains, 255, 11)
     mids = [max(1, len(ch["blocks"]) // 2) if len(ch["blocks"]) > 1 else 1 for ch in chains]
     rolled = [k for k in range(len(one.blocks)) if one.blocks[k][1] == mids[one.blocks[k][0]] - 1 and one.kinds[k] == 0
               and chains[one.blocks[k][0]]["name"].startswith("rollback")]
@@ -235,7 +125,7 @@ def test_split_calls_carry_the_state():
 
 def test_malformed_geometry_writes_only_values_and_kinds():
     ref = _ref()
-    run = Literals(ref, built_chains(ref), 255, 12, 64, 6)
+    run = PackedChains(literals(64, 6), ref, built_chains(ref), 255, 12)
     nb = len(run.blocks)
     good = run.starts
     before = run.state()
@@ -251,7 +141,7 @@ def test_malformed_geometry_writes_only_values_and_kinds():
 
 def test_ordered_on_a_side_stream():
     ref = _ref()
-    run = Literals(ref, built_chains(ref) + literal_chains(ref, 255, 11)[::29], 255, 11, 64, 6)
+    run = PackedChains(literals(64, 6), ref, built_chains(ref) + literal_chains(ref, 255, 11)[::29], 255, 11)
     s = torch.cuda.Stream()
     saved = run.srcs.dev.clone()
     with torch.cuda.stream(s):
@@ -271,7 +161,7 @@ def test_ordered_on_a_side_stream():
 
 def test_one_chain_of_4096_blocks():
     ref = _ref()
-    run = Literals(ref, at_bound([long_literal_chain(ref, 4096)]), 255, 11, 64, 6)
+    run = PackedChains(literals(64, 6), ref, at_bound([long_literal_chain(ref, 4096)]), 255, 11)
     assert len(run.blocks) == 4096
     res = run.call()
     run.check_one_call(res)

@@ -13,120 +13,15 @@ import pytest
 import torch
 
 from helpers import is_error
-from huf_repeat_cases import main_configs, bound
-from huf_chain_cases import drift_chains, chain_header
+from huf_repeat_cases import main_configs
+from huf_chain_cases import drift_chains
 from huf_chain_packed_cases import at_bound, resolve_headers
-from huf_mixed_chain_cases import (mixed_chains, ragged_chains, with_flags, ref_mixed_chain, expected_mixed, long_mixed_chain,
-                                   built_chains)
-from test_gpu_huf_repeat import Arena, ref_decode
-from test_gpu_huf_repeat_chains import _dev, _view, _guards_ok
-from test_gpu_huf_repeat_packed import Packed, regenerable, _t, _u64, EDGE, FILL, SRC_WRONG, CORRUPT, TOO_SMALL
+from huf_mixed_chain_cases import mixed_chains, ragged_chains, with_flags, long_mixed_chain, built_chains
+from huf_chain_harness import (MIXED, PackedChains, decode, ref_decode, regenerable, _ref, _t, _u64, _view, FILL, SRC_WRONG, CORRUPT,
+                               TOO_SMALL)
 import finitestateentropy_b200 as fb
 
 pytestmark = pytest.mark.gpu
-
-
-def _ref():
-    from huf_repeat_cases import ref_lib
-    ref = ref_lib()
-    if ref is None:
-        pytest.skip("compiled reference not available")
-    return ref
-
-
-class Mixed(Packed):
-    """Packed's harness (state, checks) on mixed chains: the reference loop in each block's form, and calls of the mixed calls"""
-
-    def __init__(self, ref, chains, msv, tlog):
-        self.ref, self.four, self.chains, self.msv, self.tlog = ref, None, chains, msv, tlog
-        self.want = [ref_mixed_chain(ref, ch, msv, tlog) for ch in chains]
-        self.vals, self.kinds, self.blobs, self.flags, self.starts = expected_mixed(self.want, chains)
-        self.blocks = [(c, i) for c, ch in enumerate(chains) for i in range(len(ch["blocks"]))]
-        self.first = self.starts[:-1]
-        srcs, hdrs = Arena(), Arena()
-        for k, (c, i) in enumerate(self.blocks):
-            srcs.add(chains[c]["blocks"][i]["src"], skew=k % 3)
-        self.hdr_blobs = [chain_header(ref, ch) for ch in chains]
-        for blob, _ in self.hdr_blobs:
-            hdrs.add(blob)
-        self.srcs, self.hdrs = srcs.upload(), hdrs.upload()
-        n = len(self.blocks)
-        self.sp = torch.tensor([srcs.ptr(k) for k in range(n)] or [0], dtype=torch.int64, device="cuda")[:n]
-        self.ss = torch.tensor([len(chains[c]["blocks"][i]["src"]) for c, i in self.blocks] or [0], dtype=torch.int64, device="cuda")[:n]
-        self.pr = torch.tensor([chains[c]["blocks"][i]["prefer"] for c, i in self.blocks] or [0], dtype=torch.int32, device="cuda")[:n]
-        self.sg = torch.tensor(self.flags or [0], dtype=torch.uint8, device="cuda")[:n]
-        self.reset()
-
-    def call(self, cap=None, parts=None, starts=None, stream=None, skew=3, fn=None):
-        """Packed.call through the mixed packed compress (or `fn`, a 4X / 1X packed compress, for the same inputs)"""
-        parts = parts or [(0, len(ch["blocks"])) for ch in self.chains]
-        idx, st = [], [0]
-        for c, (lo, hi) in enumerate(parts):
-            idx += [self.first[c] + i for i in range(lo, hi)]
-            st.append(len(idx))
-        if starts is not None:
-            st = starts
-        ix = torch.tensor(idx or [0], dtype=torch.int64, device="cuda")[:len(idx)]
-        if cap is None:
-            cap = int(self.ss[ix].sum()) + 32
-        buf = torch.full((cap + 2 * EDGE + skew,), FILL, dtype=torch.uint8, device="cuda")
-        out = buf[EDGE + skew:EDGE + skew + cap]
-        off, cs = _dev([0xCD] * (len(idx) + 1)), _dev([0xCD] * len(idx))
-        kinds = torch.full((len(idx) + 2 * 8,), 0xEE, dtype=torch.uint8, device="cuda")
-        sv = _dev(st)
-        state = (_view(self.ctp), _view(self.rep), _view(self.chp), _view(self.chs))
-        kw = dict(out=out, offsets=_view(off), csizes=_view(cs), kinds=kinds[8:8 + len(idx)], max_symbol_value=self.msv,
-                  table_log=self.tlog)
-        with torch.cuda.stream(stream or torch.cuda.current_stream()):
-            if fn is None:
-                fb.huf_compress_mixed_repeat_chains_packed(_view(sv), self.sp[ix], self.ss[ix], self.pr[ix], self.sg[ix], *state, **kw)
-            else:
-                fn(_view(sv), self.sp[ix], self.ss[ix], self.pr[ix], *state, **kw)
-        torch.cuda.synchronize()
-        for t in (off, cs, sv, self.ctp, self.rep, self.chp, self.chs):
-            assert _guards_ok(t)
-        kh = kinds.cpu().numpy()
-        assert (kh[:8] == 0xEE).all() and (kh[-8:] == 0xEE).all()
-        return buf, out, _u64(_view(off)), _u64(_view(cs)), kh[8:8 + len(idx)], idx
-
-    def unpacked(self, fn=None):
-        """the pointer-based chain call (mixed, or `fn`) at capacities HUF_compressBound: (dst arena, csizes, hdr ptrs, hdr sizes)"""
-        n = len(self.blocks)
-        caps = np.array([bound(int(x)) for x in self.ss.cpu().numpy()], np.uint64)
-        dst = Arena()
-        for k in range(n):
-            dst.add(np.zeros(int(caps[k]), np.uint8), skew=k % 5)
-        dst.upload()
-        dp = torch.tensor([dst.ptr(k) for k in range(n)], dtype=torch.int64, device="cuda")
-        state = (_view(self.ctp), _view(self.rep), _view(self.chp), _view(self.chs))
-        if fn is None:
-            cs, hp, hs = fb.huf_compress_mixed_repeat_chains(_t(self.starts), self.sp, self.ss, dp, _t(caps), self.pr, self.sg, *state,
-                                                             max_symbol_value=self.msv, table_log=self.tlog)
-        else:
-            cs, hp, hs = fn(_t(self.starts), self.sp, self.ss, dp, _t(caps), self.pr, *state, max_symbol_value=self.msv,
-                            table_log=self.tlog)
-        torch.cuda.synchronize()
-        return dst, _u64(cs), _u64(hp), _u64(hs)
-
-
-def decode_mixed(starts, packed, offsets, kinds, flags, hdr_ptrs, hdr_sizes, sizes, stream=None):
-    """the mixed packed decoder into destinations with canaries around each; returns (results, regenerated regions)"""
-    dsts = Arena()
-    for i, n in enumerate(sizes):
-        dsts.add(np.full(n, 0x5A, np.uint8), skew=(3 * i) % 5)
-    dsts.upload()
-    dp = torch.tensor([dsts.ptr(i) for i in range(len(sizes))] or [0], dtype=torch.int64, device="cuda")[:len(sizes)]
-    dsz = torch.tensor(np.array(sizes, np.uint64).view(np.int64), dtype=torch.int64, device="cuda")
-    res = torch.full((len(sizes) + 16,), -1, dtype=torch.int64, device="cuda")
-    with torch.cuda.stream(stream or torch.cuda.current_stream()):
-        fb.huf_decompress_mixed_repeat_packed(starts, packed, offsets, kinds, flags, hdr_ptrs, hdr_sizes, dp, dsz,
-                                              results=res[8:8 + len(sizes)])
-    torch.cuda.synchronize()
-    r = res.cpu().numpy()
-    assert (r[:8] == -1).all() and (r[-8:] == -1).all()
-    host = dsts.dev.cpu().numpy()
-    assert dsts.canaries_intact(host)
-    return r[8:8 + len(sizes)].view(np.uint64), [host[o:o + len(p)] for o, p in zip(dsts.offs, dsts.parts)]
 
 
 def _token_ptrs(run, dst, c, h, cs):
@@ -142,7 +37,7 @@ def _token_ptrs(run, dst, c, h, cs):
 def test_compress_matches_the_reference_loop(msv, tlog):
     """packed and unpacked mixed calls against the per-block-form loop: values, bytes, kinds, offsets, state, block headers"""
     ref = _ref()
-    run = Mixed(ref, mixed_chains(ref, msv, tlog), msv, tlog)
+    run = PackedChains(MIXED, ref, mixed_chains(ref, msv, tlog), msv, tlog)
     assert len(set(run.flags)) >= 3
     run.check_one_call(run.call(stream=torch.cuda.Stream()))
     run.reset()
@@ -173,7 +68,7 @@ def test_uniform_flags_equal_the_4x_and_1x_calls(flag):
     chains = with_flags(at_bound(drift_chains(ref))[::2] + ragged_chains(seed=9), pattern)
     four = flag == 0
     for msv, tlog in main_configs():
-        run = Mixed(ref, chains, msv, tlog)
+        run = PackedChains(MIXED, ref, chains, msv, tlog)
         a = run.call()
         sa = run.state()
         run.reset()
@@ -237,11 +132,11 @@ def test_round_trip_and_verdicts_of_both_forms():
     ref = _ref()
     msv, tlog = 255, 11
     chains = with_flags(at_bound(drift_chains(ref)) + ragged_chains(seed=4), "random", seed=3) + built_chains(ref)
-    run = Mixed(ref, chains, msv, tlog)
+    run = PackedChains(MIXED, ref, chains, msv, tlog)
     _, out, off, cs, kinds, _ = run.call()
     run.reset()
     sizes = [int(x) for x in run.ss.cpu().numpy()]
-    res, regions = decode_mixed(_t(run.starts), out, _t(off), _t(kinds, torch.uint8), run.sg, _view(run.chp), _view(run.chs), sizes)
+    res, regions = decode(MIXED, _t(run.starts), out, _t(off), _t(kinds, torch.uint8), run.sg, _view(run.chp), _view(run.chs), sizes)
     heads = resolve_headers(kinds, run.starts)
     n_ok = 0
     for k, (c, i) in enumerate(run.blocks):
@@ -298,13 +193,13 @@ def test_decoder_verdicts():
             buf[skew:skew + len(flat)] = torch.from_numpy(flat).cuda()
             packed = buf[skew:skew + len(flat) + 32]
             st = _t([0, 4, len(blobs)])
-            res, regions = decode_mixed(st, packed, _t(offs), _t(kinds, torch.uint8), flags, _t([0, 0]), _t([0, 0]), sizes)
+            res, regions = decode(MIXED, st, packed, _t(offs), _t(kinds, torch.uint8), flags, _t([0, 0]), _t([0, 0]), sizes)
             assert list(res) == want, (skew, pat, list(res))
             assert (regions[0] == blobs[0]).all() and (regions[1] == blobs[1][0]).all()
             for j in (2, 3, 4, 5, 6, 7, 9, 10):
                 assert (regions[j] == 0x5A).all(), j
     for bad in ([1, 4, len(blobs)], [0, 4, len(blobs) - 1], [0, 5, 4]):
-        res, regions = decode_mixed(_t(bad), packed, _t(offs), _t(kinds, torch.uint8), flags, _t([0, 0]), _t([0, 0]), sizes)
+        res, regions = decode(MIXED, _t(bad), packed, _t(offs), _t(kinds, torch.uint8), flags, _t([0, 0]), _t([0, 0]), sizes)
         assert (res == SRC_WRONG).all()
         assert all((r == 0x5A).all() for r in regions)
 
@@ -312,7 +207,7 @@ def test_decoder_verdicts():
 def test_capacity_at_block_ends():
     ref = _ref()
     chains = with_flags(at_bound(drift_chains(ref))[::5] + ragged_chains(seed=2, n_chains=1), "size")
-    run = Mixed(ref, chains, 255, 12)
+    run = PackedChains(MIXED, ref, chains, 255, 12)
     whole = run.call()
     run.check_one_call(whole)
     ends = whole[2]
@@ -348,9 +243,9 @@ def test_split_calls_carry_the_state_and_decode():
     ref = _ref()
     msv, tlog = 255, 11
     chains = with_flags(at_bound(drift_chains(ref))[::3] + ragged_chains(seed=6, n_chains=2), "alt")
-    one = Mixed(ref, chains, msv, tlog)
+    one = PackedChains(MIXED, ref, chains, msv, tlog)
     one.check_one_call(one.call())
-    two = Mixed(ref, chains, msv, tlog)
+    two = PackedChains(MIXED, ref, chains, msv, tlog)
     mids = [len(ch["blocks"]) // 2 for ch in chains]
     a = two.call(parts=[(0, m) for m in mids])
     entry = (_view(two.chp).clone(), _view(two.chs).clone())
@@ -370,8 +265,8 @@ def test_split_calls_carry_the_state_and_decode():
     for m, ch in zip(mids, chains):
         st.append(st[-1] + len(ch["blocks"]) - m)
     sizes = [int(one.ss[k]) for k in idx]
-    res, regions = decode_mixed(_t(st), out, _t(off), _t(kinds, torch.uint8), one.sg[torch.tensor(idx, device="cuda")],
-                                entry[0], entry[1], sizes)
+    res, regions = decode(MIXED, _t(st), out, _t(off), _t(kinds, torch.uint8), one.sg[torch.tensor(idx, device="cuda")],
+                          entry[0], entry[1], sizes)
     heads = resolve_headers(kinds, st)
     sub = [None] * len(one.blocks)
     for j, k in enumerate(idx):
@@ -391,7 +286,7 @@ def test_split_calls_carry_the_state_and_decode():
 def test_malformed_geometry_writes_only_verdicts_and_kinds():
     ref = _ref()
     chains = with_flags(at_bound(drift_chains(ref))[:6], "alt")
-    run = Mixed(ref, chains, 255, 12)
+    run = PackedChains(MIXED, ref, chains, 255, 12)
     nb = len(run.blocks)
     good = run.starts
     before = run.state()
@@ -408,7 +303,7 @@ def test_malformed_geometry_writes_only_verdicts_and_kinds():
 def test_both_calls_are_ordered_on_a_side_stream():
     ref = _ref()
     chains = with_flags(at_bound(drift_chains(ref))[:12], "every3")
-    run = Mixed(ref, chains, 255, 11)
+    run = PackedChains(MIXED, ref, chains, 255, 11)
     s = torch.cuda.Stream()
     sizes = [int(x) for x in run.ss.cpu().numpy()]
     saved = run.srcs.dev.clone()
@@ -445,14 +340,14 @@ def test_both_calls_are_ordered_on_a_side_stream():
 def test_one_chain_of_4096_blocks_with_alternating_flags():
     ref = _ref()
     chains = at_bound([long_mixed_chain(ref, 4096)])
-    run = Mixed(ref, chains, 255, 11)
+    run = PackedChains(MIXED, ref, chains, 255, 11)
     res = run.call()
     run.check_one_call(res)
     assert run.kinds.count(3) > 4000 and run.kinds.count(2) >= 1
     run.reset()
     _, out, off, cs, kinds, _ = res
     sizes = [int(x) for x in run.ss.cpu().numpy()]
-    r, regions = decode_mixed(_t(run.starts), out, _t(off), _t(kinds, torch.uint8), run.sg, _view(run.chp), _view(run.chs), sizes)
+    r, regions = decode(MIXED, _t(run.starts), out, _t(off), _t(kinds, torch.uint8), run.sg, _view(run.chp), _view(run.chs), sizes)
     for k, (c, i) in enumerate(run.blocks):
         src = chains[c]["blocks"][i]["src"]
         assert int(r[k]) == len(src) and (regions[k] == src).all(), k

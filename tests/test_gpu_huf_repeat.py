@@ -12,60 +12,17 @@ import pytest
 import torch
 
 from helpers import ptr, probagen, is_error
-from huf_repeat_cases import ref_lib, main_cases, main_configs, tables, table_header, ref_repeat, bound, room
+from huf_repeat_cases import main_cases, main_configs, tables, table_header, ref_repeat, bound, room
+from huf_chain_harness import Arena, ref_decode, _ref, _u64
 import finitestateentropy_b200 as fb
 
 pytestmark = pytest.mark.gpu
-CANARY, PAD = 0xC7, 4096
 ERR = {name: (1 << 64) - code for code, name in fb.ERROR_NAMES.items()}
 BIG = 128 * 1024
 
 
-def _ref():
-    ref = ref_lib()
-    if ref is None:
-        pytest.skip("compiled reference not available")
-    return ref
-
-
 def _i64(vals, dev="cuda"):
     return torch.tensor(np.array(vals, dtype=np.uint64).view(np.int64), dtype=torch.int64, device=dev)
-
-
-def _u64(t):
-    return t.cpu().numpy().view(np.uint64)
-
-
-class Arena:
-    """one device byte buffer: regions at chosen misalignments, PAD canary bytes around each"""
-
-    def __init__(self):
-        self.parts, self.offs, self.size = [], [], PAD
-
-    def add(self, data, skew=0):
-        self.size += skew
-        self.offs.append(self.size)
-        self.parts.append(np.asarray(data, np.uint8))
-        self.size += len(data) + PAD
-        self.size = (self.size + 15) & ~15
-        return len(self.offs) - 1
-
-    def upload(self):
-        host = np.full(self.size, CANARY, np.uint8)
-        for o, p in zip(self.offs, self.parts):
-            host[o:o + len(p)] = p
-        self.host = host
-        self.dev = torch.from_numpy(host).cuda()
-        return self
-
-    def ptr(self, i):
-        return self.dev.data_ptr() + self.offs[i]
-
-    def canaries_intact(self, out):
-        mask = np.ones(self.size, bool)
-        for o, p in zip(self.offs, self.parts):
-            mask[o:o + len(p)] = False
-        return bool((out[mask] == CANARY).all())
 
 
 def gpu_compress(four, cases, msv, tlog, stream=None):
@@ -219,21 +176,6 @@ def gpu_decompress(four, blobs, dst_sizes, hdrs, expect=None):
     out = dsts.dev.cpu().numpy()
     assert dsts.canaries_intact(out)
     return _u64(res), [out[o:o + len(p)] for o, p in zip(dsts.offs, dsts.parts)]
-
-
-def ref_decode(ref, four, blob, n, hdr):
-    dt = np.zeros(1 + 4096, np.uint32)
-    dt[0] = 11 * 0x01000001                                                # HUF_CREATE_STATIC_DTABLEX1(DT, HUF_TABLELOG_MAX)
-    dst = np.zeros(n + 64, np.uint8)
-    src = blob if len(blob) else np.zeros(1, np.uint8)
-    if hdr is None:
-        fn = ref.HUF_decompress4X1_DCtx if four else ref.HUF_decompress1X1_DCtx
-        return int(fn(ptr(dt), ptr(dst), n, ptr(src), len(blob))) % (1 << 64), dst[:n]
-    h = ref.HUF_readDTableX1(ptr(dt), ptr(hdr), len(hdr))
-    if is_error(h):
-        return int(h) % (1 << 64), dst[:n]
-    fn = ref.HUF_decompress4X1_usingDTable if four else ref.HUF_decompress1X1_usingDTable
-    return int(fn(ptr(dst), n, ptr(src), len(blob), ptr(dt))) % (1 << 64), dst[:n]
 
 
 @pytest.mark.parametrize("four", [True, False], ids=["4X", "1X"])

@@ -11,32 +11,12 @@ import pytest
 import torch
 
 from helpers import is_error
-from huf_repeat_cases import ref_lib, main_configs, room
+from huf_repeat_cases import main_configs, room
 from huf_chain_cases import ref_chain, single_chains, mid_chains, drift_chains, empty_chains, long_chain, chain_header
-from test_gpu_huf_repeat import Arena, ref_decode
+from huf_chain_harness import Arena, ref_decode, _ref, _dev, _view, _guards_ok, SRC_WRONG
 import finitestateentropy_b200 as fb
 
 pytestmark = pytest.mark.gpu
-SRC_WRONG = (1 << 64) - 3
-G = 8                                                                      # guard words around every array
-GUARD = -0x3838383838383839                                                # 0xC7C7... as int64
-
-
-def _dev(vals, dtype=torch.int64):
-    a = np.array(vals, dtype=np.uint64).view(np.int64) if dtype == torch.int64 else np.array(vals, np.int32)
-    t = torch.full((len(a) + 2 * G,), GUARD if dtype == torch.int64 else -0x38383839, dtype=dtype, device="cuda")
-    t[G:G + len(a)] = torch.from_numpy(a).cuda()
-    return t
-
-
-def _view(t):
-    return t[G:t.numel() - G]
-
-
-def _guards_ok(t):
-    v = t.cpu().numpy()
-    g = GUARD if t.dtype == torch.int64 else -0x38383839
-    return bool((v[:G] == g).all() and (v[-G:] == g).all())
 
 
 class Run:
@@ -149,13 +129,6 @@ class Run:
             assert int(s["rep"][c]) == F, ch["name"]
             assert (int(s["chp"][c]), int(s["chs"][c])) == self.header_value(c, H), ch["name"]
         return s
-
-
-def _ref():
-    ref = ref_lib()
-    if ref is None:
-        pytest.skip("compiled reference not available")
-    return ref
 
 
 @pytest.mark.parametrize("four", [True, False], ids=["4X", "1X"])

@@ -12,163 +12,14 @@ import pytest
 import torch
 
 from helpers import is_error
-from huf_repeat_cases import ref_lib, main_configs
-from huf_chain_cases import ref_chain, single_chains, drift_chains, empty_chains, chain_header, long_chain
-from huf_chain_packed_cases import at_bound, packed_chains, expected, resolve_headers
-from test_gpu_huf_repeat import Arena, ref_decode
-from test_gpu_huf_repeat_chains import _dev, _view, _guards_ok
+from huf_repeat_cases import main_configs
+from huf_chain_cases import single_chains, drift_chains, empty_chains, long_chain
+from huf_chain_packed_cases import at_bound, packed_chains, resolve_headers
+from huf_chain_harness import (PLAIN, PackedChains, Arena, decode, ref_decode, regenerable, _ref, _t, _u64, _view, FILL, SRC_WRONG,
+                               CORRUPT, TOO_SMALL)
 import finitestateentropy_b200 as fb
 
 pytestmark = pytest.mark.gpu
-SRC_WRONG, CORRUPT, TOO_SMALL = (1 << 64) - 3, (1 << 64) - 4, (1 << 64) - 2
-EDGE, FILL = 64, 0xC7                                                      # guard bytes around the packed buffer
-
-
-def _ref():
-    ref = ref_lib()
-    if ref is None:
-        pytest.skip("compiled reference not available")
-    return ref
-
-
-def _u64(t):
-    return t.cpu().numpy().view(np.uint64)
-
-
-class Packed:
-    """the chains' sources, tables, entry headers and per-chain state on the device, and calls of the packed compress"""
-
-    def __init__(self, ref, four, chains, msv, tlog):
-        self.ref, self.four, self.chains, self.msv, self.tlog = ref, four, chains, msv, tlog
-        self.want = [ref_chain(ref, four, ch, msv, tlog) for ch in chains]
-        self.vals, self.kinds, self.blobs, self.starts = expected(self.want, chains)
-        self.blocks = [(c, i) for c, ch in enumerate(chains) for i in range(len(ch["blocks"]))]
-        self.first = self.starts[:-1]
-        srcs, hdrs = Arena(), Arena()
-        for k, (c, i) in enumerate(self.blocks):
-            srcs.add(chains[c]["blocks"][i]["src"], skew=k % 3)
-        self.hdr_blobs = [chain_header(ref, ch) for ch in chains]
-        for blob, _ in self.hdr_blobs:
-            hdrs.add(blob)
-        self.srcs, self.hdrs = srcs.upload(), hdrs.upload()
-        n = len(self.blocks)
-        self.sp = torch.tensor([srcs.ptr(k) for k in range(n)] or [0], dtype=torch.int64, device="cuda")[:n]
-        self.ss = torch.tensor([len(chains[c]["blocks"][i]["src"]) for c, i in self.blocks] or [0], dtype=torch.int64, device="cuda")[:n]
-        self.pr = torch.tensor([chains[c]["blocks"][i]["prefer"] for c, i in self.blocks] or [0], dtype=torch.int32, device="cuda")[:n]
-        self.reset()
-
-    def reset(self):
-        """the per-chain state as the chains enter"""
-        words = 256 + 64
-        tab = np.full(64 + len(self.chains) * words, 0xC7C7C7C7, np.uint32)
-        self.toff = [64 + c * words + (c % 4) for c in range(len(self.chains))]
-        for o, ch in zip(self.toff, self.chains):
-            tab[o:o + 256] = ch["table"]
-        self.tab = torch.from_numpy(tab.view(np.int32)).cuda()
-        self.ctp = _dev([self.tab.data_ptr() + 4 * o for o in self.toff])
-        self.rep = _dev([ch["flag"] for ch in self.chains], torch.int32)
-        self.chp = _dev([self.hdrs.ptr(c) for c in range(len(self.chains))])
-        self.chs = _dev([len(b) for b, _ in self.hdr_blobs])
-
-    def state(self):
-        return dict(tabs=self.tab.cpu().numpy().view(np.uint32).copy(), rep=_view(self.rep).cpu().numpy(),
-                    chp=_u64(_view(self.chp)), chs=_view(self.chs).cpu().numpy())
-
-    def call(self, cap=None, parts=None, starts=None, stream=None, skew=3):
-        """one packed call over blocks parts[c] = (lo, hi) of each chain (all by default) into a buffer of `cap` bytes (the sum of
-        the sources + 32 by default) with EDGE guard bytes around it.  Returns (buf, out view, offsets, csizes, kinds, idx)."""
-        parts = parts or [(0, len(ch["blocks"])) for ch in self.chains]
-        idx, st = [], [0]
-        for c, (lo, hi) in enumerate(parts):
-            idx += [self.first[c] + i for i in range(lo, hi)]
-            st.append(len(idx))
-        if starts is not None:
-            st = starts
-        ix = torch.tensor(idx or [0], dtype=torch.int64, device="cuda")[:len(idx)]
-        if cap is None:
-            cap = int(self.ss[ix].sum()) + 32
-        buf = torch.full((cap + 2 * EDGE + skew,), FILL, dtype=torch.uint8, device="cuda")
-        out = buf[EDGE + skew:EDGE + skew + cap]
-        off, cs = _dev([0xCD] * (len(idx) + 1)), _dev([0xCD] * len(idx))
-        kinds = torch.full((len(idx) + 2 * 8,), 0xEE, dtype=torch.uint8, device="cuda")
-        sv = _dev(st)
-        fn = fb.huf_compress_repeat_chains_packed if self.four else fb.huf_compress1x_repeat_chains_packed
-        with torch.cuda.stream(stream or torch.cuda.current_stream()):
-            fn(_view(sv), self.sp[ix], self.ss[ix], self.pr[ix], _view(self.ctp), _view(self.rep), _view(self.chp), _view(self.chs),
-               out=out, offsets=_view(off), csizes=_view(cs), kinds=kinds[8:8 + len(idx)], max_symbol_value=self.msv, table_log=self.tlog)
-        torch.cuda.synchronize()
-        for t in (off, cs, sv, self.ctp, self.rep, self.chp, self.chs):
-            assert _guards_ok(t)
-        kh = kinds.cpu().numpy()
-        assert (kh[:8] == 0xEE).all() and (kh[-8:] == 0xEE).all()
-        return buf, out, _u64(_view(off)), _u64(_view(cs)), kh[8:8 + len(idx)], idx
-
-    def check_one_call(self, res):
-        """a whole-batch call that fits: values, stored bytes, kinds, offsets, guards and the final state"""
-        buf, out, off, cs, kinds, idx = res
-        n = len(idx)
-        assert (cs == np.array(self.vals, np.uint64)).all()
-        assert list(kinds) == self.kinds
-        lens = [len(b) for b in self.blobs]
-        assert list(off) == list(np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64)), "offsets"
-        host = buf.cpu().numpy()
-        o0 = out.data_ptr() - buf.data_ptr()
-        for k in range(n):
-            got = host[o0 + int(off[k]):o0 + int(off[k + 1])]
-            assert (got == self.blobs[k]).all(), (k, self.blocks[k])
-        assert (host[:o0] == FILL).all() and (host[o0 + int(off[n]):] == FILL).all()
-        s = self.state()
-        for c, ch in enumerate(self.chains):
-            _, (T, F, H) = self.want[c]
-            t = s["tabs"][self.toff[c]:self.toff[c] + 256]
-            assert (t == (ch["table"] if (T == ch["table"]).all() else T & 0x00FFFFFF)).all(), ch["name"]
-            assert int(s["rep"][c]) == F, ch["name"]
-            if H[0] == "chain":
-                hv = (self.hdrs.ptr(c), len(self.hdr_blobs[c][0]))
-            else:
-                k = self.first[c] + H[1]
-                hv = (out.data_ptr() + int(off[k]), int(cs[k]))
-            assert (int(s["chp"][c]), int(s["chs"][c])) == hv, ch["name"]
-        return s
-
-
-def regenerable(run, k, heads, entry_is_stand_in):
-    """whether block k must decode back to its source: a value that is not an error, not a 1X block the reference coded into a
-    single byte (its decoders read that as RLE too), and not a kind-3 block whose entry header is a stand-in (its table has none)"""
-    c, i = run.blocks[k]
-    r, src = run.vals[k], run.chains[c]["blocks"][i]["src"]
-    if is_error(r) or (r == 1 and not (src == run.blobs[k][0]).all()):
-        return False
-    return not (heads[k] is not None and heads[k][0] == "chain" and entry_is_stand_in(c))
-
-
-def decode(four, starts, packed, offsets, kinds, hdr_ptrs, hdr_sizes, sizes, expect=None, stream=None):
-    """the packed decoder into destinations with canaries around each; returns (results, regenerated regions)"""
-    dsts = Arena()
-    for i, n in enumerate(sizes):
-        fill = np.full(n, 0x5A, np.uint8)
-        if expect is not None and expect[i] is not None:
-            fill[:len(expect[i])] = ~expect[i]
-        dsts.add(fill, skew=(3 * i) % 5)
-    dsts.upload()
-    dp = torch.tensor([dsts.ptr(i) for i in range(len(sizes))] or [0], dtype=torch.int64, device="cuda")[:len(sizes)]
-    dsz = torch.tensor(np.array(sizes, np.uint64).view(np.int64), dtype=torch.int64, device="cuda")
-    fn = fb.huf_decompress_repeat_packed if four else fb.huf_decompress1x_repeat_packed
-    res = torch.full((len(sizes) + 16,), -1, dtype=torch.int64, device="cuda")
-    with torch.cuda.stream(stream or torch.cuda.current_stream()):
-        fn(starts, packed, offsets, kinds, hdr_ptrs, hdr_sizes, dp, dsz, results=res[8:8 + len(sizes)])
-    torch.cuda.synchronize()
-    r = res.cpu().numpy()
-    assert (r[:8] == -1).all() and (r[-8:] == -1).all()
-    host = dsts.dev.cpu().numpy()
-    assert dsts.canaries_intact(host)
-    return r[8:8 + len(sizes)].view(np.uint64), [host[o:o + len(p)] for o, p in zip(dsts.offs, dsts.parts)]
-
-
-def _t(vals, dtype=torch.int64):
-    if dtype == torch.uint8:
-        return torch.tensor(np.asarray(vals, np.uint8), dtype=torch.uint8, device="cuda")
-    return torch.tensor(np.array(vals, np.uint64).view(np.int64), dtype=torch.int64, device="cuda")
 
 
 @pytest.mark.parametrize("four", [True, False], ids=["4X", "1X"])
@@ -176,13 +27,13 @@ def test_compress_matches_the_reference_loop_and_the_chain_call(four):
     ref = _ref()
     for msv, tlog in main_configs():
         chains = at_bound(single_chains(ref, four, msv, tlog))[::3] + empty_chains(1) + packed_chains(ref, four, msv, tlog)
-        run = Packed(ref, four, chains, msv, tlog)
+        run = PackedChains(PLAIN[four], ref, chains, msv, tlog)
         res = run.call(stream=torch.cuda.Stream())
         run.check_one_call(res)
         _, out, off, cs, kinds, _ = res
         # the pointer-based chain call on the same inputs at capacities HUF_compressBound
         n = len(run.blocks)
-        run2 = Packed.__new__(Packed)
+        run2 = PackedChains.__new__(PackedChains)
         run2.__dict__.update(run.__dict__)
         run2.reset()
         caps = np.array([129 + int(x) + (int(x) >> 8) + 8 for x in run.ss.cpu().numpy()], np.uint64)
@@ -216,7 +67,7 @@ def test_compress_matches_the_reference_loop_and_the_chain_call(four):
 def test_one_chain_of_4096_blocks(four):
     ref = _ref()
     chains = at_bound([long_chain(ref, 4096)]) + empty_chains(1)
-    run = Packed(ref, four, chains, 255, 11)
+    run = PackedChains(PLAIN[four], ref, chains, 255, 11)
     run.check_one_call(run.call())
     assert run.kinds.count(3) > 4000 and run.kinds.count(2) >= 1
 
@@ -225,7 +76,7 @@ def test_one_chain_of_4096_blocks(four):
 def test_capacity_at_block_ends(four):
     ref = _ref()
     chains = packed_chains(ref, four, 255, 12)[::5]
-    run = Packed(ref, four, chains, 255, 12)
+    run = PackedChains(PLAIN[four], ref, chains, 255, 12)
     whole = run.call()
     run.check_one_call(whole)
     ends = whole[2]
@@ -261,10 +112,10 @@ def test_split_calls_give_one_calls_result_and_decode(four):
     ref = _ref()
     msv, tlog = 255, 11
     chains = at_bound(drift_chains(ref))[::3]                              # entry tables that are Huffman tables: they decode
-    one = Packed(ref, four, chains, msv, tlog)
+    one = PackedChains(PLAIN[four], ref, chains, msv, tlog)
     whole = one.call()
     one.check_one_call(whole)
-    two = Packed(ref, four, chains, msv, tlog)
+    two = PackedChains(PLAIN[four], ref, chains, msv, tlog)
     mids = [len(ch["blocks"]) // 2 for ch in chains]
     a = two.call(parts=[(0, m) for m in mids])
     entry = (_view(two.chp).clone(), _view(two.chs).clone())               # the second part's entry headers: inside a's buffer
@@ -285,7 +136,7 @@ def test_split_calls_give_one_calls_result_and_decode(four):
     for m, ch in zip(mids, chains):
         st.append(st[-1] + len(ch["blocks"]) - m)
     sizes = [int(one.ss[k]) for k in idx]
-    res, regions = decode(four, _t(st), out, _t(off), _t(kinds, torch.uint8), entry[0], entry[1], sizes)
+    res, regions = decode(PLAIN[four], _t(st), out, _t(off), _t(kinds, torch.uint8), entry[0], entry[1], sizes)
     ok = 0
     heads = resolve_headers(kinds, st)
     sub = [None] * len(one.blocks)
@@ -307,12 +158,12 @@ def test_round_trip_and_agreement_with_the_header_decoders(four):
     ref = _ref()
     msv, tlog = 255, 11                                                    # tables the X1 decoders' 11-bit DTable holds
     chains = at_bound(drift_chains(ref)) + [long_chain(ref, 512)]         # entry tables that are Huffman tables: they decode
-    run = Packed(ref, four, chains, msv, tlog)
+    run = PackedChains(PLAIN[four], ref, chains, msv, tlog)
     res0 = run.call()
     run.reset()
     _, out, off, cs, kinds, idx = res0
     sizes = [int(x) for x in run.ss.cpu().numpy()]
-    res, regions = decode(four, _t(run.starts), out, _t(off), _t(kinds, torch.uint8), _view(run.chp), _view(run.chs), sizes,
+    res, regions = decode(PLAIN[four], _t(run.starts), out, _t(off), _t(kinds, torch.uint8), _view(run.chp), _view(run.chs), sizes,
                           expect=[chains[c]["blocks"][i]["src"] for c, i in run.blocks])
     heads = resolve_headers(kinds, run.starts)
     n_ok = 0
@@ -370,13 +221,13 @@ def test_decoder_verdicts(four):
         buf[skew:skew + len(flat)] = torch.from_numpy(flat).cuda()
         packed = buf[skew:skew + len(flat) + 32]
         st = _t([0, 4, len(blobs)])
-        res, regions = decode(four, st, packed, _t(offs), _t(kinds, torch.uint8), _t([0, 0]), _t([0, 0]), sizes)
+        res, regions = decode(PLAIN[four], st, packed, _t(offs), _t(kinds, torch.uint8), _t([0, 0]), _t([0, 0]), sizes)
         assert list(res) == want, (skew, list(res))
         assert (regions[0] == blobs[0]).all() and (regions[1] == blobs[1][0]).all()
         for j in (2, 3, 4, 5, 6, 7, 9):
             assert (regions[j] == 0x5A).all(), j
     for bad in ([1, 4, len(blobs)], [0, 4, len(blobs) - 1], [0, 5, 4]):
-        res, regions = decode(four, _t(bad), packed, _t(offs), _t(kinds, torch.uint8), _t([0, 0]), _t([0, 0]), sizes)
+        res, regions = decode(PLAIN[four], _t(bad), packed, _t(offs), _t(kinds, torch.uint8), _t([0, 0]), _t([0, 0]), sizes)
         assert (res == SRC_WRONG).all()
         assert all((r == 0x5A).all() for r in regions)
 
@@ -385,7 +236,7 @@ def test_decoder_verdicts(four):
 def test_malformed_compress_geometry_writes_only_verdicts_and_kinds(four):
     ref = _ref()
     chains = packed_chains(ref, four, 255, 12)[:6]
-    run = Packed(ref, four, chains, 255, 12)
+    run = PackedChains(PLAIN[four], ref, chains, 255, 12)
     nb = len(run.blocks)
     good = run.starts
     before = run.state()
@@ -403,7 +254,7 @@ def test_malformed_compress_geometry_writes_only_verdicts_and_kinds(four):
 def test_both_calls_are_ordered_on_a_side_stream(four):
     ref = _ref()
     chains = at_bound(drift_chains(ref))[:12]
-    run = Packed(ref, four, chains, 255, 11)
+    run = PackedChains(PLAIN[four], ref, chains, 255, 11)
     s = torch.cuda.Stream()
     sizes = [int(x) for x in run.ss.cpu().numpy()]
     saved = run.srcs.dev.clone()
