@@ -114,27 +114,14 @@ def _blocks_args(*arrays):
 def huf_compress_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes=None, max_symbol_value=255, table_log=12):
     """HUF_compress2 on every block b: src_ptrs[b] / src_sizes[b] into dst_ptrs[b] of capacity dst_caps[b], on the current
     stream.  Returns csizes (int64; the reference's value per block, error codes as their two's-complement)."""
-    from . import lib
-    if csizes is None:
-        csizes = torch.empty(src_ptrs.numel(), dtype=torch.int64, device=src_ptrs.device)
-    n = _blocks_args(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes)
-    r = lib().FSEB200_HUF_compress_blocks(n, dst_ptrs.data_ptr(), dst_caps.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
-                                          src_sizes.data_ptr(), max_symbol_value, table_log, _stream_ptr())
-    _ret(r, "FSEB200_HUF_compress_blocks")
-    return csizes
+    return _codec_blocks("FSEB200_HUF_compress_blocks", src_ptrs, (src_ptrs, src_sizes, dst_ptrs, dst_caps), csizes,
+                         (max_symbol_value, table_log))
 
 
 def huf_decompress_blocks(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results=None):
     """HUF_decompress on every block b: csrc_ptrs[b] / csrc_sizes[b] into dst_ptrs[b] of dst_sizes[b] bytes, on the current
     stream.  Returns results (int64; regenerated size or error code per block)."""
-    from . import lib
-    if results is None:
-        results = torch.empty(csrc_ptrs.numel(), dtype=torch.int64, device=csrc_ptrs.device)
-    n = _blocks_args(csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes, results)
-    r = lib().FSEB200_HUF_decompress_blocks(n, dst_ptrs.data_ptr(), dst_sizes.data_ptr(), results.data_ptr(), csrc_ptrs.data_ptr(),
-                                            csrc_sizes.data_ptr(), _stream_ptr())
-    _ret(r, "FSEB200_HUF_decompress_blocks")
-    return results
+    return _codec_blocks("FSEB200_HUF_decompress_blocks", csrc_ptrs, (csrc_ptrs, csrc_sizes, dst_ptrs, dst_sizes), results)
 
 
 def huf_compress1x_blocks(src_ptrs, src_sizes, dst_ptrs, dst_caps, csizes=None, max_symbol_value=255, table_log=12):
@@ -412,28 +399,39 @@ def huf_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None
     is the prefix sum of the stored lengths, csizes the reference's value per block (dstSize_tooSmall for a block that does not
     fit `out`).  With out=None, `out` is allocated at sum(src_sizes) + 32 bytes, always enough: reading that sum costs one host
     synchronisation.  `packed_pointers(out, offsets)` gives the arrays huf_decompress_blocks decodes the buffer with."""
-    return _compress_packed("FSEB200_HUF_compress_packed", src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log)
+    return _compress_packed("FSEB200_HUF_compress_packed", 1, src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log)
 
 
 def huf_compress1x_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None, max_symbol_value=255, table_log=12):
     """huf_compress_packed in the single-stream format (HUF_compress1X per block); decode with huf_decompress1x_blocks"""
-    return _compress_packed("FSEB200_HUF_compress1X_packed", src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log)
+    return _compress_packed("FSEB200_HUF_compress1X_packed", 1, src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log)
 
 
-def _compress_packed(fn_name, src_ptrs, src_sizes, out, offsets, csizes, msv, tlog):
+def _compress_packed(fn_name, unit, src_ptrs, src_sizes, out, offsets, csizes, msv, tlog, fse=False, work=None):
+    """the packed compress of blocks of `unit` bytes per symbol; FSE (`fse`) also takes the staging workspace `work`.  out and
+    work, when None, are sized from the source bytes"""
     from . import lib
     n = _blocks_args(src_ptrs, src_sizes)
     dev = src_ptrs.device
-    if out is None:
-        out = torch.empty(int(src_sizes.sum().item()) + 32, dtype=torch.uint8, device=dev)    # .item(): the host sync
+    if out is None or (fse and work is None):
+        src_bytes = unit * int(src_sizes.sum().item())                                  # .item(): the host sync
+        if out is None:
+            out = torch.empty(src_bytes + 32, dtype=torch.uint8, device=dev)
+        if fse and work is None:
+            work = torch.empty(max(fse_packed_workspace(n, src_bytes), 1), dtype=torch.uint8, device=dev)
     if offsets is None:
         offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
     if csizes is None:
         csizes = torch.empty(n, dtype=torch.int64, device=dev)
-    _check(out, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64)
-    assert offsets.numel() == n + 1 and csizes.numel() == n and out.device == dev, (offsets.numel(), csizes.numel(), n)
+    _check(out, torch.uint8)
+    if fse:
+        _check(work, torch.uint8)
+    _check(offsets, torch.int64); _check(csizes, torch.int64)
+    assert offsets.numel() == n + 1 and csizes.numel() == n and out.device == dev and (not fse or work.device == dev), \
+        (offsets.numel(), csizes.numel(), n)
+    workspace = (work.data_ptr(), work.numel()) if fse else ()
     r = getattr(lib(), fn_name)(n, out.data_ptr(), out.numel(), offsets.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
-                                src_sizes.data_ptr(), msv, tlog, _stream_ptr())
+                                src_sizes.data_ptr(), msv, tlog, *workspace, _stream_ptr())
     _ret(r, fn_name)
     return out, offsets, csizes
 
@@ -490,43 +488,21 @@ def fse_compress_packed(src_ptrs, src_sizes, out=None, offsets=None, csizes=None
     csizes the reference's value per block (dstSize_tooSmall / workSpace_tooSmall for a block that does not fit `out` / `work`).
     With out or work None they are sized from sum(src_sizes) -- out at that sum + 32 bytes, work by fse_packed_workspace, both
     always enough: reading the sum costs one host synchronisation.  Decode with fse_decompress_packed."""
-    return _fse_compress_packed("FSEB200_FSE_compress_packed", 1, src_ptrs, src_sizes, out, offsets, csizes, work,
-                                max_symbol_value, table_log)
+    return _compress_packed("FSEB200_FSE_compress_packed", 1, src_ptrs, src_sizes, out, offsets, csizes, max_symbol_value, table_log,
+                            fse=True, work=work)
 
 
 def fseu16_compress_packed(src_ptrs, src_symbols, out=None, offsets=None, csizes=None, work=None, max_symbol_value=0, table_log=12):
     """fse_compress_packed for FSE_compressU16: src_symbols[b] 16-bit symbols at src_ptrs[b] (2-byte aligned); `out` and `work`
     default to 2 * sum(src_symbols) + 32 bytes and the workspace of 2 * sum(src_symbols) source bytes"""
-    return _fse_compress_packed("FSEB200_FSEU16_compress_packed", 2, src_ptrs, src_symbols, out, offsets, csizes, work,
-                                max_symbol_value, table_log)
+    return _compress_packed("FSEB200_FSEU16_compress_packed", 2, src_ptrs, src_symbols, out, offsets, csizes, max_symbol_value,
+                            table_log, fse=True, work=work)
 
 
 def fse_packed_workspace(n_blocks, src_bytes):
     """bytes of workspace that never run short for n_blocks blocks of src_bytes source bytes in all (U16: 2 * symbols)"""
     from . import lib
     return int(lib().FSEB200_FSE_packed_workspace(n_blocks, src_bytes))
-
-
-def _fse_compress_packed(fn_name, unit, src_ptrs, src_sizes, out, offsets, csizes, work, msv, tlog):
-    from . import lib
-    n = _blocks_args(src_ptrs, src_sizes)
-    dev = src_ptrs.device
-    if out is None or work is None:
-        src_bytes = unit * int(src_sizes.sum().item())                                  # .item(): the host sync
-        if out is None:
-            out = torch.empty(src_bytes + 32, dtype=torch.uint8, device=dev)
-        if work is None:
-            work = torch.empty(max(fse_packed_workspace(n, src_bytes), 1), dtype=torch.uint8, device=dev)
-    if offsets is None:
-        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    if csizes is None:
-        csizes = torch.empty(n, dtype=torch.int64, device=dev)
-    _check(out, torch.uint8); _check(work, torch.uint8); _check(offsets, torch.int64); _check(csizes, torch.int64)
-    assert offsets.numel() == n + 1 and csizes.numel() == n and out.device == dev and work.device == dev, (offsets.numel(), csizes.numel(), n)
-    r = getattr(lib(), fn_name)(n, out.data_ptr(), out.numel(), offsets.data_ptr(), csizes.data_ptr(), src_ptrs.data_ptr(),
-                                src_sizes.data_ptr(), msv, tlog, work.data_ptr(), work.numel(), _stream_ptr())
-    _ret(r, fn_name)
-    return out, offsets, csizes
 
 
 def fse_decompress_packed(packed, offsets, dst_ptrs, dst_sizes, results=None):

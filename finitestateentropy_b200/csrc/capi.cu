@@ -174,7 +174,7 @@ FSEB_API size_t FSEB200_HUF_compress_blocks(size_t nBlocks, void* const* dDsts, 
                                             const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
     return blocks_call(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes,
-                       [&](const BlockDescs& g) { return launch_huf_encode_blocks(g, 4, maxSymbolValue, tableLog, (cudaStream_t)stream); });
+                       [&](const BlockDescs& g) { return launch_huf_encode_descs(g, 4, maxSymbolValue, tableLog, (cudaStream_t)stream); });
 }
 FSEB_API size_t FSEB200_HUF_decompress_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                               const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
@@ -186,7 +186,7 @@ FSEB_API size_t FSEB200_HUF_compress1X_blocks(size_t nBlocks, void* const* dDsts
                                               const void* const* dSrcs, const size_t* dSrcSizes, unsigned maxSymbolValue, unsigned tableLog, void* stream)
 {
     return blocks_call(nBlocks, dDsts, dDstCapacities, dCSizes, dSrcs, dSrcSizes,
-                       [&](const BlockDescs& g) { return launch_huf_encode_blocks(g, 1, maxSymbolValue, tableLog, (cudaStream_t)stream); });
+                       [&](const BlockDescs& g) { return launch_huf_encode_descs(g, 1, maxSymbolValue, tableLog, (cudaStream_t)stream); });
 }
 FSEB_API size_t FSEB200_HUF_decompress1X_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults,
                                                 const void* const* dCSrcs, const size_t* dCSrcSizes, void* stream)
@@ -206,18 +206,20 @@ size_t huf_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstC
         RepeatDescs g;
         static_cast<BlockDescs&>(g) = d;
         g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.prefer = dPreferRepeat;
-        return launch_huf_encode_repeat(g, nStreams, msv, tlog, (cudaStream_t)stream);
+        return launch_huf_encode_descs(g, nStreams, msv, tlog, (cudaStream_t)stream);
     });
 }
+// nStreams as forms_given's
 size_t huf_header_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstSizes, size_t* dResults, const void* const* dCSrcs,
-                         const size_t* dCSrcSizes, const void* const* dHeaders, const size_t* dHeaderSizes, int nStreams, void* stream)
+                         const size_t* dCSrcSizes, const void* const* dHeaders, const size_t* dHeaderSizes, int nStreams, void* stream,
+                         const unsigned char* dSingleStream = nullptr)
 {
-    if (nBlocks && (!dHeaders || !dHeaderSizes)) return (size_t)err(E_SRC_WRONG);
+    if (nBlocks && (!dHeaders || !dHeaderSizes || !forms_given(nStreams, dSingleStream))) return (size_t)err(E_SRC_WRONG);
     return blocks_call(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, [&](const BlockDescs& d) {
         HeaderDescs g;
         static_cast<BlockDescs&>(g) = d;
         g.hdr = (const u8* const*)dHeaders; g.hdrSize = (const u64*)dHeaderSizes;
-        return launch_huf_decode_headers(g, nStreams, (cudaStream_t)stream);
+        return launch_huf_decode_headers(g, nStreams, (cudaStream_t)stream, dSingleStream);
     });
 }
 }
@@ -226,13 +228,7 @@ FSEB_API size_t FSEB200_HUF_decompress_mixed_repeat_blocks(size_t nBlocks, void*
                                                           const void* const* dCSrcs, const size_t* dCSrcSizes, const void* const* dHeaders,
                                                           const size_t* dHeaderSizes, const unsigned char* dSingleStream, void* stream)
 {
-    if (nBlocks && (!dHeaders || !dHeaderSizes || !dSingleStream)) return (size_t)err(E_SRC_WRONG);
-    return blocks_call(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, [&](const BlockDescs& d) {
-        HeaderDescs g;
-        static_cast<BlockDescs&>(g) = d;
-        g.hdr = (const u8* const*)dHeaders; g.hdrSize = (const u64*)dHeaderSizes;
-        return launch_huf_decode_headers_mixed(g, dSingleStream, (cudaStream_t)stream);
-    });
+    return huf_header_blocks(nBlocks, dDsts, dDstSizes, dResults, dCSrcs, dCSrcSizes, dHeaders, dHeaderSizes, 0, stream, dSingleStream);
 }
 FSEB_API size_t FSEB200_HUF_compress4X_repeat_blocks(size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities, size_t* dCSizes,
                                                      const void* const* dSrcs, const size_t* dSrcSizes, unsigned* const* dCTables, int* dRepeats,
@@ -250,8 +246,7 @@ FSEB_API size_t FSEB200_HUF_compress1X_repeat_blocks(size_t nBlocks, void* const
 }
 // Chains: blocks of one stream in one call, the stream's state carried from block to block on the device (common.cuh ChainDescs).
 namespace {
-// nStreams 4 or 1: every block in that form; 0: mixed, each block's form in dSingleStream, which must then be given
-bool forms_given(int nStreams, const void* dSingleStream) { return nStreams || dSingleStream; }
+// nStreams as forms_given's
 size_t huf_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstCapacities,
                          size_t* dCSizes, const void* const* dSrcs, const size_t* dSrcSizes, const int* dPreferRepeat,
                          unsigned* const* dCTables, int* dRepeats, const void** dChainHeaders, size_t* dChainHeaderSizes,
@@ -266,8 +261,7 @@ size_t huf_repeat_chains(size_t nChains, const size_t* dChainStarts, size_t nBlo
         g.start = (const u64*)dChainStarts; g.nChains = (u32)nChains; g.prefer = dPreferRepeat;
         g.ctable = (u32* const*)dCTables; g.repeat = dRepeats; g.hdr = (const u8**)dChainHeaders; g.hdrSize = (u64*)dChainHeaderSizes;
         g.blkHdr = (const u8**)dHeaders; g.blkHdrSize = (u64*)dHeaderSizes; g.fact = nullptr; g.single = dSingleStream;
-        return nStreams ? launch_huf_encode_chains(g, nStreams, msv, tlog, (cudaStream_t)stream)
-                        : launch_huf_encode_chains_mixed(g, msv, tlog, (cudaStream_t)stream);
+        return launch_huf_encode_descs(g, nStreams, msv, tlog, (cudaStream_t)stream);
     });
 }
 }
@@ -321,19 +315,12 @@ void chain_packed_descs(ChainPackedDescs& g, size_t nChains, const size_t* dChai
     g.pk.src = g.src; g.pk.srcSize = g.srcSize; g.pk.nBlocks = g.nBlocks;
     g.kind = dKinds; g.end = nullptr; g.malformed = nullptr;
 }
-// The form of a packed chain compress: every block in nStreams streams (4 or 1), or (0) each block's form in dSingleStream --
-// read, or under zstd's literal policy (`literals`, with minLiterals and minGainLog) chosen by the device and written there.
-struct ChainForm {
-    int nStreams;
-    unsigned char* dSingleStream;
-    bool literals;
-    unsigned minLiterals, minGainLog;
-};
-size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut, size_t outCapacity,
-                                size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs,
-                                const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats,
-                                const void** dChainHeaders, size_t* dChainHeaderSizes, const ChainForm& f, unsigned msv, unsigned tlog,
-                                void* stream)
+}
+size_t fseb::huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut, size_t outCapacity,
+                                      size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds, const void* const* dSrcs,
+                                      const size_t* dSrcSizes, const int* dPreferRepeat, unsigned* const* dCTables, int* dRepeats,
+                                      const void** dChainHeaders, size_t* dChainHeaderSizes, const ChainForm& f, unsigned msv,
+                                      unsigned tlog, void* stream)
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dOut || !dOffsets || !dCSizes || !dKinds || !dSrcs ||
@@ -347,18 +334,17 @@ size_t huf_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size
         ChainPackedLiteralsDescs g;
         static_cast<ChainPackedDescs&>(g) = d;
         g.single = f.dSingleStream; g.minLiterals = f.minLiterals; g.minGainLog = f.minGainLog;
-        return ok_or_generic(launch_huf_encode_literals_chains_packed(g, msv, tlog, (cudaStream_t)stream));
+        return ok_or_generic(launch_huf_encode_descs(g, 0, msv, tlog, (cudaStream_t)stream));
     }
     ChainPackedMixedDescs g;
     static_cast<ChainPackedDescs&>(g) = d;
     g.single = f.dSingleStream;
-    return ok_or_generic(f.nStreams ? launch_huf_encode_chains_packed(g, f.nStreams, msv, tlog, (cudaStream_t)stream)
-                                    : launch_huf_encode_chains_packed_mixed(g, msv, tlog, (cudaStream_t)stream));
+    return ok_or_generic(launch_huf_encode_descs(g, f.nStreams, msv, tlog, (cudaStream_t)stream));
 }
-size_t huf_repeat_unpack(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstSizes,
-                         size_t* dResults, const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
-                         const void* const* dChainHeaders, const size_t* dChainHeaderSizes, int nStreams, void* stream,
-                         const unsigned char* dSingleStream = nullptr)
+size_t fseb::huf_repeat_unpack(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* const* dDsts, const size_t* dDstSizes,
+                               size_t* dResults, const void* dIn, const size_t* dOffsets, const unsigned char* dKinds,
+                               const void* const* dChainHeaders, const size_t* dChainHeaderSizes, int nStreams, void* stream,
+                               const unsigned char* dSingleStream)
 {
     if (nBlocks == 0) return 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull || !dChainStarts || !dDsts || !dDstSizes || !dResults || !dIn ||
@@ -369,7 +355,6 @@ size_t huf_repeat_unpack(size_t nChains, const size_t* dChainStarts, size_t nBlo
                                                              (const u64*)dOffsets, dKinds, (const u8* const*)dChainHeaders,
                                                              (const u64*)dChainHeaderSizes, (u32)nBlocks, nStreams, (cudaStream_t)stream,
                                                              dSingleStream));
-}
 }
 FSEB_API size_t FSEB200_HUF_compress4X_repeat_chains_packed(size_t nChains, const size_t* dChainStarts, size_t nBlocks, void* dOut,
                                                             size_t outCapacity, size_t* dOffsets, size_t* dCSizes, unsigned char* dKinds,
@@ -459,7 +444,7 @@ size_t huf_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffse
     PackedDescs g;
     g.out = (u8*)dOut; g.outCap = outCapacity; g.offset = (u64*)dOffsets; g.result = (u64*)dCSizes;
     g.src = (const u8* const*)dSrcs; g.srcSize = (const u64*)dSrcSizes; g.nBlocks = (u32)nBlocks;
-    return ok_or_generic(launch_huf_encode_packed(g, nStreams, msv, tlog, (cudaStream_t)stream));
+    return ok_or_generic(launch_huf_encode_descs(g, nStreams, msv, tlog, (cudaStream_t)stream));
 }
 }
 FSEB_API size_t FSEB200_HUF_compress_packed(size_t nBlocks, void* dOut, size_t outCapacity, size_t* dOffsets, size_t* dCSizes,

@@ -446,7 +446,7 @@ FSEB_API size_t FSEB200_frame_compress_device(int codec, unsigned blockSizeId, s
         else {
             PackedDescs g;
             g.out = packed; g.outCap = total; g.offset = offset; g.result = value; g.src = srcs; g.srcSize = hSize; g.nBlocks = (u32)nb;
-            e = launch_huf_encode_packed(g, 4, 255, 11, s);
+            e = launch_huf_encode_descs(g, 4, 255, 11, s);
         }
     }
     // the stream waits on the device for the checksums (also after a failure, before the scratch is freed on it); then the

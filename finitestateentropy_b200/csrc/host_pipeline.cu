@@ -270,7 +270,7 @@ cudaError_t queue_packed_compress(Ring<3>& P, int k, const HostChunk& c, int cod
     PackedDescs g;
     g.out = P.dB[k]; g.outCap = bytes; g.offset = d + L.offset; g.result = d + L.value;
     g.src = src; g.srcSize = d + L.size; g.nBlocks = (u32)cb;
-    return launch_huf_encode_packed(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
+    return launch_huf_encode_descs(g, codec == 1 ? 4 : 1, maxSymbolValue, tableLog, s);
 }
 
 // The finish of a packed compress chunk c whose offsets `lo` (chunk-local, cb + 1) and values have landed in the pinned image:
@@ -392,11 +392,11 @@ FSEB_API size_t FSEB200_decompress_host_packed(int codec, void* hDst, const size
 // ================================================================================================
 // packed chains of table reuse on HOST buffers: FSEB200_HUF_compress{4X,1X}_repeat_chains_packed and
 // FSEB200_HUF_decompress{4X,1X}_repeat_packed through the packed pair's ring and chunk budget, chain boundaries ignored; each
-// chunk runs the device call unchanged on chunk-local geometry.  Chains are contiguous ranges of blocks, so the chains that meet
-// a chunk are a contiguous range of which only the first can have started in an earlier chunk: at most one chain crosses each
-// chunk boundary, and its state (compress) or its last tree header (decompress) is all that passes from chunk to chunk.
-// codec: 1 = Huff0 4X, 3 = Huff0 1X; the mixed pair (a form per block, hSingleStream) runs the same code as codec 0, and the
-// literal-policy compress (the forms an output) as codec 0 with its own device call.
+// chunk runs the device call's helper (capi_common.h huf_repeat_chains_packed, huf_repeat_unpack) unchanged on chunk-local
+// geometry.  Chains are contiguous ranges of blocks, so the chains that meet a chunk are a contiguous range of which only the
+// first can have started in an earlier chunk: at most one chain crosses each chunk boundary, and its state (compress) or its last
+// tree header (decompress) is all that passes from chunk to chunk.  codec: 1 = Huff0 4X, 3 = Huff0 1X; the mixed pair (a form
+// per block, hSingleStream) and the literal-policy compress (the forms an output) run the same code with their own ChainForm.
 // ================================================================================================
 namespace {
 // The most of a tree header a Huff0 decoder reads (HUF_readStats: 1 + 127 bytes in the FSE form, 1 + 64 raw); a header's size
@@ -493,34 +493,31 @@ struct EntryHeader { size_t chain; const u8* p; u64 n; };
 }
 
 namespace {
-// The literal-policy compress: the forms come back in `single`, and its two thresholds
-struct LiteralsOut { unsigned char* single; unsigned minLiterals, minGainLog; };
-
-// codec 1 (4X), 3 (1X) or 0 (mixed: the form of block b from hSingle[b]; with lit, the literal policy, which writes the forms)
-size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hOut, size_t outCapacity,
-                            size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds, const void* hSrc, const size_t* hSrcSizes,
-                            const int* hPreferRepeat, const unsigned char* hSingle, unsigned* const* hCTables, int* hRepeats,
-                            const void** hChainHeaders, size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog,
-                            const LiteralsOut* lit = nullptr)
+// `form` is the device call's; its dSingleStream is set per chunk to the device copy of hSingle, the blocks' forms -- read
+// (nStreams 0) or, under the literal policy, written
+size_t host_chains_compress(const ChainForm& form, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hOut,
+                            size_t outCapacity, size_t* hOffsets, size_t* hCSizes, unsigned char* hKinds, const void* hSrc,
+                            const size_t* hSrcSizes, const int* hPreferRepeat, unsigned char* hSingle, unsigned* const* hCTables,
+                            int* hRepeats, const void** hChainHeaders, size_t* hChainHeaderSizes, unsigned maxSymbolValue,
+                            unsigned tableLog)
 {
-    bool const mixed = codec == 0 && !lit;
+    bool const lit = form.literals, mixed = !form.nStreams && !lit;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
     if (nBlocks == 0) return 0;
     if (!hChainStarts || !hOut || !hOffsets || !hCSizes || !hKinds || !hSrc || !hSrcSizes || !hPreferRepeat || !hCTables ||
-        !hRepeats || !hChainHeaders || !hChainHeaderSizes || (mixed && !hSingle) ||
-        (lit && (!lit->single || lit->minGainLog < 1 || lit->minGainLog > 31))) return (size_t)err(E_SRC_WRONG);
+        !hRepeats || !hChainHeaders || !hChainHeaderSizes || !forms_given(form.nStreams, hSingle) ||
+        (lit && (form.minGainLog < 1 || form.minGainLog > 31))) return (size_t)err(E_SRC_WRONG);
     if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
         for (size_t b = 0; b < nBlocks; b++) { hCSizes[b] = (size_t)err(E_SRC_WRONG); hKinds[b] = 4; }
         return 0;
     }
-    auto const compress = codec == 1 ? FSEB200_HUF_compress4X_repeat_chains_packed : FSEB200_HUF_compress1X_repeat_chains_packed;
     ChunkMax most;
     std::vector<HostChunk> const chunks = cut_chunks(hSrcSizes, nBlocks, 1, [](size_t) { return (u64)0; }, most);
     std::vector<ChunkChains> cc;
     size_t words = 0;
     for (const HostChunk& c : chunks) {
         cc.emplace_back(hChainStarts, nChains, c);
-        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n, mixed, lit != nullptr).end);
+        words = std::max(words, ChainCompressWords(c.b1 - c.b0, cc.back().n, mixed, lit).end);
     }
     auto& P = packed_ring();
     std::lock_guard<std::mutex> lock(P.mu);
@@ -548,7 +545,7 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
     auto queue = [&](size_t ci, int k) -> cudaError_t {
         const HostChunk& c = chunks[ci];
         size_t const cb = c.b1 - c.b0, c0 = cc[ci].c0;
-        ChainCompressWords const L(cb, cc[ci].n, mixed, lit != nullptr);
+        ChainCompressWords const L(cb, cc[ci].n, mixed, lit);
         u64 const bytes = c.a1 - c.a0;
         cudaStream_t const s = P.st[k];
         u64* const h = P.hD[k], * const d = P.dD[k];
@@ -560,33 +557,23 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
         if (bytes && (r = cudaMemcpyAsync(P.dA[k], (const u8*)hSrc + c.a0, bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if ((r = cudaMemcpyAsync(d, h, L.offset * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if (ci && (r = cudaStreamWaitEvent(s, ev.ev[(ci - 1) % P.NS], 0)) != cudaSuccess) return r;
-        size_t const v = lit
-            ? FSEB200_HUF_compress_literals_chains_packed(
-                  cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
-                  (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size), (const int*)(d + L.prefer),
-                  (unsigned char*)(d + L.singleOut), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
-                  (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, lit->minLiterals,
-                  lit->minGainLog, s)
-            : mixed
-            ? FSEB200_HUF_compress_mixed_repeat_chains_packed(
-                  cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
-                  (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size), (const int*)(d + L.prefer),
-                  (const unsigned char*)(d + L.single), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
-                  (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, s)
-            : compress(cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
-                       (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size),
-                       (const int*)(d + L.prefer), (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0,
-                       (const void**)(S.d + SL.hdr) + c0, (size_t*)(S.d + SL.hdrSize) + c0, maxSymbolValue, tableLog, s);
+        ChainForm f = form;
+        if (!f.nStreams) f.dSingleStream = (unsigned char*)(d + (lit ? L.singleOut : L.single));
+        size_t const v = huf_repeat_chains_packed(
+            cc[ci].n, (const size_t*)(d + L.start), cb, P.dB[k], bytes, (size_t*)(d + L.offset), (size_t*)(d + L.value),
+            (unsigned char*)(d + L.kind), (const void* const*)(d + L.ptr), (const size_t*)(d + L.size), (const int*)(d + L.prefer),
+            (unsigned* const*)(S.d + SL.tptr) + c0, (int*)(S.d + SL.flag) + c0, (const void**)(S.d + SL.hdr) + c0,
+            (size_t*)(S.d + SL.hdrSize) + c0, f, maxSymbolValue, tableLog, s);
         if (v) return cudaErrorLaunchFailure;
         if ((r = cudaEventRecord(ev.ev[k], s)) != cudaSuccess) return r;
         return cudaMemcpyAsync(h + L.offset, d + L.offset, (L.end - L.offset) * sizeof(u64), cudaMemcpyDeviceToHost, s);
     };
     u64 total = 0;
     auto finish = [&](size_t ci, int k) -> cudaError_t {
-        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n, mixed, lit != nullptr);
+        ChainCompressWords const L(chunks[ci].b1 - chunks[ci].b0, cc[ci].n, mixed, lit);
         cudaError_t const r = cudaStreamSynchronize(P.st[k]);
         if (r != cudaSuccess) return r;
-        if (lit) std::memcpy(lit->single + chunks[ci].b0, P.hD[k] + L.singleOut, chunks[ci].b1 - chunks[ci].b0);
+        if (lit) std::memcpy(hSingle + chunks[ci].b0, P.hD[k] + L.singleOut, chunks[ci].b1 - chunks[ci].b0);
         return finish_packed(chunks[ci], P.hD[k] + L.offset, P.hD[k] + L.value, (const u8*)(P.hD[k] + L.kind), P.dB[k], P.st[k],
                              (u8*)hOut, outCapacity, hOffsets, hCSizes, hKinds, total);
     };
@@ -607,22 +594,21 @@ size_t host_chains_compress(int codec, size_t nChains, const size_t* hChainStart
     return 0;
 }
 
-// codec 1 (4X), 3 (1X) or 0 (mixed: the form of block b from hSingle[b])
-size_t host_chains_decompress(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hDst, const size_t* hDstSizes,
+// nStreams 4 (4X), 1 (1X) or 0 (mixed: the form of block b from hSingle[b])
+size_t host_chains_decompress(int nStreams, size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hDst, const size_t* hDstSizes,
                               size_t* hResults, const void* hIn, const size_t* hOffsets, const unsigned char* hKinds,
                               const unsigned char* hSingle, const void* const* hChainHeaders, const size_t* hChainHeaderSizes)
 {
-    bool const mixed = codec == 0;
+    bool const mixed = nStreams == 0;
     if (nBlocks > 0xFFFFFFFFull || nChains > 0xFFFFFFFFull) return (size_t)err(E_SRC_WRONG);
     if (nBlocks == 0) return 0;
     if (!hChainStarts || !hDst || !hDstSizes || !hResults || !hIn || !hOffsets || !hKinds || !hChainHeaders || !hChainHeaderSizes ||
-        (mixed && !hSingle)) return (size_t)err(E_SRC_WRONG);
+        !forms_given(nStreams, hSingle)) return (size_t)err(E_SRC_WRONG);
     for (size_t b = 0; b < nBlocks; b++) if (hOffsets[b + 1] < hOffsets[b]) return (size_t)err(E_SRC_WRONG);
     if (!chains_sound(hChainStarts, nChains, nBlocks)) {            // the device call's verdicts, and nothing else written
         for (size_t b = 0; b < nBlocks; b++) hResults[b] = (size_t)err(E_SRC_WRONG);
         return 0;
     }
-    auto const decompress = codec == 1 ? FSEB200_HUF_decompress4X_repeat_packed : FSEB200_HUF_decompress1X_repeat_packed;
     ChunkMax most;
     std::vector<HostChunk> const chunks = cut_chunks(hDstSizes, nBlocks, 1, [&](size_t b) { return (u64)(hOffsets[b + 1] - hOffsets[b]); }, most);
     // The device decoder finds a kind-3 block's header in its chunk when a kind-2 block of its chain precedes it there.  Otherwise
@@ -673,15 +659,10 @@ size_t host_chains_decompress(int codec, size_t nChains, const size_t* hChainSta
         cudaError_t r;
         if (in && (r = cudaMemcpyAsync(P.dB[k], (const u8*)hIn + in0, in, cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
         if ((r = cudaMemcpyAsync(d, h, L.value * sizeof(u64), cudaMemcpyHostToDevice, s)) != cudaSuccess) return r;
-        size_t const v = mixed
-            ? FSEB200_HUF_decompress_mixed_repeat_packed(cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr),
-                                                         (const size_t*)(d + L.size), (size_t*)(d + L.value), P.dB[k],
-                                                         (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind),
-                                                         (const unsigned char*)(d + L.single), (const void* const*)(d + L.hdr),
-                                                         (const size_t*)(d + L.hdrSize), s)
-            : decompress(cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr), (const size_t*)(d + L.size),
-                         (size_t*)(d + L.value), P.dB[k], (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind),
-                         (const void* const*)(d + L.hdr), (const size_t*)(d + L.hdrSize), s);
+        size_t const v = huf_repeat_unpack(
+            cc[ci].n, (const size_t*)(d + L.start), cb, (void* const*)(d + L.ptr), (const size_t*)(d + L.size), (size_t*)(d + L.value),
+            P.dB[k], (const size_t*)(d + L.offset), (const unsigned char*)(d + L.kind), (const void* const*)(d + L.hdr),
+            (const size_t*)(d + L.hdrSize), nStreams, s, mixed ? (const unsigned char*)(d + L.single) : nullptr);
         if (v) return cudaErrorLaunchFailure;
         if (bytes && (r = cudaMemcpyAsync((u8*)hDst + c.a0, P.dA[k], bytes, cudaMemcpyDeviceToHost, s)) != cudaSuccess) return r;
         return cudaMemcpyAsync(h + L.value, d + L.value, cb * sizeof(u64), cudaMemcpyDeviceToHost, s);
@@ -706,8 +687,9 @@ FSEB_API size_t FSEB200_compress_host_repeat_chains_packed(int codec, size_t nCh
                                                            unsigned maxSymbolValue, unsigned tableLog)
 {
     if (codec != 1 && codec != 3) return (size_t)err(E_SRC_WRONG);
-    return host_chains_compress(codec, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
-                                hPreferRepeat, nullptr, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue, tableLog);
+    return host_chains_compress(ChainForm{codec == 1 ? 4 : 1}, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes,
+                                hKinds, hSrc, hSrcSizes, hPreferRepeat, nullptr, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes,
+                                maxSymbolValue, tableLog);
 }
 FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains, const size_t* hChainStarts, size_t nBlocks,
                                                       void* hDst, const size_t* hDstSizes, size_t* hResults,
@@ -715,8 +697,8 @@ FSEB_API size_t FSEB200_decompress_host_repeat_packed(int codec, size_t nChains,
                                                       const void* const* hChainHeaders, const size_t* hChainHeaderSizes)
 {
     if (codec != 1 && codec != 3) return (size_t)err(E_SRC_WRONG);
-    return host_chains_decompress(codec, nChains, hChainStarts, nBlocks, hDst, hDstSizes, hResults, hIn, hOffsets, hKinds, nullptr,
-                                  hChainHeaders, hChainHeaderSizes);
+    return host_chains_decompress(codec == 1 ? 4 : 1, nChains, hChainStarts, nBlocks, hDst, hDstSizes, hResults, hIn, hOffsets, hKinds,
+                                  nullptr, hChainHeaders, hChainHeaderSizes);
 }
 FSEB_API size_t FSEB200_compress_host_mixed_repeat_chains_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
                                                                  void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
@@ -725,9 +707,9 @@ FSEB_API size_t FSEB200_compress_host_mixed_repeat_chains_packed(size_t nChains,
                                                                  unsigned* const* hCTables, int* hRepeats, const void** hChainHeaders,
                                                                  size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog)
 {
-    return host_chains_compress(0, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
-                                hPreferRepeat, hSingleStream, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue,
-                                tableLog);
+    return host_chains_compress(ChainForm{0}, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc,
+                                hSrcSizes, hPreferRepeat, const_cast<unsigned char*>(hSingleStream), hCTables, hRepeats, hChainHeaders,
+                                hChainHeaderSizes, maxSymbolValue, tableLog);
 }
 FSEB_API size_t FSEB200_compress_host_literals_chains_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks,
                                                              void* hOut, size_t outCapacity, size_t* hOffsets, size_t* hCSizes,
@@ -737,10 +719,9 @@ FSEB_API size_t FSEB200_compress_host_literals_chains_packed(size_t nChains, con
                                                              size_t* hChainHeaderSizes, unsigned maxSymbolValue, unsigned tableLog,
                                                              unsigned minLiterals, unsigned minGainLog)
 {
-    LiteralsOut const lit = { hSingleStream, minLiterals, minGainLog };
-    return host_chains_compress(0, nChains, hChainStarts, nBlocks, hOut, outCapacity, hOffsets, hCSizes, hKinds, hSrc, hSrcSizes,
-                                hPreferRepeat, nullptr, hCTables, hRepeats, hChainHeaders, hChainHeaderSizes, maxSymbolValue,
-                                tableLog, &lit);
+    return host_chains_compress(ChainForm{0, nullptr, true, minLiterals, minGainLog}, nChains, hChainStarts, nBlocks, hOut, outCapacity,
+                                hOffsets, hCSizes, hKinds, hSrc, hSrcSizes, hPreferRepeat, hSingleStream, hCTables, hRepeats,
+                                hChainHeaders, hChainHeaderSizes, maxSymbolValue, tableLog);
 }
 FSEB_API size_t FSEB200_decompress_host_mixed_repeat_packed(size_t nChains, const size_t* hChainStarts, size_t nBlocks, void* hDst,
                                                             const size_t* hDstSizes, size_t* hResults, const void* hIn,

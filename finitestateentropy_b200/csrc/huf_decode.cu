@@ -663,6 +663,32 @@ huf_decode_kernel(Geo g, u8* __restrict__ dst, const u8* __restrict__ cbuf, cons
     }
 }
 
+// ---- mixed forms (single[b]: 0 4X, else 1X): the header decoder runs once per form over the same batch.  Each launch sees the other
+// form's blocks with a size above HUF_BLOCK_MAX, which it settles as srcSize_wrong without reading or writing a byte; the 1X launch
+// writes its verdicts to scratch, and the merge takes them for the 1X blocks.
+constexpr int FORM_THREADS = 256;
+struct HufMixedSplit {
+    const u64* dstCap; const u8* single; u64* cap4; u64* cap1; const u64* res1; u64* result;
+    u32 nBlocks;
+};
+
+__global__ void __launch_bounds__(FORM_THREADS) huf_mixed_split_kernel(HufMixedSplit g)
+{
+    u64 const b = (u64)blockIdx.x * FORM_THREADS + threadIdx.x;
+    if (b >= g.nBlocks) return;
+    u64 const n = g.dstCap[b], none = (u64)HUF_BLOCK_MAX + 1;
+    bool const one = g.single[b] != 0;
+    g.cap4[b] = one ? none : n;
+    g.cap1[b] = one ? n : none;
+}
+
+__global__ void __launch_bounds__(FORM_THREADS) huf_mixed_merge_kernel(HufMixedSplit g)
+{
+    u64 const b = (u64)blockIdx.x * FORM_THREADS + threadIdx.x;
+    if (b >= g.nBlocks) return;
+    if (g.single[b]) g.result[b] = g.res1[b];
+}
+
 }  // namespace hufd
 
 namespace {
@@ -746,11 +772,29 @@ cudaError_t launch_huf_decode_blocks(const BlockDescs& g, int nStreams, cudaStre
 }
 
 // header-less blocks (HeaderDescs): X1 verdicts only -- HUF_decompress{4X,1X}1_DCtx for a block with its own header, HUF_readDTableX1
-// on the caller's header + HUF_decompress{4X,1X}1_usingDTable otherwise.  The same passes, budgets and grid shape.
-cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream)
+// on the caller's header + HUF_decompress{4X,1X}1_usingDTable otherwise.  The same passes, budgets and grid shape.  nStreams 0: each
+// block in the form single[b] names, one decode per form (hufd::HufMixedSplit).
+cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream, const u8* single)
 {
-    return nStreams == 1 ? huf_decode<HeaderDescs, 1>(g, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 1u)
-                         : huf_decode<HeaderDescs, 4>(g, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 1u);
+    if (nStreams == 1) return huf_decode<HeaderDescs, 1>(g, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 1u);
+    if (nStreams) return huf_decode<HeaderDescs, 4>(g, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 1u);
+    if (g.nBlocks == 0) return cudaSuccess;
+    size_t const n = g.nBlocks;
+    cudaError_t e;
+    u64* const s = (u64*)stream_scratch(13, stream, 3 * sizeof(u64) * n, &e);       // cap4, cap1, the 1X launch's verdicts
+    if (e != cudaSuccess) return e;
+    hufd::HufMixedSplit m;
+    m.dstCap = g.dstCap; m.single = single; m.cap4 = s; m.cap1 = s + n; m.res1 = s + 2 * n; m.result = g.result; m.nBlocks = g.nBlocks;
+    unsigned const grid = (unsigned)((n + hufd::FORM_THREADS - 1) / hufd::FORM_THREADS);
+    hufd::huf_mixed_split_kernel<<<grid, hufd::FORM_THREADS, 0, stream>>>(m);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    HeaderDescs d = g;
+    d.dstCap = m.cap4;
+    if ((e = huf_decode<HeaderDescs, 4>(d, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 1u)) != cudaSuccess) return e;
+    d.dstCap = m.cap1; d.result = s + 2 * n;
+    if ((e = huf_decode<HeaderDescs, 1>(d, nullptr, nullptr, nullptr, nullptr, nullptr, stream, 1u)) != cudaSuccess) return e;
+    hufd::huf_mixed_merge_kernel<<<grid, hufd::FORM_THREADS, 0, stream>>>(m);
+    return cudaGetLastError();
 }
 
 }  // namespace fseb

@@ -1279,55 +1279,42 @@ cudaError_t launch_huf_encode(const BatchGeom& g, void* cbuf, u64* csizes, const
     return huf_encode<BatchGeom, 4>(g, cbuf, csizes, src, msv, tlog, stream);
 }
 
-// The descriptor geometries, nStreams 4 (the 4X format) or 1 (1X); the host never reads their arrays:
+// The descriptor geometries (launchers.h launch_huf_encode_descs); the host never reads their arrays:
 //   BlockDescs        HUF_compress2 / HUF_compress1X per block
 //   PackedDescs       the same, with the scan and placement between plan and emit
 //   RepeatDescs       HUF_compress4X_repeat / HUF_compress1X_repeat per block (table reuse)
 //   ChainDescs        chains of table reuse: plan, the chains' decisions, emit -- the repeat call block after block per chain
 //   ChainPackedDescs  packed chains: plan, the chains' decisions, the placement scan and raw copies, emit, the streams' state
-//   Mixed<...>        either chain geometry with a form per block: the same steps, and two emit launches (4X, 1X)
-//   ChainPackedLiteralsDescs  packed chains under zstd's literal policy: as Mixed<ChainPackedDescs>, the forms and kinds decided by
-//                     the chain kernel, the placement and raw copies by kind
+//   Mixed<...>        either chain geometry with a form per block (stream mode 0): the same steps, and two emit launches (4X, 1X)
+//   ChainPackedLiteralsDescs  packed chains under zstd's literal policy, stream mode 0 only: as Mixed<ChainPackedDescs>, the forms
+//                     and kinds decided by the chain kernel, the placement and raw copies by kind
+namespace {
+// the geometry a call runs as when every block takes the form nStreams names: a Mixed<Base> runs as its Base
+template <class Geo> struct OneForm { using type = Geo; };
+template <class Base> struct OneForm<Mixed<Base>> { using type = Base; };
+}  // namespace
 template <class Geo>
-static cudaError_t huf_encode_descs(const Geo& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
+cudaError_t launch_huf_encode_descs(const Geo& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
 {
-    return nStreams == 1 ? huf_encode<Geo, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
-                         : huf_encode<Geo, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+    using One = typename OneForm<Geo>::type;
+    if constexpr (std::is_same_v<Geo, ChainPackedLiteralsDescs>) {
+        return nStreams ? cudaErrorInvalidValue : huf_encode<Geo, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+    } else {
+        if constexpr (!std::is_same_v<One, Geo>)
+            if (nStreams == 0) return huf_encode<Geo, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+        return nStreams == 1 ? huf_encode<One, 1>(g, nullptr, nullptr, nullptr, msv, tlog, stream)
+                             : huf_encode<One, 4>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
+    }
 }
-cudaError_t launch_huf_encode_blocks(const BlockDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode_descs(g, nStreams, msv, tlog, stream);
-}
-cudaError_t launch_huf_encode_packed(const PackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode_descs(g, nStreams, msv, tlog, stream);
-}
-cudaError_t launch_huf_encode_repeat(const RepeatDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode_descs(g, nStreams, msv, tlog, stream);
-}
-cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode_descs(g, nStreams, msv, tlog, stream);
-}
-cudaError_t launch_huf_encode_chains_packed(const ChainPackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode_descs(g, nStreams, msv, tlog, stream);
-}
-// mixed chains (common.cuh Mixed): each block in the form its flag names -- stream mode 0
-cudaError_t launch_huf_encode_chains_mixed(const ChainMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode<ChainMixedDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
-}
-cudaError_t launch_huf_encode_chains_packed_mixed(const ChainPackedMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode<ChainPackedMixedDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
-}
-// packed chains under the literal policy (common.cuh ChainPackedLiteralsDescs): stream mode 0, the forms decided by the chain kernel
-cudaError_t launch_huf_encode_literals_chains_packed(const ChainPackedLiteralsDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream)
-{
-    return huf_encode<ChainPackedLiteralsDescs, 0>(g, nullptr, nullptr, nullptr, msv, tlog, stream);
-}
+// defined for these geometries only: a call on any other fails to link
+template cudaError_t launch_huf_encode_descs(const BlockDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const PackedDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const RepeatDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const ChainDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const ChainPackedDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const ChainMixedDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const ChainPackedMixedDescs&, int, unsigned, unsigned, cudaStream_t);
+template cudaError_t launch_huf_encode_descs(const ChainPackedLiteralsDescs&, int, unsigned, unsigned, cudaStream_t);
 
 // the chain geometry's verdict (start[0] == 0, start[nChains] == nBlocks, never decreasing) to *malformed, for the decoders
 cudaError_t launch_huf_chain_check(const u64* start, u32 nChains, u32 nBlocks, u32* malformed, cudaStream_t stream)

@@ -7,8 +7,7 @@
 //   2. the descriptor decoder (pass A, pass B, the X2 verdict pass) on them;
 //   3. a kernel gives an empty block (n == 0 and L == 0, what the packed compress stores for it) the result 0 -- the decoder
 //      answers dstSize 0 with dstSize_tooSmall.
-// It also holds the decompress of packed chains of table reuse (FSEB200_HUF_decompress{4X,1X,_mixed}_repeat_packed), below, and the
-// header decoder over blocks of both forms (FSEB200_HUF_decompress_mixed_repeat_blocks).
+// It also holds the decompress of packed chains of table reuse (FSEB200_HUF_decompress{4X,1X,_mixed}_repeat_packed), below.
 #include "common.cuh"
 #include "launchers.h"
 #include "launch_util.cuh"
@@ -123,53 +122,7 @@ __global__ void __launch_bounds__(pack::COPY_THREADS) huf_chain_stored_kernel(Hu
     if (threadIdx.x == 0) g.result[b] = act == ACT_SRC_WRONG ? err(E_SRC_WRONG) : act == ACT_CORRUPT ? err(E_CORRUPT) : n;
 }
 
-// ---- mixed forms (single[b]: 0 4X, else 1X): the header decoder runs once per form over the same batch.  Each launch sees the other
-// form's blocks with a size above HUF_BLOCK_MAX, which it settles as srcSize_wrong without reading or writing a byte; the 1X launch
-// writes its verdicts to scratch, and the merge takes them for the 1X blocks.
-struct HufMixedSplit {
-    const u64* dstCap; const u8* single; u64* cap4; u64* cap1; const u64* res1; u64* result;
-    u32 nBlocks;
-};
-
-__global__ void __launch_bounds__(THREADS) huf_mixed_split_kernel(HufMixedSplit g)
-{
-    u64 const b = (u64)blockIdx.x * THREADS + threadIdx.x;
-    if (b >= g.nBlocks) return;
-    u64 const n = g.dstCap[b], none = (u64)HUF_BLOCK_MAX + 1;
-    bool const one = g.single[b] != 0;
-    g.cap4[b] = one ? none : n;
-    g.cap1[b] = one ? n : none;
-}
-
-__global__ void __launch_bounds__(THREADS) huf_mixed_merge_kernel(HufMixedSplit g)
-{
-    u64 const b = (u64)blockIdx.x * THREADS + threadIdx.x;
-    if (b >= g.nBlocks) return;
-    if (g.single[b]) g.result[b] = g.res1[b];
-}
-
 }  // namespace hufp
-
-cudaError_t launch_huf_decode_headers_mixed(const HeaderDescs& g, const u8* single, cudaStream_t stream)
-{
-    if (g.nBlocks == 0) return cudaSuccess;
-    size_t const n = g.nBlocks;
-    cudaError_t e;
-    u64* const s = (u64*)stream_scratch(13, stream, 3 * sizeof(u64) * n, &e);       // cap4, cap1, the 1X launch's verdicts
-    if (e != cudaSuccess) return e;
-    hufp::HufMixedSplit m;
-    m.dstCap = g.dstCap; m.single = single; m.cap4 = s; m.cap1 = s + n; m.res1 = s + 2 * n; m.result = g.result; m.nBlocks = g.nBlocks;
-    unsigned const grid = (unsigned)((n + hufp::THREADS - 1) / hufp::THREADS);
-    hufp::huf_mixed_split_kernel<<<grid, hufp::THREADS, 0, stream>>>(m);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    HeaderDescs d = g;
-    d.dstCap = m.cap4;
-    if ((e = launch_huf_decode_headers(d, 4, stream)) != cudaSuccess) return e;
-    d.dstCap = m.cap1; d.result = s + 2 * n;
-    if ((e = launch_huf_decode_headers(d, 1, stream)) != cudaSuccess) return e;
-    hufp::huf_mixed_merge_kernel<<<grid, hufp::THREADS, 0, stream>>>(m);
-    return cudaGetLastError();
-}
 
 cudaError_t launch_huf_decompress_repeat_packed(const u64* start, u32 nChains, u8* const* dst, const u64* dstSize, u64* result,
                                                 const u8* in, const u64* offset, const u8* kind, const u8* const* chainHdr,
@@ -199,8 +152,7 @@ cudaError_t launch_huf_decompress_repeat_packed(const u64* start, u32 nChains, u
     HeaderDescs d;
     d.dst = dst; d.dstCap = g.decCap; d.result = result; d.src = g.decSrc; d.srcSize = g.decSize; d.nBlocks = nBlocks;
     d.hdr = g.hdr; d.hdrSize = g.hdrSize;
-    e = nStreams ? launch_huf_decode_headers(d, nStreams, stream) : launch_huf_decode_headers_mixed(d, single, stream);
-    if (e != cudaSuccess) return e;
+    if ((e = launch_huf_decode_headers(d, nStreams, stream, single)) != cudaSuccess) return e;
     pack::launch_per_block(hufp::huf_chain_stored_kernel, n, stream, g);
     return cudaGetLastError();
 }

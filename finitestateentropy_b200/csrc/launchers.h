@@ -16,20 +16,15 @@ cudaError_t launch_fse_encode(const BatchGeom& g, void* cbuf, u64* csizes, const
 cudaError_t launch_fseu16_decode(const BatchGeom& g, void* dst, const void* cbuf, const u64* csizes, u64* results, const void* orig, cudaStream_t s);
 cudaError_t launch_fseu16_encode(const BatchGeom& g, void* cbuf, u64* csizes, const void* src, unsigned msv, unsigned tlog, cudaStream_t s);
 
-// per-block descriptors (common.cuh BlockDescs, PackedDescs)
-cudaError_t launch_huf_encode_blocks(const BlockDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
-cudaError_t launch_huf_encode_packed(const PackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
+// per-block descriptors (common.cuh BlockDescs, PackedDescs, ...).  The Huff0 encoder of every descriptor geometry, instantiated
+// for each in huf_encode.cu: nStreams 4 (the 4X format) or 1 (1X) for every block, or 0 for the per-block forms of Mixed<...> and
+// ChainPackedLiteralsDescs (which takes 0 only).  A Mixed<Base> with nStreams 4 or 1 runs as its Base.
+template <class Geo>
+cudaError_t launch_huf_encode_descs(const Geo& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_decode_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
-cudaError_t launch_huf_encode_repeat(const RepeatDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
-cudaError_t launch_huf_encode_chains(const ChainDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
-cudaError_t launch_huf_encode_chains_packed(const ChainPackedDescs& g, int nStreams, unsigned msv, unsigned tlog, cudaStream_t stream);
-cudaError_t launch_huf_encode_chains_mixed(const ChainMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream);
-cudaError_t launch_huf_encode_chains_packed_mixed(const ChainPackedMixedDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream);
-cudaError_t launch_huf_encode_literals_chains_packed(const ChainPackedLiteralsDescs& g, unsigned msv, unsigned tlog, cudaStream_t stream);
 cudaError_t launch_huf_chain_check(const u64* start, u32 nChains, u32 nBlocks, u32* malformed, cudaStream_t stream);
-cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream);
-// the same per block in the form single[b] names (0: 4X, else 1X), huf_packed.cu
-cudaError_t launch_huf_decode_headers_mixed(const HeaderDescs& g, const u8* single, cudaStream_t stream);
+// nStreams 4 or 1 for every block, or 0: per block, the form single[b] names (0: 4X, else 1X)
+cudaError_t launch_huf_decode_headers(const HeaderDescs& g, int nStreams, cudaStream_t stream, const u8* single = nullptr);
 cudaError_t launch_huf_x2_fixup_blocks(const BlockDescs& g, int nStreams, cudaStream_t stream);
 cudaError_t launch_fse_encode_blocks(const BlockDescs& g, bool wide, unsigned msv, unsigned tlog, cudaStream_t s);
 cudaError_t launch_fse_decode_blocks(const BlockDescs& g, bool wide, cudaStream_t s);
@@ -44,7 +39,7 @@ cudaError_t launch_huf_decompress_packed(u8* const* dst, const u64* dstSize, u64
 cudaError_t launch_huf_decompress_repeat_packed(const u64* start, u32 nChains, u8* const* dst, const u64* dstSize, u64* result,
                                                 const u8* in, const u64* offset, const u8* kind, const u8* const* chainHdr,
                                                 const u64* chainHdrSize, u32 nBlocks, int nStreams, cudaStream_t stream,
-                                                const u8* single = nullptr);   // nStreams 0: per block, the form single[b] names
+                                                const u8* single = nullptr);   // as launch_huf_decode_headers
 // A whole batch of frames laid out at once (the device-memory call): frame f is blocks [first[f], first[f + 1]), role[b] >> 32
 // is block b's frame, and every frame has a block (an empty frame a placeholder of 0 source bytes).  offsets (nFrames + 1) and
 // results get the batch call's values, and only frames that end at or before `capacity` are written; work: frame_body_work bytes.
