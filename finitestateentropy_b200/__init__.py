@@ -7,14 +7,19 @@ device memory / streams / torch.distributed.  There is NO CPU implementation her
 library is missing, importing `lib()` raises."""
 import ctypes as C
 import os
+import re
 
 from . import _build
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+HEADER = os.path.join(os.path.dirname(_HERE), "include", "fse_b200.h")
 _LIB = None
 
-c_sz = C.c_size_t
-c_vp = C.c_void_p
+# the scalar C types prototypes() maps; any pointer is c_void_p, except a `const char*` return (c_char_p)
+_SCALARS = {"size_t": C.c_size_t, "unsigned": C.c_uint, "int": C.c_int, "double": C.c_double, "unsigned char": C.c_ubyte,
+            "uint32_t": C.c_uint32, "uint64_t": C.c_uint64}
+# words that are part of a type, never a parameter's name: `unsigned long` or `int size_t` raises rather than losing a word
+_C_TYPE_WORDS = {"void", "char", "short", "int", "long", "float", "double", "signed", "unsigned", "struct", "union", "enum"} | set(_SCALARS)
 
 BLOCK_SIZE = 32768                     # programs/bench.c:98
 ERR_MAXCODE = 9                        # lib/error_public.h:55
@@ -37,7 +42,8 @@ def error_code(code):
 
 
 def lib():
-    """Loads (building in-tree first if needed) the CUDA library.  Fails loudly; never falls back."""
+    """Loads (building in-tree first if needed) the CUDA library, every prototype of include/fse_b200.h declared on it.  Fails
+    loudly; never falls back."""
     global _LIB
     if _LIB is None:
         path = _build.LIB
@@ -48,80 +54,55 @@ def lib():
                 if not os.path.exists(path):
                     raise RuntimeError("libfse_b200.so is missing and cannot be built: %r -- there is no CPU fallback" % (exc,))
         L = C.CDLL(path)
-        _declare(L)
+        declare(L, HEADER)
         _LIB = L
     return _LIB
 
 
-def _declare(L):
-    def sig(name, res, *args):
-        f = getattr(L, name)
-        f.restype = res
-        f.argtypes = list(args)
+def _ctype(decl, name, is_return):
+    """ctypes type of a C return type, or of a parameter declaration (its name, if any, last)"""
+    t = " ".join(re.sub(r"\bconst\b", " ", decl).split())
+    if "*" in t:
+        return C.c_char_p if is_return and t.replace(" ", "") == "char*" else C.c_void_p
+    if is_return and t == "void":
+        return None
+    if not is_return and t not in _SCALARS:
+        head, _, last = t.rpartition(" ")
+        if re.fullmatch(r"[A-Za-z_]\w*", last) and last not in _C_TYPE_WORDS:    # the parameter's name
+            t = head
+    if t not in _SCALARS:
+        raise ValueError("%s: no ctypes mapping for the C type %r" % (name, decl.strip()))
+    return _SCALARS[t]
 
-    sig("FSEB200_batch_blocks", c_sz, c_sz, c_sz)
-    sig("FSEB200_HUF_decompress_batch", c_sz, c_vp, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp)
-    sig("HUF_decompress", c_sz, c_vp, c_sz, c_vp, c_sz)
-    sig("FSEB200_HUF_compress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    sig("FSEB200_HUF_decompress_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_HUF_compress1X_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    sig("FSEB200_HUF_decompress1X_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    for name in ("FSEB200_HUF_compress4X_repeat_blocks", "FSEB200_HUF_compress1X_repeat_blocks"):
-        sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    for name in ("FSEB200_HUF_compress4X_repeat_chains", "FSEB200_HUF_compress1X_repeat_chains"):
-        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    for name in ("FSEB200_HUF_compress4X_repeat_chains_packed", "FSEB200_HUF_compress1X_repeat_chains_packed"):
-        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    for name in ("FSEB200_HUF_decompress4X_repeat_packed", "FSEB200_HUF_decompress1X_repeat_packed"):
-        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    for name in ("FSEB200_HUF_decompress4X_repeat_blocks", "FSEB200_HUF_decompress1X_repeat_blocks"):
-        sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_HUF_compress_mixed_repeat_chains", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    sig("FSEB200_HUF_decompress_mixed_repeat_blocks", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_HUF_compress_mixed_repeat_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    sig("FSEB200_HUF_decompress_mixed_repeat_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp)
-    sig("FSEB200_HUF_compress_literals_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint, c_vp)
-    for name in ("FSEB200_HUF_compress_packed", "FSEB200_HUF_compress1X_packed"):
-        sig(name, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-    for codec in ("FSE", "FSEU16"):
-        sig("FSEB200_%s_compress_blocks" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp)
-        sig("FSEB200_%s_decompress_blocks" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-        sig("FSEB200_%s_compress_packed" % codec, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, c_vp, c_sz, c_vp)
-        sig("FSEB200_%s_decompress_packed" % codec, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_FSE_packed_workspace", c_sz, c_sz, c_sz)
-    for name in ("FSEB200_HUF_decompress_packed", "FSEB200_HUF_decompress1X_packed"):
-        sig(name, c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_compress_host_packed", c_sz, C.c_int, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_sz, C.c_uint, C.c_uint)
-    sig("FSEB200_decompress_host_packed", c_sz, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz)
-    sig("FSEB200_compress_host_repeat_chains_packed", c_sz, C.c_int, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint)
-    sig("FSEB200_decompress_host_repeat_packed", c_sz, C.c_int, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_compress_host_mixed_repeat_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint)
-    sig("FSEB200_decompress_host_mixed_repeat_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_compress_host_literals_chains_packed", c_sz, c_sz, c_vp, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-        c_vp, c_vp, c_vp, c_vp, C.c_uint, C.c_uint, C.c_uint, C.c_uint)
-    sig("FSEB200_frame_compressBound", c_sz, c_sz, C.c_uint)
-    sig("FSEB200_frame_compress_host", c_sz, C.c_int, C.c_uint, c_vp, c_sz, c_vp, c_sz)
-    sig("FSEB200_frame_decompress_bound", c_sz, c_vp, c_sz)
-    sig("FSEB200_frame_decompress_host", c_sz, c_vp, c_sz, c_vp, c_sz)
-    sig("FSEB200_frame_compress_host_batch", c_sz, C.c_int, C.c_uint, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_frame_decompress_host_batch", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_frame_compress_device", c_sz, C.c_int, C.c_uint, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_frame_decompress_bound_device", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_frame_decompress_device", c_sz, c_sz, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp)
-    sig("FSEB200_XXH32", C.c_uint, c_vp, c_sz, C.c_uint)
-    for name in ("FSEB200_HUF_compress_batch", "FSEB200_FSE_compress_batch", "FSEB200_FSE_decompress_batch",
-                 "FSEB200_FSEU16_compress_batch", "FSEB200_FSEU16_decompress_batch"):
-        if hasattr(L, name):
-            if "decompress" in name:
-                sig(name, c_sz, c_vp, c_sz, c_sz, c_vp, c_sz, c_vp, c_vp, c_vp, c_vp)
-            else:
-                sig(name, c_sz, c_vp, c_sz, c_vp, c_vp, c_sz, c_sz, C.c_uint, C.c_uint, c_vp)
+
+def prototypes(header_path):
+    """{name: (restype, argtypes)} of every `ret name(args);` prototype in a C header.  Comments and preprocessor lines are
+    ignored; a statement that is not such a prototype, or a type without a mapping, raises."""
+    text = open(header_path).read()
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^[ \t]*#.*$", " ", text, flags=re.M)
+    out = {}
+    for stmt in text.split(";"):
+        stmt = re.split(r"[{}]", stmt)[-1].strip()    # what follows `extern "C" {` or an enum's braces
+        if not stmt:
+            continue
+        m = re.fullmatch(r"([\w\s*]+?)\s*\b(\w+)\s*\(([^()]*)\)", stmt)
+        if not m:
+            raise ValueError("%s: not a prototype: %r" % (header_path, stmt))
+        ret, name, args = m.groups()
+        args = [] if args.strip() in ("", "void") else args.split(",")
+        out[name] = (_ctype(ret, name, True), [_ctype(a, name, False) for a in args])
+    return out
+
+
+def declare(lib, header_path, names=None):
+    """Sets restype and argtypes on the ctypes.CDLL `lib` for every prototype of `header_path` (only `names`, if given).  A name
+    the library does not export raises AttributeError."""
+    protos = prototypes(header_path)
+    for name in protos if names is None else names:
+        f = getattr(lib, name)
+        f.restype, f.argtypes = protos[name]
+    return lib
 
 
 from .batch import (huf_decompress_batch, huf_compress_batch, fse_compress_batch, fse_decompress_batch,  # noqa: E402,F401

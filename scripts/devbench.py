@@ -1,6 +1,6 @@
 """Developer micro-benchmark (not the judged bench.py): times one batched kernel on HBM-resident data.
 usage: python scripts/devbench.py {huf_enc|huf_dec|fse_enc|fse_dec|u16_enc|u16_dec} [MiB] [p] [iters]"""
-import ctypes as C, os, sys
+import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import finitestateentropy_b200 as fb
@@ -16,11 +16,9 @@ codec, op = what.split("_")
 src = torch.empty(n, dtype=torch.uint8, device="cuda")
 st = torch.cuda.current_stream().cuda_stream
 if codec == "u16":
-    L.FSEB200_genU16.restype = C.c_size_t; L.FSEB200_genU16.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_uint, C.c_double, C.c_uint, C.c_void_p]
     assert L.FSEB200_genU16(src.data_ptr(), n // 2, 0, 240, p, 1, st) == 0
     SLOT = 32768; enc = lambda **k: fb.fseu16_compress_batch(src, BLOCK, SLOT, 0, 12, **k); dec = fb.fseu16_decompress_batch
 else:
-    L.FSEB200_probagen.restype = C.c_size_t; L.FSEB200_probagen.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_double, C.c_void_p]
     assert L.FSEB200_probagen(src.data_ptr(), n, 0, p, st) == 0
     SLOT = fb.compress_bound(BLOCK)
     e = fb.huf_compress_batch if codec == "huf" else fb.fse_compress_batch

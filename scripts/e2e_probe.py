@@ -1,12 +1,11 @@
 """Developer probe: PCIe copy rates and the two host-API phases timed separately (wall clock, host buffers pinned)."""
-import ctypes as C, os, sys, time
+import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import finitestateentropy_b200 as fb
 L = fb.lib()
 n = 1 << 30; BLOCK = 32768; SLOT = fb.compress_bound(BLOCK); nb = n // BLOCK
 src = torch.empty(n, dtype=torch.uint8, device="cuda")
-L.FSEB200_probagen.restype = C.c_size_t; L.FSEB200_probagen.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_double, C.c_void_p]
 L.FSEB200_probagen(src.data_ptr(), n, 0, 0.14, torch.cuda.current_stream().cuda_stream); torch.cuda.synchronize()
 h_src = torch.empty(n, dtype=torch.uint8, pin_memory=True); h_src.copy_(src)
 h_c = torch.empty(nb * SLOT + 64, dtype=torch.uint8, pin_memory=True)
@@ -24,9 +23,6 @@ def both():
     d.copy_(h_src, non_blocking=True)
     with torch.cuda.stream(s2): h_out.copy_(src, non_blocking=True)
 print("H2D+D2H concurrently 1 GiB each  %.2f ms" % t(both))
-for name, a in (("FSEB200_compress_host", [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_uint, C.c_uint]),
-                ("FSEB200_decompress_host", [C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p])):
-    f = getattr(L, name); f.restype = C.c_size_t; f.argtypes = a
 print("compress_host   %.2f ms" % t(lambda: L.FSEB200_compress_host(1, h_c.data_ptr(), SLOT, h_cs.data_ptr(), h_src.data_ptr(), n, BLOCK, 255, 12)))
 print("decompress_host %.2f ms" % t(lambda: L.FSEB200_decompress_host(1, h_out.data_ptr(), n, BLOCK, h_c.data_ptr(), SLOT, h_cs.data_ptr(), h_res.data_ptr(), h_src.data_ptr())))
 print("ok", bool(torch.equal(h_out, h_src)), "csum", int(h_cs.sum()))

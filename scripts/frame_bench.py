@@ -84,13 +84,7 @@ def main():
     import torch
     import finitestateentropy_b200 as fb
     from helpers import probagen
-    import ctypes as C
     L = fb.lib()
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    L.FSEB200_compress_host.restype = sz
-    L.FSEB200_compress_host.argtypes = [C.c_int, vp, sz, vp, vp, sz, sz, u, u]
-    L.FSE_compressBound.restype = sz
-    L.FSE_compressBound.argtypes = [sz]
     n = int(args.gib * GIB)
     out = {"bench": "frame", "runs": args.runs, "bytes": n, "block_size_id": BID}
     out.update(gpu_info())

@@ -30,22 +30,10 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 GIB = 1 << 30
 BLOCK = 32768
-
-
-def declare(L):
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    L.FSEB200_probagen.restype = sz; L.FSEB200_probagen.argtypes = [vp, sz, sz, C.c_double, vp]
-    L.FSEB200_genU16.restype = sz; L.FSEB200_genU16.argtypes = [vp, sz, sz, u, C.c_double, u, vp]
-    for codec in ("FSE", "FSEU16"):
-        for name, args in (("compress_batch", [vp, sz, vp, vp, sz, sz, u, u, vp]), ("decompress_batch", [vp, sz, sz, vp, sz, vp, vp, vp, vp]),
-                           ("compress_blocks", [sz, vp, vp, vp, vp, vp, u, u, vp]), ("decompress_blocks", [sz, vp, vp, vp, vp, vp, vp]),
-                           ("compress_packed", [sz, vp, sz, vp, vp, vp, vp, u, u, vp, sz, vp]), ("decompress_packed", [sz, vp, vp, vp, vp, vp, vp])):
-            f = getattr(L, "FSEB200_%s_%s" % (codec, name))
-            f.restype = sz; f.argtypes = args
-    L.FSEB200_FSE_packed_workspace.restype = sz; L.FSEB200_FSE_packed_workspace.argtypes = [sz, sz]
 
 
 def fbound(n):
@@ -82,8 +70,8 @@ def encoder_shares(sizes, wide):
 def child(codec, reps):
     import numpy as np
     import torch
-    L = C.CDLL(os.path.join(ROOT, "finitestateentropy_b200", "libfse_b200.so"))
-    declare(L)
+    import finitestateentropy_b200 as fb
+    L = fb.declare(C.CDLL(os.path.join(ROOT, "finitestateentropy_b200", "libfse_b200.so")), fb.HEADER)
     wide = codec == "u16"
     w = 2 if wide else 1
     name = "FSEU16" if wide else "FSE"

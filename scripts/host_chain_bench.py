@@ -30,15 +30,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--runs", type=int, default=5)
     args = ap.parse_args()
-    import ctypes as C
     import numpy as np
     import torch
     import finitestateentropy_b200 as fb
     from host_packed_bench import gpu_info
     torch.cuda.set_device(0)
     L = fb.lib()
-    sz, vp = C.c_size_t, C.c_void_p
-    L.FSEB200_probagen.restype = sz; L.FSEB200_probagen.argtypes = [vp, sz, sz, C.c_double, vp]
     total, n = GIB, GIB // BLOCK
 
     def pinned(k, dtype=torch.uint8):

@@ -18,7 +18,6 @@ line with the GPU's name, power limit and SM clocks.
     python scripts/host_packed_bench.py --runs 5
 """
 import argparse
-import ctypes as C
 import json
 import os
 import statistics
@@ -102,12 +101,6 @@ def main():
     import finitestateentropy_b200 as fb
     torch.cuda.set_device(0)
     L = fb.lib()
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    L.FSEB200_probagen.restype = sz; L.FSEB200_probagen.argtypes = [vp, sz, sz, C.c_double, vp]
-    L.FSEB200_compress_host.restype = sz
-    L.FSEB200_compress_host.argtypes = [C.c_int, vp, sz, vp, vp, sz, sz, u, u]
-    L.FSEB200_decompress_host.restype = sz
-    L.FSEB200_decompress_host.argtypes = [C.c_int, vp, sz, sz, vp, sz, vp, vp, vp]
     total = int(args.gib * GIB) // BLOCK * BLOCK
     slot = fb.compress_bound(BLOCK)
 

@@ -40,27 +40,10 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 GIB = 1 << 30
 BLOCK = 32768
-
-
-def declare(L):
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    L.FSEB200_probagen.restype = sz; L.FSEB200_probagen.argtypes = [vp, sz, sz, C.c_double, vp]
-    L.FSEB200_HUF_compress_batch.restype = sz; L.FSEB200_HUF_compress_batch.argtypes = [vp, sz, vp, vp, sz, sz, u, u, vp]
-    L.FSEB200_HUF_decompress_batch.restype = sz; L.FSEB200_HUF_decompress_batch.argtypes = [vp, sz, sz, vp, sz, vp, vp, vp, vp]
-    have = hasattr(L, "FSEB200_HUF_compress_blocks")
-    have1x = hasattr(L, "FSEB200_HUF_compress1X_blocks")
-    for suffix, present in (("", have), ("1X", have1x)):
-        if present:
-            f = getattr(L, "FSEB200_HUF_compress%s_blocks" % suffix); f.restype = sz; f.argtypes = [sz, vp, vp, vp, vp, vp, u, u, vp]
-            f = getattr(L, "FSEB200_HUF_decompress%s_blocks" % suffix); f.restype = sz; f.argtypes = [sz, vp, vp, vp, vp, vp, vp]
-    have_packed = hasattr(L, "FSEB200_HUF_compress_packed")
-    if have_packed:
-        for suffix in ("", "1X"):
-            f = getattr(L, "FSEB200_HUF_compress%s_packed" % suffix); f.restype = sz; f.argtypes = [sz, vp, sz, vp, vp, vp, vp, u, u, vp]
-    return have, have1x, have_packed
 
 
 def ragged_sizes(total, seed=7, lo=1024, hi=128 * 1024):
@@ -92,13 +75,10 @@ def cpu_ref_rates(src_host, nblocks):
     """the compiled reference's single-thread HUF_compress1X / HUF_decompress1X_DCtx on the first nblocks 32 KB blocks: ms per GiB"""
     import time
     import numpy as np
-    path = os.path.join(ROOT, "oracle", "_ref", "libfse_ref.so")
-    if not os.path.exists(path):
+    from helpers import REF_SO, load_ref
+    if not os.path.exists(REF_SO):
         return None
-    R = C.CDLL(path)
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    R.HUF_compress1X.restype = sz; R.HUF_compress1X.argtypes = [vp, sz, vp, sz, u, u]
-    R.HUF_decompress1X_DCtx.restype = sz; R.HUF_decompress1X_DCtx.argtypes = [vp, vp, sz, vp, sz]
+    R = load_ref()
     bound = 129 + BLOCK + (BLOCK >> 8) + 8
     cbuf = np.zeros(nblocks * bound + 64, np.uint8)
     out = np.zeros(BLOCK + 64, np.uint8)
@@ -120,8 +100,11 @@ def cpu_ref_rates(src_host, nblocks):
 def child(lib_path, reps):
     import numpy as np
     import torch
+    import finitestateentropy_b200 as fb
     L = C.CDLL(lib_path)
-    have, have1x, have_packed = declare(L)
+    fb.declare(L, fb.HEADER, [n for n in fb.prototypes(fb.HEADER) if hasattr(L, n)])   # an older build lacks the later calls
+    have, have1x, have_packed = (hasattr(L, n) for n in ("FSEB200_HUF_compress_blocks", "FSEB200_HUF_compress1X_blocks",
+                                                         "FSEB200_HUF_compress_packed"))
     dev = torch.device("cuda")
     stream = torch.cuda.current_stream().cuda_stream
     slot = 512 + BLOCK + (BLOCK >> 7) + 12

@@ -10,7 +10,6 @@ Every shape is warmed up, and the chain call's values are checked against the lo
 gives the kernels' own device time per call (plan, the chains' decisions, emit).
 Prints one JSON line: the GPU's name and power limit, and per case the median and range in ms per GiB of source bytes."""
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -51,8 +50,6 @@ def main():
     n = int(args.gib * GIB) // BLOCK * BLOCK
     nb = n // BLOCK
     L = fb.lib()
-    L.FSEB200_probagen.restype = ctypes.c_size_t
-    L.FSEB200_probagen.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_double, ctypes.c_void_p]
     src = torch.empty(n, dtype=torch.uint8, device="cuda")
     assert L.FSEB200_probagen(src.data_ptr(), n, 0, 0.14, torch.cuda.current_stream().cuda_stream) == 0
     cap = fb.compress_bound(BLOCK)

@@ -45,10 +45,7 @@ def timed(fn):
 
 
 def p14(n, seed):
-    import ctypes
     L = fb.lib()
-    L.FSEB200_probagen.restype = ctypes.c_size_t
-    L.FSEB200_probagen.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_double, ctypes.c_void_p]
     src = torch.empty(n, dtype=torch.uint8, device="cuda")
     assert L.FSEB200_probagen(src.data_ptr(), n, seed, 0.14, torch.cuda.current_stream().cuda_stream) == 0
     return src

@@ -11,7 +11,6 @@ the plain descriptor call of the same blocks, run by run:
   dec_ext   decode of header-less blocks (the `valid` output) with external headers.
 Prints one JSON line: the GPU's name and power limit, and per case the median and range in ms per GiB of source bytes."""
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -49,17 +48,16 @@ def main():
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--gib", type=float, default=1.0)
     args = ap.parse_args()
-    from huf_repeat_cases import ref_lib, ref_table, table_header
+    from helpers import load_ref
+    from huf_repeat_cases import ref_table, table_header
     import numpy as np
     n = int(args.gib * GIB) // BLOCK * BLOCK
     nb = n // BLOCK
     L = fb.lib()
-    L.FSEB200_probagen.restype = ctypes.c_size_t
-    L.FSEB200_probagen.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_double, ctypes.c_void_p]
     src = torch.empty(n, dtype=torch.uint8, device="cuda")
     assert L.FSEB200_probagen(src.data_ptr(), n, 0, 0.14, torch.cuda.current_stream().cuda_stream) == 0
     sample = src[:65536].cpu().numpy()
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         raise SystemExit("the compiled reference (oracle/_ref) builds the check table and its header")
     table = ref_table(ref, sample)

@@ -1,11 +1,10 @@
 import sys, os
 sys.path.insert(0, "/root/repo")
-import torch, ctypes as C
+import torch
 import finitestateentropy_b200 as fb
 L = fb.lib()
 n = 4 << 20
 src = torch.empty(n, dtype=torch.uint8, device="cuda")
-L.FSEB200_probagen.restype = C.c_size_t; L.FSEB200_probagen.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_double, C.c_void_p]
 L.FSEB200_probagen(src.data_ptr(), n, 0, 0.14, torch.cuda.current_stream().cuda_stream)
 ts=[]
 cb, cs = fb.huf_compress_batch(src, 32768, fb.compress_bound(32768), 255, 12)

@@ -4,9 +4,13 @@ and builds the input zoo modelled on the reference fuzzers' buffers
 import ctypes as C
 import os
 import subprocess
+import sys
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:                 # tests/golden/make_golden.py and the scripts put only tests/ on the path
+    sys.path.insert(0, ROOT)
+import finitestateentropy_b200 as fb     # noqa: E402
 ORACLE_DIR = os.path.join(ROOT, "oracle")
 PORT_SO = os.path.join(ORACLE_DIR, "_build", "libfse_oracle.so")
 REF_SO = os.path.join(ORACLE_DIR, "_ref", "libfse_ref.so")
@@ -25,6 +29,11 @@ def err_code(r):
     return (2 ** 64 - r) if is_error(r) else 0
 
 
+def declared_arity():
+    """{name: parameter count} of every prototype the binding reads from include/fse_b200.h"""
+    return {n: len(args) for n, (_, args) in fb.prototypes(fb.HEADER).items()}
+
+
 def _sig(fn, res, *args):
     fn.restype = res
     fn.argtypes = list(args)
@@ -36,50 +45,13 @@ _ref = None
 
 
 def load_port():
-    """our plain-C restatement (always buildable: gcc only)"""
+    """our plain-C restatement (always buildable: gcc only), declared from oracle/fse_oracle.h"""
     global _port
     if _port is None:
         src = os.path.join(ORACLE_DIR, "fse_oracle.c")
         if (not os.path.exists(PORT_SO)) or os.path.getmtime(PORT_SO) < os.path.getmtime(src):
             subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "port"])
-        L = C.CDLL(PORT_SO)
-        P = C.POINTER
-        _sig(L.orc_hist_count, sz, P(u), P(u), vp, sz)
-        _sig(L.orc_optimal_tablelog, u, u, sz, u, u)
-        _sig(L.orc_fse_normalize, sz, P(C.c_short), u, P(u), sz, u)
-        _sig(L.orc_fse_ncount_bound, sz, u, u)
-        _sig(L.orc_fse_write_ncount, sz, vp, sz, P(C.c_short), u, u)
-        _sig(L.orc_fse_read_ncount, sz, P(C.c_short), P(u), P(u), vp, sz)
-        _sig(L.orc_fse_build_ctable, sz, vp, P(C.c_short), u, u)
-        _sig(L.orc_fse_build_dtable, sz, vp, P(C.c_short), u, u)
-        _sig(L.orc_fse_build_dtable_u16, sz, vp, P(C.c_short), u, u)
-        _sig(L.orc_fse_encode, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_fse_decode, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_fse_compress2, sz, vp, sz, vp, sz, u, u)
-        _sig(L.orc_fse_decompress, sz, vp, sz, vp, sz)
-        _sig(L.orc_fse_compress_u16, sz, vp, sz, vp, sz, u, u)
-        _sig(L.orc_fse_decompress_u16, sz, vp, sz, vp, sz)
-        _sig(L.orc_huf_build_ctable, sz, vp, P(u), u, u)
-        _sig(L.orc_huf_write_ctable, sz, vp, sz, vp, u, u)
-        _sig(L.orc_huf_encode4x, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_huf_encode1x, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_huf_compress2, sz, vp, sz, vp, sz, u, u)
-        _sig(L.orc_huf_read_stats, sz, vp, sz, vp, P(C.c_uint32), P(C.c_uint32), vp, sz)
-        _sig(L.orc_huf_read_dtable_x1, sz, vp, vp, sz)
-        _sig(L.orc_huf_read_dtable_x2, sz, vp, vp, sz)
-        _sig(L.orc_huf_decode4x2, sz, vp, sz, vp, sz, vp); _sig(L.orc_huf_decode1x2, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_huf_decode4x1, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_huf_decode1x1, sz, vp, sz, vp, sz, vp)
-        _sig(L.orc_huf_decompress, sz, vp, sz, vp, sz)
-        _sig(L.orc_huf_decompress4x1, sz, vp, sz, vp, sz); _sig(L.orc_huf_decompress4x2, sz, vp, sz, vp, sz)
-        _sig(L.orc_huf_select_decoder, u, sz, sz)
-        _sig(L.orc_probagen, None, vp, sz, C.c_double)
-        _sig(L.orc_gen_u16, None, vp, sz, u, C.c_double, C.c_uint32)
-        _sig(L.orc_xxh64, C.c_uint64, vp, sz, C.c_uint64)
-        _sig(L.orc_xxh32, C.c_uint32, vp, sz, C.c_uint32)
-        _sig(L.orc_compress_blocks, sz, C.c_int, vp, sz, sz, vp, sz, vp, u, u)
-        _sig(L.orc_decompress_blocks, sz, C.c_int, vp, vp, sz, sz, vp, sz, vp, vp)
-        _port = L
+        _port = fb.declare(C.CDLL(PORT_SO), os.path.join(ORACLE_DIR, "fse_oracle.h"))
     return _port
 
 
@@ -88,7 +60,9 @@ def have_ref():
 
 
 def load_ref():
-    """the unmodified reference library compiled by oracle/Makefile (None if it cannot be had)"""
+    """the unmodified reference library compiled by oracle/Makefile (None if it cannot be had).  Its calls are declared from
+    include/fse_b200.h, which states the reference API's prototypes (tests/golden/ref_prototype_arity.json pins their arity);
+    the few it does not state are declared here."""
     global _ref
     if _ref is None:
         if not os.path.exists(REF_SO):
@@ -96,46 +70,12 @@ def load_ref():
                 return None
             subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "ref"])
         L = C.CDLL(REF_SO)
-        P = C.POINTER
-        _sig(L.HIST_count, sz, P(u), P(u), vp, sz)
-        _sig(L.FSE_optimalTableLog, u, u, sz, u)
-        _sig(L.HUF_optimalTableLog, u, u, sz, u)
-        _sig(L.FSE_normalizeCount, sz, P(C.c_short), u, P(u), sz, u)
-        _sig(L.FSE_NCountWriteBound, sz, u, u)
-        _sig(L.FSE_writeNCount, sz, vp, sz, P(C.c_short), u, u)
-        _sig(L.FSE_readNCount, sz, P(C.c_short), P(u), P(u), vp, sz)
-        _sig(L.FSE_buildCTable, sz, vp, P(C.c_short), u, u)
-        _sig(L.FSE_buildCTableU16, sz, vp, P(C.c_short), u, u)
-        _sig(L.FSE_buildDTable, sz, vp, P(C.c_short), u, u)
-        _sig(L.FSE_buildDTableU16, sz, vp, P(C.c_short), u, u)
-        _sig(L.FSE_compress_usingCTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.FSE_decompress_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.FSE_compress2, sz, vp, sz, vp, sz, u, u)
-        _sig(L.FSE_compress, sz, vp, sz, vp, sz)
-        _sig(L.FSE_decompress, sz, vp, sz, vp, sz)
-        _sig(L.FSE_compressBound, sz, sz)
-        _sig(L.FSE_compressU16, sz, vp, sz, vp, sz, u, u)
-        _sig(L.FSE_decompressU16, sz, vp, sz, vp, sz)
-        _sig(L.HUF_buildCTable, sz, vp, P(u), u, u)
-        _sig(L.HUF_writeCTable, sz, vp, sz, vp, u, u)
-        _sig(L.HUF_compress4X_usingCTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_compress1X_usingCTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_compress2, sz, vp, sz, vp, sz, u, u)
-        _sig(L.HUF_compress, sz, vp, sz, vp, sz)
-        _sig(L.HUF_readStats, sz, vp, sz, vp, P(C.c_uint32), P(C.c_uint32), vp, sz)
-        _sig(L.HUF_readDTableX1, sz, vp, vp, sz)
-        _sig(L.HUF_readDTableX2, sz, vp, vp, sz)
-        _sig(L.HUF_decompress4X2_usingDTable, sz, vp, sz, vp, sz, vp); _sig(L.HUF_decompress1X2_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_readDTableX2, sz, vp, vp, sz)
-        _sig(L.HUF_decompress4X2_usingDTable, sz, vp, sz, vp, sz, vp); _sig(L.HUF_decompress1X2_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_decompress4X1_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_decompress4X2_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_decompress4X_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_decompress1X1_usingDTable, sz, vp, sz, vp, sz, vp)
-        _sig(L.HUF_decompress, sz, vp, sz, vp, sz)
-        _sig(L.HUF_decompress4X1, sz, vp, sz, vp, sz)
-        _sig(L.HUF_decompress4X2, sz, vp, sz, vp, sz)
-        _sig(L.HUF_selectDecoder, C.c_uint32, sz, sz)
+        fb.declare(L, fb.HEADER, [n for n in fb.prototypes(fb.HEADER) if n.startswith(("FSE_", "HUF_", "HIST_")) and hasattr(L, n)])
+        _sig(L.FSE_buildCTableU16, sz, vp, vp, u, u)
+        _sig(L.FSE_buildDTableU16, sz, vp, vp, u, u)
+        _sig(L.FSE_compressU16_usingCTable, sz, vp, sz, vp, sz, vp)
+        for name in ("HUF_decompress4X1_DCtx", "HUF_decompress1X1_DCtx", "HUF_decompress1X_DCtx"):
+            _sig(getattr(L, name), sz, vp, vp, sz, vp, sz)
         _sig(L.refshim_compress_blocks, C.c_double, C.c_int, vp, sz, sz, vp, sz, vp, u, u, C.c_int)
         _sig(L.refshim_decompress_blocks, C.c_double, C.c_int, vp, vp, sz, sz, vp, sz, vp, vp, C.c_int)
         _ref = L

@@ -6,8 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import ptr, is_error
-from huf_repeat_cases import ref_lib, bound
+from helpers import ptr, is_error, load_ref
+from huf_repeat_cases import bound
 from huf_chain_cases import ref_chain, chain_header
 from huf_chain_packed_cases import expected, resolve_headers
 from huf_mixed_chain_cases import ref_mixed_chain, expected_mixed
@@ -25,7 +25,7 @@ BLOCK_OVERHEAD = 512                                    # what a block adds to a
 
 
 def _ref():
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
     return ref

@@ -6,9 +6,9 @@ import itertools
 
 import numpy as np
 
-from helpers import load_ref, ptr, probagen, is_error
+from helpers import ptr, probagen, is_error
 
-S, V, U = C.c_size_t, C.c_void_p, C.c_uint
+U = C.c_uint
 FLAGS = (0, 1, 2, 3, -1)
 PREFERS = (0, 1)
 SIZES = (0, 1, 5, 11, 12, 4099, 32768, 131072, 131073)
@@ -23,27 +23,6 @@ def bound(n):
 def room(n, cap):
     """bytes of destination a block can be written into at capacity `cap` (more is never touched: <= 12 bits per symbol)"""
     return min(cap, 2 * n + 1024)
-
-
-def ref_lib():
-    ref = load_ref()
-    if ref is None:
-        return None
-    for name in ("HUF_compress4X_repeat", "HUF_compress1X_repeat"):
-        f = getattr(ref, name)
-        f.restype = S
-        f.argtypes = [V, S, V, S, U, U, V, S, V, C.POINTER(C.c_int), C.c_int, C.c_int]
-    ref.HUF_readCTable.restype = S
-    ref.HUF_readCTable.argtypes = [V, C.POINTER(U), V, S, C.POINTER(U)]
-    ref.HUF_estimateCompressedSize.restype = S
-    ref.HUF_estimateCompressedSize.argtypes = [V, V, U]
-    ref.HUF_validateCTable.restype = C.c_int
-    ref.HUF_validateCTable.argtypes = [V, V, U]
-    for name in ("HUF_decompress4X1_DCtx", "HUF_decompress1X1_DCtx"):
-        f = getattr(ref, name)
-        f.restype = S
-        f.argtypes = [V, V, S, V, S]
-    return ref
 
 
 def ref_table(ref, data, tlog=12):

@@ -5,7 +5,6 @@ reference, non-zero (with the assertion) otherwise.
 Sweep: Huff0, FSE and U16 batches of mixed fixtures at two block sizes and three placements through gpu_common.placed_check,
 and the host-buffer tier (FSEB200_compress_host / decompress_host) for the three codecs with raw / RLE blocks and a ragged
 last block."""
-import ctypes as C
 import os
 import sys
 
@@ -59,10 +58,6 @@ def host_tier():
     """FSEB200_compress_host / decompress_host against the reference: at FSEB200_HOST_CHUNK_BLOCKS=64 the 400 blocks below are
     seven chunks, more than the pipeline's four streams"""
     L = fb.lib()
-    L.FSEB200_compress_host.restype = C.c_size_t
-    L.FSEB200_compress_host.argtypes = [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_uint, C.c_uint]
-    L.FSEB200_decompress_host.restype = C.c_size_t
-    L.FSEB200_decompress_host.argtypes = [C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     rng = np.random.default_rng(44)
     block = 4096
     for codec, cid in (("huf", 1), ("fse", 0), ("u16", 2)):

@@ -2,7 +2,6 @@
 the stored length of a block from its compress value, the offsets, the capacity rule, and the packed image built from the
 compiled reference's HUF_compress2 / HUF_compress1X at HUF_compressBound(n).  Used by tests/test_packed_model.py (CPU) and
 tests/test_gpu_packed.py (the GPU calls against it)."""
-import ctypes as C
 
 import numpy as np
 
@@ -34,17 +33,6 @@ def layout(vals, sizes, out_capacity):
         fits.append(ok and not is_error(int(v)))
         final.append(int(v) if ok else ERR_DST_TOO_SMALL)
     return offs, final, fits
-
-
-def ref_lib(lib):
-    """the compiled reference with the single-stream calls declared"""
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    for name, res, args in (("HUF_compress1X", sz, (vp, sz, vp, sz, u, u)),
-                            ("HUF_decompress1X_DCtx", sz, (vp, vp, sz, vp, sz))):
-        f = getattr(lib, name)
-        f.restype = res
-        f.argtypes = list(args)
-    return lib
 
 
 def ref_values(lib, srcs, msv, tl, onex=False):

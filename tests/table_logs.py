@@ -147,16 +147,8 @@ def fse_steps(ref, cap, data, msv, tl):
     return total, bytes(hdr) + bytes(body[:cs])
 
 
-def _u16_sigs(ref):
-    ref.FSE_countU16.restype = C.c_size_t
-    ref.FSE_countU16.argtypes = [C.POINTER(U), C.POINTER(U), C.c_void_p, C.c_size_t]
-    ref.FSE_compressU16_usingCTable.restype = C.c_size_t
-    ref.FSE_compressU16_usingCTable.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
-
-
 def u16_steps(ref, cap, data, msv, tl):
     """FSE_compressU16 (lib/fseU16.c:203-251) one reference function at a time: (value, bytes [0, value))"""
-    _u16_sigs(ref)
     data = np.ascontiguousarray(data, np.uint16)
     n = len(data)
     if n <= 1:
@@ -259,7 +251,6 @@ def u16_tl13_stream(ref, data, tl=13):
     nrm = (C.c_short * 300)(*norm)
     assert ref.FSE_buildCTableU16(ptr(ct), nrm, msv, tl) == 0
     hdr = write_ncount(norm, msv, tl)
-    _u16_sigs(ref)
     body = np.zeros(bound(2 * len(data)) + 16, np.uint8)
     cs = ref.FSE_compressU16_usingCTable(ptr(body), bound(2 * len(data)), ptr(data), len(data), ptr(ct))
     assert 0 < cs and not is_error(cs)

@@ -31,6 +31,17 @@ def test_library_builds_loads_and_exports_everything():
     lib = ctypes.CDLL(path)
     missing = [n for n in _declared() if not hasattr(lib, n)]
     assert not missing, missing
+    # the binding declares exactly the prototypes this independent scan names: one the parser skipped or misread shows here
+    assert sorted(fb.prototypes(fb.HEADER)) == _declared()
+    assert all(getattr(fb.lib(), n).argtypes is not None for n in _declared())
+    # a type without a mapping raises, even when its last word could be read as a parameter's name
+    import tempfile
+    import pytest
+    with tempfile.TemporaryDirectory() as d:
+        for proto in ("size_t f(unsigned long);", "size_t f(unsigned short n);", "size_t f(int size_t);", "long f(int n);"):
+            open(os.path.join(d, "h.h"), "w").write(proto)
+            with pytest.raises(ValueError):
+                fb.prototypes(os.path.join(d, "h.h"))
     exported = subprocess.check_output(["nm", "-D", "--defined-only", path]).decode()
     assert " T HUF_decompress" in exported and " T FSEB200_HUF_decompress_batch" in exported
     # scalar helpers are host arithmetic and may be called without a GPU
@@ -70,11 +81,10 @@ def test_constant_pattern_tables_match_the_reference():
         import pytest
         pytest.skip("compiled reference not available")
     lib = ctypes.CDLL(_build.build_lib())
-    for L in (lib, ref):
-        for n in ("FSE_buildCTable_raw", "FSE_buildDTable_raw"):
-            f = getattr(L, n); f.restype = ctypes.c_size_t; f.argtypes = [ctypes.c_void_p, ctypes.c_uint]
-        for n in ("FSE_buildCTable_rle", "FSE_buildDTable_rle"):
-            f = getattr(L, n); f.restype = ctypes.c_size_t; f.argtypes = [ctypes.c_void_p, ctypes.c_ubyte]
+    for n in ("FSE_buildCTable_raw", "FSE_buildDTable_raw"):
+        f = getattr(lib, n); f.restype = ctypes.c_size_t; f.argtypes = [ctypes.c_void_p, ctypes.c_uint]
+    for n in ("FSE_buildCTable_rle", "FSE_buildDTable_rle"):
+        f = getattr(lib, n); f.restype = ctypes.c_size_t; f.argtypes = [ctypes.c_void_p, ctypes.c_ubyte]
     for nb in range(0, 9):
         a = np.zeros(1 + 128 + 2 * 256 + 8, np.uint32); b = np.zeros_like(a)
         ra, rb = lib.FSE_buildCTable_raw(ptr(a), nb), ref.FSE_buildCTable_raw(ptr(b), nb)
@@ -121,11 +131,9 @@ def test_ctable_helpers_match_the_reference():
         pytest.skip("compiled reference not available")
     lib = ctypes.CDLL(_build.build_lib())
     U = ctypes.c_uint
-    for L in (lib, ref):
-        L.HUF_getNbBits.restype = U; L.HUF_getNbBits.argtypes = [ctypes.c_void_p, U]
-        L.HUF_estimateCompressedSize.restype = ctypes.c_size_t; L.HUF_estimateCompressedSize.argtypes = [ctypes.c_void_p, ctypes.c_void_p, U]
-        L.HUF_validateCTable.restype = ctypes.c_int; L.HUF_validateCTable.argtypes = [ctypes.c_void_p, ctypes.c_void_p, U]
-    ref.HUF_buildCTable.restype = ctypes.c_size_t; ref.HUF_buildCTable.argtypes = [ctypes.c_void_p, ctypes.c_void_p, U, U]
+    lib.HUF_getNbBits.restype = U; lib.HUF_getNbBits.argtypes = [ctypes.c_void_p, U]
+    lib.HUF_estimateCompressedSize.restype = ctypes.c_size_t; lib.HUF_estimateCompressedSize.argtypes = [ctypes.c_void_p, ctypes.c_void_p, U]
+    lib.HUF_validateCTable.restype = ctypes.c_int; lib.HUF_validateCTable.argtypes = [ctypes.c_void_p, ctypes.c_void_p, U]
     rng = np.random.default_rng(5)
     for it in range(20):
         msv = int(rng.integers(1, 256))

@@ -9,6 +9,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from helpers import declared_arity
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = os.path.join(ROOT, "oracle", "_ref", "fse_ref")
 NEW_CALLS = {"FSEB200_frame_compressBound": 2, "FSEB200_frame_compress_host": 6,
@@ -26,14 +28,8 @@ def _lib():
     return fb.lib()
 
 
-def _declarations():
-    text = open(os.path.join(ROOT, "include", "fse_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return {m.group(1): m.group(2).count(",") + 1 for m in re.finditer(r"\b(FSEB200_\w+)\s*\(([^;]*)\)\s*;", text)}
-
-
 def test_header_declares_the_frame_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in NEW_CALLS} == NEW_CALLS
 
 

@@ -8,7 +8,8 @@ import subprocess
 import numpy as np
 import pytest
 
-from test_frame_abi import _declarations, _frame, _stored_frames, ERR, MAGIC
+from helpers import declared_arity
+from test_frame_abi import _frame, _stored_frames, ERR, MAGIC
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BATCH_CALLS = {"FSEB200_frame_compress_host_batch": 9, "FSEB200_frame_decompress_host_batch": 6}
@@ -25,7 +26,7 @@ def _words(values):
 
 
 def test_header_declares_and_library_exports_the_batch_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in BATCH_CALLS} == BATCH_CALLS
     from finitestateentropy_b200 import _build
     exported = subprocess.check_output(["nm", "-D", "--defined-only", _build.build_lib()]).decode()

@@ -8,7 +8,8 @@ import subprocess
 import numpy as np
 import pytest
 
-from test_frame_abi import _declarations, ERR, MAGIC
+from helpers import declared_arity
+from test_frame_abi import ERR, MAGIC
 
 DEVICE_CALLS = {"FSEB200_frame_compress_device": 10, "FSEB200_frame_decompress_bound_device": 5,
                 "FSEB200_frame_decompress_device": 7}
@@ -25,7 +26,7 @@ def _words(values):
 
 
 def test_header_declares_and_library_exports_the_device_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in DEVICE_CALLS} == DEVICE_CALLS
     from finitestateentropy_b200 import _build
     exported = subprocess.check_output(["nm", "-D", "--defined-only", _build.build_lib()]).decode()

@@ -6,7 +6,6 @@ checks.  The block contents and layouts are those of tests/test_gpu_blocks.py (i
 
 Run as a script (`python tests/test_gpu_blocks_1x.py --child`) it repeats subsets of the ragged tests under the environment it
 was started with: test_knobs_1x starts it with FSEB200_HUFD_ROWS / _ROWS_B set."""
-import ctypes as C
 import os
 import subprocess
 import sys
@@ -26,18 +25,6 @@ from test_gpu_blocks import (POISON, CANARY, ERR_SRC_WRONG, SPECIAL_SIZES, conte
 pytestmark = pytest.mark.gpu
 
 DTABLE_X2_MAX = 12 * 0x01000001                     # HUF_CREATE_STATIC_DTABLEX2(dctx, HUF_TABLELOG_MAX) header
-
-
-def _ref1x():
-    lib = _ref()
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    for name, res, args in (("HUF_compress1X", sz, (vp, sz, vp, sz, u, u)),
-                            ("HUF_decompress1X_DCtx", sz, (vp, vp, sz, vp, sz)),
-                            ("HUF_decompress1X1", sz, (vp, sz, vp, sz))):
-        f = getattr(lib, name)
-        f.restype = res
-        f.argtypes = list(args)
-    return lib
 
 
 # ---- reference side ---------------------------------------------------------------------------------------------------------
@@ -171,7 +158,7 @@ def ragged_compress1x_check(seed, count, subset_every):
     rng = np.random.default_rng(seed)
     host, offs, sizes = ragged_sources(rng, count)
     assert set(SPECIAL_SIZES) <= set(sizes)
-    lib = _ref1x()
+    lib = _ref()
     at_bound, _ = ref_compress1x(lib, host, offs, sizes, [hbound(n) for n in sizes], 255, 12)
     caps = capacities_1x(rng, sizes, at_bound)
     want = check_compress1x(lib, host, offs, sizes, caps, 255, 12)
@@ -193,7 +180,7 @@ def packed_decode1x_fixture(seed, count):
     import torch
     import finitestateentropy_b200 as fb
     rng = np.random.default_rng(seed)
-    lib = _ref1x()
+    lib = _ref()
     sizes = [int(x) for x in rng.integers(6, HUF_BLOCK_MAX + 1, count // 2)] + \
             [int(rng.choice((8192, 32768, 4099, 777, 40, 13))) for _ in range(count - count // 2)]
     datas = [content(rng, n, i if i % 9 not in (6, 7) else 1) for i, n in enumerate(sizes)]   # compressible kinds only
@@ -259,7 +246,7 @@ def test_head_decode_every_residue_1x(p, kind):
     """blocks of 32,771 symbols, block b's output at residue b mod 32: its one stream decodes (-b) & 31 head symbols"""
     import torch
     import finitestateentropy_b200 as fb
-    lib = _ref1x()
+    lib = _ref()
     n = 32771
     data = [probagen(n + 97 * i, p)[97 * i:] for i in range(64)]
     blocks, csizes = [], []
@@ -293,7 +280,7 @@ def test_large_batch_two_rounds_1x():
     sizes = [int(x) for x in rng.integers(64, 3000, 64000)] + [32768] * 300
     order = rng.permutation(len(sizes))
     sizes = [sizes[i] for i in order]
-    lib = _ref1x()
+    lib = _ref()
     host, offs, sizes = ragged_sources(rng, len(sizes), sizes)
     want = check_compress1x(lib, host, offs, sizes, [hbound(n) for n in sizes], 255, 12)
     idx = [i for i, v in enumerate(want) if 1 < int(v) and not is_error(int(v))]
@@ -312,7 +299,7 @@ def test_large_batch_two_rounds_1x():
 
 def test_knobs_1x():
     """the single-pass decoder at the smallest row budget, in a child process"""
-    _ref1x()
+    _ref()
     e = dict(os.environ, FSEB200_HUFD_ROWS="160", FSEB200_HUFD_ROWS_B="0")
     r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, capture_output=True, text=True, timeout=1200)
     assert r.returncode == 0 and "child ok" in r.stdout, (r.stdout[-2000:], r.stderr[-4000:])

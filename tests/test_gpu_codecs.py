@@ -104,13 +104,6 @@ def test_u16_zoo():
 def test_golden_small_vectors_through_host_api():
     """tests/golden/vectors_small.npz through the reference-named one-block entry points (host pointers)"""
     L = fb.lib()
-    for name, res, args in (("FSE_compress2", C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, U, U]),
-                            ("HUF_compress2", C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, U, U]),
-                            ("FSE_compressU16", C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, U, U]),
-                            ("FSE_decompress", C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
-                            ("HUF_decompress", C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
-                            ("FSE_decompressU16", C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t])):
-        f = getattr(L, name); f.restype = res; f.argtypes = args
     z = np.load(os.path.join(HERE, "golden", "vectors_small.npz"))
     for k in range(int(z["count"][0])):
         d = np.ascontiguousarray(z["in_%d" % k]); codec = int(z["codec_%d" % k][0])
@@ -181,20 +174,9 @@ def test_table_level_api_images():
     if not isref:
         pytest.skip("table images are compared against the compiled reference only")
     L = fb.lib()
-    P = C.POINTER
-    def sig(n, *a):
-        f = getattr(L, n); f.restype = C.c_size_t; f.argtypes = list(a); return f
-    g_hist = sig("HIST_count", P(U), P(U), C.c_void_p, C.c_size_t)
-    g_norm = sig("FSE_normalizeCount", P(C.c_short), U, P(U), C.c_size_t, U)
-    g_wn = sig("FSE_writeNCount", C.c_void_p, C.c_size_t, P(C.c_short), U, U)
-    g_rn = sig("FSE_readNCount", P(C.c_short), P(U), P(U), C.c_void_p, C.c_size_t)
-    g_ct = sig("FSE_buildCTable", C.c_void_p, P(C.c_short), U, U)
-    g_dt = sig("FSE_buildDTable", C.c_void_p, P(C.c_short), U, U)
-    g_hct = sig("HUF_buildCTable", C.c_void_p, P(U), U, U)
-    g_hw = sig("HUF_writeCTable", C.c_void_p, C.c_size_t, C.c_void_p, U, U)
-    g_hrs = sig("HUF_readStats", C.c_void_p, C.c_size_t, P(C.c_uint32), P(C.c_uint32), P(C.c_uint32), C.c_void_p, C.c_size_t)
-    g_hdt = sig("HUF_readDTableX1", C.c_void_p, C.c_void_p, C.c_size_t)
-    L.FSE_optimalTableLog.argtypes = [U, C.c_size_t, U]; L.HUF_optimalTableLog.argtypes = [U, C.c_size_t, U]
+    g_hist, g_norm, g_wn, g_rn = L.HIST_count, L.FSE_normalizeCount, L.FSE_writeNCount, L.FSE_readNCount
+    g_ct, g_dt, g_hct, g_hw, g_hrs, g_hdt = (L.FSE_buildCTable, L.FSE_buildDTable, L.HUF_buildCTable, L.HUF_writeCTable, L.HUF_readStats,
+                                             L.HUF_readDTableX1)
     rng = np.random.default_rng(25)
     for it in range(25):
         n = int(rng.integers(300, 40000)); d = zoo(rng, n)
@@ -251,12 +233,8 @@ def test_table_level_api_images():
         assert np.array_equal(dA[:ncell], dB[:ncell])
         # payload coding with the caller's tables: FSE_compress_usingCTable / FSE_decompress_usingDTable /
         # HUF_compress4X_usingCTable / HUF_decompress4X[1]_usingDTable (same images on both sides)
-        g_euc = sig("FSE_compress_usingCTable", C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
-        g_dud = sig("FSE_decompress_usingDTable", C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
-        g_huc = sig("HUF_compress4X_usingCTable", C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
-        g_hud = sig("HUF_decompress4X_usingDTable", C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
-        for r_ in ("FSE_compress_usingCTable", "FSE_decompress_usingDTable", "HUF_compress4X_usingCTable", "HUF_decompress4X_usingDTable"):
-            f = getattr(lib, r_); f.restype = C.c_size_t; f.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+        g_euc, g_dud = L.FSE_compress_usingCTable, L.FSE_decompress_usingDTable
+        g_huc, g_hud = L.HUF_compress4X_usingCTable, L.HUF_decompress4X_usingDTable
         for cap in (n + 600, max(16, n // 3)):
             oa = np.zeros(cap + 16, np.uint8); ob = np.zeros(cap + 16, np.uint8)
             ea = g_euc(ptr(oa), cap, ptr(d), n, ptr(ctb)); eb = lib.FSE_compress_usingCTable(ptr(ob), cap, ptr(d), n, ptr(ctb))
@@ -372,13 +350,6 @@ def test_raw_and_rle_tables_through_payload_calls():
     if not isref:
         pytest.skip("needs the compiled reference")
     L = fb.lib()
-    def sig(M, n, *a):
-        f = getattr(M, n); f.restype = C.c_size_t; f.argtypes = list(a); return f
-    for M in (L, lib):
-        sig(M, "FSE_buildCTable_raw", C.c_void_p, U); sig(M, "FSE_buildDTable_raw", C.c_void_p, U)
-        sig(M, "FSE_buildCTable_rle", C.c_void_p, C.c_ubyte); sig(M, "FSE_buildDTable_rle", C.c_void_p, C.c_ubyte)
-        sig(M, "FSE_compress_usingCTable", C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
-        sig(M, "FSE_decompress_usingDTable", C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
     rng = np.random.default_rng(77)
     for nb in (1, 3, 6, 8):
         n = int(rng.integers(50, 5000))
@@ -409,13 +380,6 @@ def test_single_stream_huff0():
     if not isref:
         pytest.skip("needs the compiled reference")
     L = fb.lib()
-    for M in (L, lib):
-        for n_, a_ in (("HUF_compress1X", [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, U, U]),
-                       ("HUF_decompress1X1", [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
-                       ("HUF_compress1X_usingCTable", [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
-                       ("HUF_buildCTable", [C.c_void_p, C.c_void_p, U, U]),
-                       ("HIST_count", [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t])):
-            f = getattr(M, n_); f.restype = C.c_size_t; f.argtypes = a_
     rng = np.random.default_rng(91)
     for it in range(14):
         n = int(rng.integers(1, 30000)) if it else 20000
@@ -452,14 +416,6 @@ def test_double_symbol_table_and_decoders():
     if not isref:
         pytest.skip("needs the compiled reference")
     L = fb.lib()
-    S = C.c_size_t; V = C.c_void_p
-    for M in (L, lib):
-        for n_, a_ in (("HUF_readDTableX2", [V, V, S]), ("HUF_decompress4X2_usingDTable", [V, S, V, S, V]), ("HUF_decompress1X2_usingDTable", [V, S, V, S, V]),
-                       ("HUF_decompress4X_usingDTable", [V, S, V, S, V]), ("HUF_decompress1X_usingDTable", [V, S, V, S, V]),
-                       ("HUF_compress4X_usingCTable", [V, S, V, S, V]), ("HUF_compress1X_usingCTable", [V, S, V, S, V]),
-                       ("HUF_buildCTable", [V, V, U, U]), ("HUF_writeCTable", [V, S, V, U, U]), ("HIST_count", [V, V, V, S])):
-            f = getattr(M, n_); f.restype = S; f.argtypes = a_
-    lib.HUF_optimalTableLog.argtypes = [U, S, U]
     rng = np.random.default_rng(313)
     done = 0
     for it in range(40):

@@ -12,7 +12,6 @@
   at small FSEB200_HOST_PACKED_CHUNK_BYTES budgets (many chunks, a block above the budget, short FSE blocks across chunks).
 
 Run as a script (`python tests/test_gpu_frame.py --child`) it repeats the round trips under the environment it was started with."""
-import ctypes as C
 import os
 import subprocess
 import sys
@@ -227,9 +226,7 @@ def compare_with_ref(frame, tmp, what):
         assert got == want, (what, r)
     elif rc == 39:                                                   # the decoder's error: same name
         assert _is_err(r), (what, r, err[-200:])
-        fn = _lib().FSE_getErrorName
-        fn.restype, fn.argtypes = C.c_char_p, [C.c_size_t]
-        name = fn(r).decode()
+        name = _lib().FSE_getErrorName(r).decode()
         assert name in err, (what, name, err[-200:])
     else:
         assert rc in EXIT_VERDICT and r == ERR[EXIT_VERDICT[rc]], (what, rc, r, err[-200:])

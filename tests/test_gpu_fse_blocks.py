@@ -152,10 +152,8 @@ def header_cut_u16(cblock, cs):
 
 def one_block_u16(host, o, n, cap, msv, tl):
     """this library's own one-block FSE_compressU16 (host pointers): (value, bytes)"""
-    import ctypes as C
     import finitestateentropy_b200 as fb
     f = fb.lib().FSE_compressU16
-    f.restype = C.c_size_t; f.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint, C.c_uint]
     src = np.ascontiguousarray(host[o: o + 2 * n])
     buf = np.zeros(cap + 8, np.uint8)
     v = f(ptr(buf), cap, ptr(src), n, msv, tl)

@@ -21,7 +21,7 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
 from helpers import gen_u16, is_error                                             # noqa: E402
-from packed_paths import ref_lib, ref_values                                      # noqa: E402
+from packed_paths import ref_values                                               # noqa: E402
 from test_gpu_blocks import POISON, CANARY, content, _ref, _u64, _dev64           # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -183,7 +183,7 @@ def test_capacities(codec):
 
 
 def test_huf_values_match_the_reference():
-    lib = ref_lib(_ref())
+    lib = _ref()
     for codec in ("huf", "huf1x"):
         data, sizes = blocks(codec, "ragged", seed=821, count=40)
         _, _, cs = host_round_trip(codec, data, sizes)

@@ -14,7 +14,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from helpers import is_error                                                      # noqa: E402
-from packed_paths import ref_lib, ref_values, image, ref_decode                   # noqa: E402
+from packed_paths import ref_values, image, ref_decode                            # noqa: E402
 from test_gpu_blocks import POISON, CANARY, ragged_sources, _ref, _u64, _dev64    # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -77,7 +77,7 @@ def test_packed_compress_round_trip(onex):
     buffer ends 32 bytes after the last block"""
     import torch
     import finitestateentropy_b200 as fb
-    lib = ref_lib(_ref())
+    lib = _ref()
     rng = np.random.default_rng(701)
     host, offs, sizes = ragged_sources(rng, 500)
     w12 = weight12_block()

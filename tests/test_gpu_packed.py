@@ -14,7 +14,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from helpers import is_error                                                      # noqa: E402
-from packed_paths import ERR_DST_TOO_SMALL, ref_lib, ref_values, image, stored_len, ref_decode   # noqa: E402
+from packed_paths import ERR_DST_TOO_SMALL, ref_values, image, stored_len, ref_decode           # noqa: E402
 from test_gpu_blocks import POISON, CANARY, ERR_SRC_WRONG, ragged_sources, _ref, _u64, _dev64   # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -25,7 +25,7 @@ OUT_OFFSETS = [0, 1, 4, 8, 16, 32, 64, 96]
 
 
 def _lib():
-    return ref_lib(_ref())
+    return _ref()
 
 
 def fixture(seed, count, sizes=None):

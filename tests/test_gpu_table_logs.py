@@ -234,21 +234,6 @@ HOST_PARAMS = sorted({(tl, msv) for tl in T.TABLE_LOGS for msv in (0, TOP, 255)}
 FIXTURE = {"huf": (huf_fixture, 1), "huf1x": (huf_fixture, 1), "fse": (fse_fixture, 1), "u16": (u16_fixture, 2)}
 
 
-def _host_sigs(lib, names):
-    sz, vp, u = C.c_size_t, C.c_void_p, C.c_uint
-    for name in names:
-        f = getattr(lib, name)
-        f.restype = sz
-        f.argtypes = [vp, sz, vp, sz, u, u] if "compress" in name and "decompress" not in name else \
-                     ([vp, vp, sz, vp, sz] if name.endswith("DCtx") else [vp, sz, vp, sz])
-    return lib
-
-
-def _ref_lib():
-    ref = load_ref()
-    return _host_sigs(ref, ["HUF_compress1X", "HUF_decompress1X1", "HUF_decompress1X_DCtx"])
-
-
 def expect(codec, ref, data, cap, msv, tl):
     """(value, bytes the block keeps) of the reference for one block: its block call, or the step-by-step oracle where that
     call is not safe (FSE / U16 requests that are raised or whose workspace layout overflows)"""
@@ -306,7 +291,7 @@ def test_uniform_batch_every_parameter(codec):
     import torch
     import finitestateentropy_b200 as fb
     from gpu_common import CANARY, POISON, cpu_decompress
-    ref = _ref_lib()
+    ref = load_ref()
     make, w = FIXTURE[codec]
     blocks = make()
     block = len(blocks[0]) * w
@@ -402,7 +387,7 @@ def test_descriptors_every_parameter(codec):
     import test_gpu_blocks as B4
     import test_gpu_blocks_1x as B1
     import test_gpu_fse_blocks as BF
-    ref = _ref_lib()
+    ref = load_ref()
     make, w = FIXTURE[codec]
     blocks = make()
     rng = np.random.default_rng(77)
@@ -464,9 +449,8 @@ def test_one_block_host_calls(codec):
     every tableLog and every maxSymbolValue, then its HUF_decompress / HUF_decompress1X1 / FSE_decompress / FSE_decompressU16 on
     the result, each against the reference; destinations are poisoned beyond the capacity"""
     import finitestateentropy_b200 as fb
-    ref = _ref_lib()
-    L = _host_sigs(fb.lib(), ["HUF_compress2", "HUF_compress1X", "FSE_compress2", "FSE_compressU16",
-                              "HUF_decompress", "HUF_decompress1X1", "FSE_decompress", "FSE_decompressU16"])
+    ref = load_ref()
+    L = fb.lib()
     enc = {"huf": L.HUF_compress2, "huf1x": L.HUF_compress1X, "fse": L.FSE_compress2, "u16": L.FSE_compressU16}[codec]
     dec = {"huf": L.HUF_decompress, "huf1x": L.HUF_decompress1X1, "fse": L.FSE_decompress, "u16": L.FSE_decompressU16}[codec]
     make, w = FIXTURE[codec]

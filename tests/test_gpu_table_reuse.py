@@ -16,24 +16,14 @@ from helpers import load_ref, ptr, zoo, probagen, is_error
 import finitestateentropy_b200 as fb
 
 pytestmark = pytest.mark.gpu
-S, V, U = C.c_size_t, C.c_void_p, C.c_uint
+U = C.c_uint
 
 
 def _libs():
     ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
-    L = fb.lib()
-    for X in (L, ref):
-        X.HUF_compress4X_repeat.restype = S
-        X.HUF_compress4X_repeat.argtypes = [V, S, V, S, U, U, V, S, V, C.POINTER(C.c_int), C.c_int, C.c_int]
-        X.HUF_compress1X_repeat.restype = S
-        X.HUF_compress1X_repeat.argtypes = [V, S, V, S, U, U, V, S, V, C.POINTER(C.c_int), C.c_int, C.c_int]
-        X.HUF_readCTable.restype = S
-        X.HUF_readCTable.argtypes = [V, C.POINTER(U), V, S, C.POINTER(U)]
-    L.FSEB200_HUF_compress4X_usingCTable_batch.restype = S
-    L.FSEB200_HUF_compress4X_usingCTable_batch.argtypes = [V, S, V, V, S, S, V, V]
-    return L, ref
+    return fb.lib(), ref
 
 
 def _ref_table(ref, data):

@@ -2,7 +2,6 @@
 count, tier-2 workspace and host pipeline used to be process-wide singletons bound to the first device).  With two or more GPUs
 device 1 runs first, so nothing may be bound to device 0; with one GPU the same sequence re-uses that device's cached state.
 The middle pass runs on a side stream, so state kept per (device, stream) is exercised on any number of GPUs."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -19,8 +18,6 @@ def test_both_devices_from_one_process():
     n = torch.cuda.device_count()
     assert n >= 1
     L = fb.lib()
-    L.HUF_compress2.restype = C.c_size_t; L.HUF_compress2.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint, C.c_uint]
-    L.FSE_compress2.restype = C.c_size_t; L.FSE_compress2.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint, C.c_uint]
     data = probagen(64 * BLOCK + 777, 0.14)
     for codec, enc, dec, one in (("huf", fb.huf_compress_batch, fb.huf_decompress_batch, L.HUF_compress2),
                                  ("fse", fb.fse_compress_batch, fb.fse_decompress_batch, L.FSE_compress2)):

@@ -2,27 +2,21 @@
 FSEB200_decompress_host_repeat_packed): the header declares them, the library exports them, and every verdict the host settles
 before any device work -- bad arguments, nBlocks == 0, malformed chain geometry -- is answered without a GPU, writing only what
 the device calls would write."""
-import os
 import re
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import declared_arity
+
 CALLS = {"FSEB200_compress_host_repeat_chains_packed": 18, "FSEB200_decompress_host_repeat_packed": 12}
 ERR_SRC_WRONG = 2 ** 64 - 3
 FILL = 0x7777777777777777
 
 
-def _declarations():
-    text = open(os.path.join(ROOT, "include", "fse_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return {m.group(1): m.group(2).count(",") + 1 for m in re.finditer(r"\b(FSEB200_\w+)\s*\(([^;]*)\)\s*;", text)}
-
-
 def test_header_declares_the_host_chain_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in CALLS} == CALLS
 
 

@@ -1,26 +1,20 @@
 """CPU-side checks of the packed Huff0 decompress and the packed host-buffer calls: the header declares them, the library exports
 them, and the host calls' argument checks -- which answer before any device work -- return srcSize_wrong or 0 without a GPU."""
 import ctypes as C
-import os
 import re
 import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import declared_arity
+
 NEW_CALLS = ("FSEB200_HUF_decompress_packed", "FSEB200_HUF_decompress1X_packed",
              "FSEB200_compress_host_packed", "FSEB200_decompress_host_packed")
 ERR_SRC_WRONG = 2 ** 64 - 3
 
 
-def _declarations():
-    text = open(os.path.join(ROOT, "include", "fse_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return {m.group(1): m.group(2).count(",") + 1 for m in re.finditer(r"\b(FSEB200_\w+)\s*\(([^;]*)\)\s*;", text)}
-
-
 def test_header_declares_the_packed_host_calls():
-    decl = _declarations()
+    decl = declared_arity()
     arity = {"FSEB200_HUF_decompress_packed": 7, "FSEB200_HUF_decompress1X_packed": 7,
              "FSEB200_compress_host_packed": 10, "FSEB200_decompress_host_packed": 7}
     assert {n: decl.get(n) for n in NEW_CALLS} == arity

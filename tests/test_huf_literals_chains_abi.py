@@ -3,7 +3,6 @@ FSEB200_compress_host_literals_chains_packed): declarations and exports, the arg
 compiled reference alone -- the claims the case set rests on: each built chain's policy loop differs from the plain mixed loop
 (flags by the size rule) in the way it claims, and every block the policy loop stores with a value that is not an error decodes
 back to its source with the reference's decoders (but for the weight-12 exception)."""
-import ctypes as C
 import re
 import subprocess
 from collections import Counter
@@ -12,9 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_frame_abi import _declarations
-from helpers import is_error, ptr
-from huf_repeat_cases import ref_lib
+from helpers import is_error, ptr, load_ref, declared_arity
 from huf_chain_cases import chain_header
 from huf_chain_packed_cases import resolve_headers
 from huf_literals_chain_cases import (ref_literals_chain, expected_literals, built_chains, literal_chains, plain_mixed_chain,
@@ -31,14 +28,14 @@ def _lib():
 
 
 def _ref():
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
     return ref
 
 
 def test_header_declares_and_library_exports_the_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in CALLS} == CALLS
     from finitestateentropy_b200 import _build
     exported = subprocess.check_output(["nm", "-D", "--defined-only", _build.build_lib()]).decode()
@@ -104,15 +101,6 @@ def test_built_chains_show_their_rules():
         assert claim_holds(ch["name"], pol, plain_mixed_chain(ref, ch, 255, 11)), ch["name"]
 
 
-def _decoders(ref):
-    ref.HUF_readDTableX1.restype = C.c_size_t
-    ref.HUF_readDTableX1.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    for name in ("HUF_decompress4X1_usingDTable", "HUF_decompress1X1_usingDTable"):
-        f = getattr(ref, name)
-        f.restype = C.c_size_t
-        f.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
-
-
 def _decode(ref, hdr, n, single, payload=None):
     """HUF_readDTableX1 on hdr, then the block's form on payload (by default what follows the header in hdr): (regenerated bytes,
     value), or (None, the header's error) -- the reference's weight-12 exception"""
@@ -135,7 +123,6 @@ def test_the_loops_stream_decodes_on_the_reference(policy):
     kind 3 with the header of the last kind-2 block of its chain or the chain's entry header (HUF_readDTableX1, then the block's
     form); the reference's weight-12 exception aside"""
     ref = _ref()
-    _decoders(ref)
     ml, mgl = policy
     chains = literal_chains(ref, 255, 11)
     want = [ref_literals_chain(ref, ch, 255, 11, ml, mgl) for ch in chains]

@@ -3,7 +3,6 @@ FSEB200_HUF_decompress_mixed_repeat_{blocks,packed}): declarations and exports, 
 Python wrappers' argument checks, and -- on the compiled reference alone -- the claims the calls rest on: a kind-3 block decodes with
 the header its chain resolves to whatever form wrote that header, and the case set reaches every input where the form changes the
 bytes."""
-import ctypes as C
 import re
 import subprocess
 from collections import Counter
@@ -12,9 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-from test_frame_abi import _declarations
-from helpers import is_error, ptr
-from huf_repeat_cases import ref_lib, main_configs
+from helpers import is_error, ptr, load_ref, declared_arity
+from huf_repeat_cases import main_configs
 from huf_chain_cases import chain_header
 from huf_chain_packed_cases import resolve_headers
 from huf_mixed_chain_cases import mixed_chains, ref_mixed_chain, expected_mixed, form_counts, pattern_flags, PATTERNS
@@ -33,14 +31,14 @@ def _lib():
 
 
 def _ref():
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
     return ref
 
 
 def test_header_declares_and_library_exports_the_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in CALLS} == CALLS
     from finitestateentropy_b200 import _build
     exported = subprocess.check_output(["nm", "-D", "--defined-only", _build.build_lib()]).decode()
@@ -164,21 +162,11 @@ def test_flag_patterns():
     assert len(PATTERNS) == 6
 
 
-def _dtable_x1(ref):
-    ref.HUF_readDTableX1.restype = C.c_size_t
-    ref.HUF_readDTableX1.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    for name in ("HUF_decompress4X1_usingDTable", "HUF_decompress1X1_usingDTable"):
-        f = getattr(ref, name)
-        f.restype = C.c_size_t
-        f.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
-
-
 def test_cross_form_headers_decode_on_the_reference():
     """for every kind-3 block of the case set: HUF_readDTableX1 on the header its chain resolves to (the last kind-2 block before
     it, of either form, or the chain's entry header), then HUF_decompress{4X1,1X1}_usingDTable in the block's own form, regenerates
     its source -- on the compiled reference, not on this library.  Also counts the inputs where the form changes the bytes."""
     ref = _ref()
-    _dtable_x1(ref)
     seen, counts = Counter(), Counter()
     for msv, tlog in main_configs():
         chains = mixed_chains(ref, msv, tlog)

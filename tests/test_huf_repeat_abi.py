@@ -11,9 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import ptr, is_error
-from test_frame_abi import _declarations
-from huf_repeat_cases import ref_lib, main_cases, main_configs, U
+from helpers import ptr, is_error, load_ref, declared_arity
+from huf_repeat_cases import main_cases, main_configs, U
 
 CALLS = {"FSEB200_HUF_compress4X_repeat_blocks": 12, "FSEB200_HUF_compress1X_repeat_blocks": 12,
          "FSEB200_HUF_decompress4X_repeat_blocks": 9, "FSEB200_HUF_decompress1X_repeat_blocks": 9}
@@ -26,7 +25,7 @@ def _lib():
 
 
 def test_header_declares_and_library_exports_the_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in CALLS} == CALLS
     from finitestateentropy_b200 import _build
     exported = subprocess.check_output(["nm", "-D", "--defined-only", _build.build_lib()]).decode()
@@ -143,7 +142,7 @@ def trace(ref, four, src, cap, msv, tlog, table, flag, prefer):
 
 
 def test_gpu_inputs_reach_every_outcome_of_the_decision_order():
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
     seen = Counter()

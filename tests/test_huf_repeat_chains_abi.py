@@ -9,11 +9,10 @@ import numpy as np
 import pytest
 import torch
 
-from test_frame_abi import _declarations
 from test_huf_repeat_abi import trace
-from huf_repeat_cases import ref_lib, main_configs, bound
+from huf_repeat_cases import main_configs, bound
 from huf_chain_cases import mid_chains, drift_chains
-from helpers import is_error
+from helpers import is_error, load_ref, declared_arity
 
 CALLS = {"FSEB200_HUF_compress4X_repeat_chains": 18, "FSEB200_HUF_compress1X_repeat_chains": 18}
 SRC_WRONG = (1 << 64) - 3
@@ -25,7 +24,7 @@ def _lib():
 
 
 def test_header_declares_and_library_exports_the_calls():
-    decl = _declarations()
+    decl = declared_arity()
     assert {n: decl.get(n) for n in CALLS} == CALLS
     from finitestateentropy_b200 import _build
     exported = subprocess.check_output(["nm", "-D", "--defined-only", _build.build_lib()]).decode()
@@ -95,7 +94,7 @@ def walk(ref, four, chain, msv, tlog):
 
 
 def test_mid_chain_blocks_reach_every_outcome():
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
     seen = Counter()

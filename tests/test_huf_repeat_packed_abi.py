@@ -10,8 +10,8 @@ import numpy as np
 import pytest
 import torch
 
-from test_frame_abi import _declarations
-from huf_repeat_cases import ref_lib, main_configs
+from helpers import load_ref, declared_arity
+from huf_repeat_cases import main_configs
 from huf_chain_cases import ref_chain
 from huf_chain_packed_cases import packed_chains, expected, resolve_headers
 
@@ -26,7 +26,7 @@ def _lib():
 
 
 def test_header_declares_and_library_exports_the_calls():
-    decl = _declarations()
+    decl = declared_arity()
     calls = dict(COMPRESS, **DECOMPRESS)
     assert {n: decl.get(n) for n in calls} == calls
     from finitestateentropy_b200 import _build
@@ -112,7 +112,7 @@ def test_wrappers_check_dtypes_and_devices():
 def test_kinds_and_chain_starts_name_the_loops_header_for_every_block():
     """the decoder's resolution, restated on the reference loop's kinds, names the header the loop coded every block with; and
     the chains reach every kind, kind 3 as a chain's first block (the entry header) and a raw block after a saved table"""
-    ref = ref_lib()
+    ref = load_ref()
     if ref is None:
         pytest.skip("compiled reference not available")
     seen = Counter()
